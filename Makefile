@@ -1,4 +1,4 @@
-# Builds libparseable_b200.so (CUDA, sm_100a only) in-tree, the C oracle and the
+# Builds libparseable_b200.so (CUDA, sm_90a only) in-tree, the C oracle and the
 # CPU test harness for the pure decode functions.  No PyTorch, no Triton.
 NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
@@ -8,7 +8,7 @@ NCCL_INC  := $(if $(PY_NCCL),-I$(PY_NCCL)/include,)
 # link the torch-bundled libnccl.so.2 when present (same soname as the system one, so a
 # process that also imports torch ends up with a single NCCL)
 NCCL_LIB  := $(if $(PY_NCCL),-L$(PY_NCCL)/lib -l:libnccl.so.2 -Xlinker -rpath -Xlinker $(PY_NCCL)/lib,-lnccl)
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-Wall,-Wno-unused-function --expt-relaxed-constexpr $(NCCL_INC) -Iinclude $(EXTRA)
 CSRC      := parseable_b200/csrc
 OBJDIR    ?= build

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — rows/s of the Parseable query hot path on B200 (BASELINE.json metric).
+"""bench.py — rows/s of the Parseable query hot path on H100 (BASELINE.json metric).
 
 Headline workload (BASELINE.json configs[3], "C4"), weak scaling, one rank per GPU:
     SELECT host, status, COUNT(*), SUM(bytes), MIN(latency_ms), MAX(latency_ms), SUM(duration_s), MAX(cpu)
@@ -20,7 +20,11 @@ c2     = second workload on the same line (BASELINE.json configs[1]): WHERE leve
 --impl reference: the declared CPU stand-in for the reference's DataFusion path (BASELINE.md §3):
          pyarrow/Acero, all host threads, same files, same query, on rank 0's shard.
 
-Launch: python bench.py [--gpus N --steps K --warmup W]; under torchrun one rank per GPU.
+Launch: python bench.py [--gpus N --steps K --warmup W] [--dump-outputs DIR]; under torchrun one rank per GPU.
+--dump-outputs DIR writes what the last timed step of each timed GPU path returned as DIR/<name>.npy (float64, or
+float32 for the key bytes): the C4 table sorted by its keys and the C2 row ids (a fixed, seeded sample when they
+exceed the size cap).  The input files are generated from fixed seeds, so two builds run with the same arguments can
+be compared output for output.
 """
 from __future__ import annotations
 
@@ -87,8 +91,9 @@ def ensure_data(n_row_groups: int, rank: int = 0, world: int = 1, all_workers: b
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons, sampled from before the warm-up to the end of the timed regions
-    (B200_PROFILING.md); the summary only keeps the samples taken inside a timed region."""
+    """nvidia-smi clocks / throttle reasons, sampled from before the warm-up to the end of the timed regions;
+    the summary only keeps the samples taken inside a timed region.  The card's name and power limit are read
+    once: a rate means little without them."""
 
     def __init__(self, gpu_index: int):
         self.rows = []
@@ -97,6 +102,12 @@ class ClockSampler:
         self.windows = []
 
     def start(self):
+        try:
+            out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(self.idx)],
+                                 capture_output=True, text=True, timeout=30).stdout.strip()
+            self.card = dict(zip(("name", "power_limit"), [x.strip() for x in out.split(",")]))
+        except Exception:
+            self.card = {}
         q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
              "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
         try:
@@ -116,7 +127,7 @@ class ClockSampler:
 
     def stop(self) -> dict:
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"], "samples": 0}
+            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"], "samples": 0, "card": self.card}
         time.sleep(0.05)
         self.proc.terminate()
         try:
@@ -130,7 +141,7 @@ class ClockSampler:
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = sorted({names[i] for r in inside if len(r) >= 6 for i in range(4) if r[2 + i] == "Active"})
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
-                "samples": len(sm), "samples_total": len(self.rows)}
+                "samples": len(sm), "samples_total": len(self.rows), "card": self.card}
 
 
 # ------------------------------------------------------------------ queries
@@ -186,6 +197,39 @@ def tables_agree(a, b, what: str):
         else:
             assert x.equals(y), f"{what}: column {name} differs"
     return True
+
+
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, c4, c2_ids):
+    """The last timed step's results as .npy files: the C4 table in canonical order (keys as UTF-8 bytes in a
+    zero-padded float32 matrix, every other column float64) and the C2 row ids (float64; exact below 2**53).  Row ids
+    that would take the total past DUMP_CAP_BYTES are replaced by a sample at fixed, seeded positions, which are
+    written next to them."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    c4 = canon(c4)
+    out = {}
+    keys = [h.encode() for h in c4["host"].to_pylist()]
+    width = max((len(k) for k in keys), default=0)
+    mat = np.zeros((len(keys), width), np.float32)
+    for i, k in enumerate(keys):
+        mat[i, : len(k)] = np.frombuffer(k, np.uint8)
+    out["c4_host_utf8"] = mat
+    for name in C4_NAMES[1:]:
+        out["c4_" + name.replace("(", "_").replace(")", "").replace("*", "star")] = c4[name].to_numpy().astype(np.float64)
+    if c2_ids is not None:
+        room = (DUMP_CAP_BYTES - sum(a.nbytes for a in out.values())) // 8
+        if len(c2_ids) <= room:
+            out["c2_row_ids"] = c2_ids.astype(np.float64)
+        else:
+            pos = np.sort(np.random.default_rng(0).choice(len(c2_ids), room // 2, replace=False))
+            out["c2_row_ids_sample_positions"] = pos.astype(np.float64)
+            out["c2_row_ids"] = c2_ids[pos].astype(np.float64)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    return sorted(out)
 
 
 def plain_schema():
@@ -258,14 +302,11 @@ def run_reference(args, rank: int, world: int):
     pa.set_cpu_count(cores)
     pa.set_io_thread_count(cores)
     vals = []
-    t_start = time.time()
     acero_groupby(shard, nrg)                             # warm: page cache, thread pools
-    while len(vals) < max(1, args.steps):
+    for _ in range(args.steps):
         t = time.time()
         _, rows = acero_groupby(shard, nrg)
         vals.append((rows / (time.time() - t), rows, time.time() - t))
-        if len(vals) >= 5 and time.time() - t_start > 150.0:
-            break
     vs = sorted(v[0] for v in vals)
     v = vs[len(vs) // 2]                                  # median
     ms = 1000.0 * sorted(x[2] for x in vals)[len(vals) // 2]
@@ -318,7 +359,10 @@ def main():
     ap.add_argument("--skip-cpu", action="store_true")
     ap.add_argument("--skip-e2e", action="store_true")
     ap.add_argument("--skip-c2", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's results as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -444,7 +488,8 @@ def main():
     value = rows_per_gpu * world / (dt / args.steps)
     algo_bytes = r.metrics["algorithmic_bytes"]
     d2h_res = r.metrics["d2h_bytes"]
-    assert r.table().num_rows == groups
+    c4_last = r.table()
+    assert c4_last.num_rows == groups
     if rank == 0:
         print(f"[bench] C4 resident step: wall {ms_per_step:.3f} ms = pq_query_open {sum(host_ms) / len(host_ms):.3f} ms (device {sum(dev_ms) / len(dev_ms):.3f} ms, "
               f"scan kernels {sum(scan_ms) / len(scan_ms):.3f} ms, all-reduce {sum(ar_ms) / len(ar_ms):.3f} ms) + binding/Arrow import; table open {open_s:.2f} s",
@@ -466,7 +511,7 @@ def main():
         for _ in range(2):
             re_ = prov_e.aggregate(keys, aggs, tf, flags=ar_flag)
         barrier()
-        k = max(3, min(args.steps, 6))
+        k = args.steps
         t_a = time.perf_counter()
         for _ in range(k):
             re_ = prov_e.aggregate(keys, aggs, tf, flags=ar_flag)
@@ -485,6 +530,7 @@ def main():
 
     # ================= second workload: C2 scan + filter =================
     c2 = None
+    c2_last_ids = None
     if not args.skip_c2:
         flt = c2_filters() + tf
         tbl2 = DeviceTable(files, C2_COLS)
@@ -518,6 +564,7 @@ def main():
         clocks.window(t_a, t_b)
         dt2 = max_over_ranks(t_b - t_a)
         launches += l2
+        c2_last_ids = np.concatenate([b.column(0).to_numpy() for b in r2.batches]) if r2.batches else np.array([], np.int64)
         c2 = {"workload": C2_WORKLOAD, "value": rows_per_gpu * world / (dt2 / args.steps), "unit": "rows/s", "ms_per_step": 1000.0 * dt2 / args.steps,
               "selected_rows_per_gpu": sel, "kernel": "k_flat_filter", "kernel_ms": sum(k_ms2) / len(k_ms2),
               "algorithmic_bytes": r2.metrics["algorithmic_bytes"], "d2h_bytes_per_step": r2.metrics["d2h_bytes"],
@@ -528,7 +575,7 @@ def main():
             for _ in range(2):
                 r2e = prov2e.scan(filters=flt)
             barrier()
-            k = max(3, min(args.steps, 10))
+            k = args.steps
             t_a = time.perf_counter()
             for _ in range(k):
                 r2e = prov2e.scan(filters=flt)
@@ -555,23 +602,16 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_kind = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s (B200_PROFILING.md)"
-    traffic = {}
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        pass
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_kind = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet 3.35 TB/s (not measured)"
 
-    def roof(kernel, kernel_ms, bytes_, traffic_key):
+    def roof(kernel, kernel_ms, bytes_):
         ach = bytes_ / (kernel_ms * 1e-3) / 1e9 if kernel_ms > 0 else 0.0
-        # the ncu capture was taken at the default size: no figure for other table sizes
         return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": traffic.get(traffic_key) if args.row_groups == RGS_PER_GPU else None,
                 "kernel": kernel, "kernel_ms": kernel_ms, "algorithmic_bytes": bytes_, "peak_kind": peak_kind}
 
     if c2 is not None:
-        c2["roofline"] = roof("k_flat_filter", c2["kernel_ms"], c2["algorithmic_bytes"], "k_flat_filter_dram_bytes_per_launch")
+        c2["roofline"] = roof("k_flat_filter", c2["kernel_ms"], c2["algorithmic_bytes"])
     cpu_baseline = None
     if not args.skip_cpu:
         cores = os.cpu_count() or 1
@@ -614,7 +654,7 @@ def main():
                    "groups": groups, "l2": "inputs (encoded chunks read per step) larger than L2; no explicit flush",
                    "parallelism": f"file shards x{world} (file i -> rank i % N), one grouped ncclAllReduce of the partial tables per step" if world > 1
                    else "1 GPU, no collective"},
-        "roofline": roof("k_flat_agg (+k_acc_reduce)", k_ms, algo_bytes, "k_flat_agg_dram_bytes_per_launch"),
+        "roofline": roof("k_flat_agg (+k_acc_reduce)", k_ms, algo_bytes),
         "allreduce_ms": sum(ar_ms) / len(ar_ms), "device_ms_per_step": sum(dev_ms) / len(dev_ms),
         "e2e": e2e, "gpu_launches": launches, "clocks": clk, "cpu_baseline": cpu_baseline,
         "d2h_bytes_per_step_resident": d2h_res, "c2": c2, "numa": numa,
@@ -623,6 +663,8 @@ def main():
     line["step_ms_quantiles"] = {"p10": q[len(q) // 10], "p50": q[len(q) // 2], "p90": q[(len(q) * 9) // 10], "max": q[-1]}
     line["step_ms"] = [round(x, 3) for x in step_ms]      # rank 0's wall time of every timed step, in order
     line["checks"] = checks
+    if args.dump_outputs:
+        line["dumped"] = dump_outputs(args.dump_outputs, c4_last, c2_last_ids)
     print(json.dumps(line), flush=True)
     if world > 1:
         dist.barrier(group=gloo)

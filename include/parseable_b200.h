@@ -1,5 +1,5 @@
 /*
- * parseable_b200.h — C ABI of the B200-native columnar query hot path for Parseable.
+ * parseable_b200.h — C ABI of the H100-native columnar query hot path for Parseable.
  *
  * This is the drop-in boundary of SURVEY.md §8(b).  Each entry point names the
  * reference interface it replaces (paths relative to /root/reference):

@@ -47,7 +47,7 @@ struct PqTable {
 
 extern "C" {
 
-const char* pq_version(void) { return "parseable_b200 0.1.0 (sm_100a)"; }
+const char* pq_version(void) { return "parseable_b200 0.1.0 (sm_90a)"; }
 
 int pq_device_count(void) {
   int n = 0;

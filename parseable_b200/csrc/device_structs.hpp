@@ -1,4 +1,4 @@
-// POD structures shared by the host planner and the sm_100a kernels.
+// POD structures shared by the host planner and the sm_90a kernels.
 // Vocabulary follows the reference's domain: row groups, column chunks, pages,
 // dictionaries (SURVEY.md §8 row a10), not ML terms.
 #pragma once

@@ -1,4 +1,4 @@
-// Host side of the B200 query path: HBM-resident tables of encoded column
+// Host side of the H100 query path: HBM-resident tables of encoded column
 // chunks, query planning (row-group pruning, work items, predicate/aggregate
 // compilation) and the kernel launch sequence.  Mirrors, on the host, what
 // StandardTableProvider::scan + create_parquet_physical_plan do before
@@ -44,6 +44,8 @@ class Context {
   int device() const { return device_; }
   int sm_count() const { return sm_count_; }
   size_t smem_optin() const { return smem_optin_; }
+  size_t smem_per_sm() const { return smem_per_sm_; }
+  size_t l2_bytes() const { return l2_bytes_; }
   // pinned staging buffers, grow-only cache
   uint8_t* pinned_acquire(size_t bytes);
   void pinned_release(uint8_t* p);
@@ -55,6 +57,8 @@ class Context {
   int device_ = 0;
   int sm_count_ = 0;
   size_t smem_optin_ = 0;
+  size_t smem_per_sm_ = 0;
+  size_t l2_bytes_ = 0;
   struct Pinned { uint8_t* p; size_t cap; bool busy; };
   std::vector<Pinned> pinned_;
 };

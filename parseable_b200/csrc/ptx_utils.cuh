@@ -1,4 +1,4 @@
-// sm_100a inline-PTX helpers: mbarrier + TMA 1-D bulk copies (cp.async.bulk,
+// sm_90a inline-PTX helpers: mbarrier + TMA 1-D bulk copies (cp.async.bulk,
 // SASS UBLKCP) used to stage encoded page bytes in shared memory.
 #pragma once
 #include <cstdint>

@@ -63,11 +63,15 @@ void Context::init(const int* devices, int n) {
   PQB_CUDA(cudaSetDevice(dev));
   cudaDeviceProp prop;
   PQB_CUDA(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major < 10) throw Error(PQ_ERR_CUDA, "parseable_b200 needs an sm_100a device (found sm_" +
-                                                     std::to_string(prop.major * 10 + prop.minor) + ")");
+  // the library carries sm_90a code only, which no other compute capability can run
+  if (prop.major != 9 || prop.minor != 0)
+    throw Error(PQ_ERR_CUDA, "parseable_b200 needs an sm_90a (Hopper) device (found sm_" +
+                                 std::to_string(prop.major * 10 + prop.minor) + ")");
   device_ = dev;
   sm_count_ = prop.multiProcessorCount;
   smem_optin_ = prop.sharedMemPerBlockOptin;
+  smem_per_sm_ = prop.sharedMemPerMultiprocessor;
+  l2_bytes_ = size_t(prop.l2CacheSize);
   // keep freed blocks in the stream-ordered pool: query-time cudaMallocAsync stays cheap
   cudaMemPool_t pool;
   PQB_CUDA(cudaDeviceGetDefaultMemPool(&pool, dev));

@@ -34,7 +34,7 @@ def test_exports_match_header(lib):
     assert declared == set(L.EXPORTS)
     for name in declared:
         assert hasattr(lib, name), name
-    assert b"sm_100a" in lib.pq_version()
+    assert b"sm_90a" in lib.pq_version()
 
 
 def test_struct_layouts_match_header(lib, tmp_path):

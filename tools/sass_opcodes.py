@@ -1,4 +1,4 @@
-"""SASS opcode histogram per kernel of the shipped library (cuobjdump -sass) -> profiles/sass_opcodes_r2.txt.
+"""SASS opcode histogram per kernel of the shipped library (cuobjdump -sass) (printed to stdout).
 
     python tools/sass_opcodes.py parseable_b200/libparseable_b200.so > profiles/sass_opcodes_r2.txt
 """
@@ -39,7 +39,7 @@ def main():
         m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_.]+)", line)
         if m and kern:
             ops[kern][m.group(1)] += 1
-    print(f"# SASS opcode histogram of {lib} (cuobjdump -sass, sm_100a cubins only; tools/sass_opcodes.py)")
+    print(f"# SASS opcode histogram of {lib} (cuobjdump -sass, sm_90a cubins only; tools/sass_opcodes.py)")
     print("# UBLKCP = cp.async.bulk (TMA 1-D bulk copy), SYNCS.* = mbarrier ops (ARRIVE.TRANS64, PHASECHK.TRANS64.TRYWAIT), REDUX = warp reduce,")
     print("# ATOMS = shared-memory atomics, RED/REDG/ATOMG/ATOM = global reductions / atomics, LD/ST = generic loads / stores\n")
     for k, c in ops.items():

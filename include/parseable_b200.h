@@ -143,7 +143,13 @@ typedef enum {
   PQ_AGG_SUM = 2,
   PQ_AGG_MIN = 3,
   PQ_AGG_MAX = 4,
-  PQ_AGG_AVG = 5
+  PQ_AGG_AVG = 5,
+  /* COUNT(DISTINCT col) (the alerts' CountDistinct, src/alerts/mod.rs:245-251): Int64, never NULL, named
+   * "count(distinct <col>)".  NULL inputs do not count; a group whose inputs are all NULL gets 0.  Values are
+   * distinct as GROUP BY keys are: strings by bytes, integers / timestamps / booleans by value, Float64 by bit
+   * pattern (-0.0 and 0.0 differ, as do NaNs with different payloads).  Utf8, Int64, Timestamp(ms), Float64 and
+   * Boolean columns; refused (PQ_ERR_UNSUPPORTED) under PQ_QUERY_ALLREDUCE. */
+  PQ_AGG_COUNT_DISTINCT = 6
 } PqAggFn;
 
 typedef struct {

@@ -23,7 +23,7 @@ PQ_T_NULL, PQ_T_BOOL, PQ_T_I64, PQ_T_F64, PQ_T_UTF8, PQ_T_TS_MS = range(6)
 PQ_OP_CMP, PQ_OP_IS_NULL, PQ_OP_IS_NOT_NULL, PQ_OP_LIKE, PQ_OP_AND, PQ_OP_OR, PQ_OP_NOT, PQ_OP_CONST = range(1, 9)
 PQ_EQ, PQ_NE, PQ_LT, PQ_LE, PQ_GT, PQ_GE = range(6)
 PQ_LIKE_NEGATED, PQ_LIKE_CASE_INSENSITIVE = 1, 2
-PQ_AGG_COUNT_STAR, PQ_AGG_COUNT, PQ_AGG_SUM, PQ_AGG_MIN, PQ_AGG_MAX, PQ_AGG_AVG = range(6)
+PQ_AGG_COUNT_STAR, PQ_AGG_COUNT, PQ_AGG_SUM, PQ_AGG_MIN, PQ_AGG_MAX, PQ_AGG_AVG, PQ_AGG_COUNT_DISTINCT = range(7)
 PQ_QUERY_COUNT_ONLY, PQ_QUERY_ALLREDUCE, PQ_QUERY_EMIT_ROW_IDS = 1, 2, 4
 PQ_JSON_LINES = 1
 PQ_COMM_ID_BYTES = 128

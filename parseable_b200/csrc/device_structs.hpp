@@ -135,15 +135,32 @@ struct DevLeaf {
 enum DevPredKind : uint8_t { PK_LEAF = 1, PK_AND = 2, PK_OR = 3, PK_NOT = 4, PK_CONST = 5 };
 struct DevPredOp { uint8_t kind; uint8_t arg; /* leaf id, or const: 0 F, 1 T, 2 NULL */ };
 
-enum DevAggFn : uint8_t { AG_COUNT_STAR = 0, AG_COUNT = 1, AG_SUM = 2, AG_MIN = 3, AG_MAX = 4, AG_AVG = 5 };
+enum DevAggFn : uint8_t { AG_COUNT_STAR = 0, AG_COUNT = 1, AG_SUM = 2, AG_MIN = 3, AG_MAX = 4, AG_AVG = 5, AG_COUNT_DISTINCT = 6 };
 struct DevAgg {
   uint8_t fn;
   uint8_t col;       // column slot
   uint8_t kind;      // DevKind of the input (I64 / F64 / BOOL)
-  uint8_t acc_slot;  // which 8-byte accumulator array
+  uint8_t acc_slot;  // which 8-byte accumulator array (COUNT(DISTINCT): the per-group count of first sightings)
   uint8_t nn_slot;   // which non-null counter array (one per aggregated column)
   uint8_t update_nn; // 1: this aggregate bumps nn[nn_slot] (first aggregate over its column)
-  uint8_t _pad[2];
+  uint8_t dset;      // COUNT(DISTINCT): which presence structure (DevPlan.dist), one per distinct column
+  uint8_t dset_owner;  // COUNT(DISTINCT): 1 = this aggregate feeds the structure; a second one over the same column shares its cell
+};
+
+// COUNT(DISTINCT col): which (group slot, value id) pairs were seen.  Value ids are the GROUP BY ids of the column
+// (ensure_key: 0 .. card-1, NULL excluded).  Dense form: group slot s owns row_words 32-bit words at bits + s * row_words
+// (rows padded to whole words: one word never holds two groups).  Pair form: open addressing on (slot << 32 | id).
+struct DevDistinct {
+  uint8_t col;          // column slot
+  uint8_t kind;         // DevKeyKind: KK_DICT_LUT (ids through gid / FK_IDS pages) or KK_BOOL (the bit is the id)
+  uint8_t hashed;       // 1: pair set, 0: dense bitmap
+  uint8_t _pad;
+  uint32_t card;        // distinct non-NULL values of the column (0: every row NULL)
+  uint32_t row_words;   // dense: words per group slot
+  uint32_t hmask;       // pair set: capacity - 1
+  const uint32_t* gid;  // gid LUT of the column (entry = chunk.lut_base + idx)
+  unsigned int* bits;   // dense bitmap
+  unsigned long long* pairs;   // pair set (~0: empty)
 };
 
 enum DevKeyKind : uint8_t { KK_DICT_LUT = 0, KK_BOOL = 1, KK_BIN = 2 };   // KK_BIN: DATE_BIN of an Int64 / Timestamp column
@@ -202,6 +219,9 @@ struct DevPlan {
   uint32_t f64_global;         // 1: f64 SUM / AVG cells always go to L2 (no native shared-memory f64 atomic)
   uint32_t hashed;             // 1: the key space is wider than the dense table: group cells are found through DevScanArgs.hkeys
   uint32_t hmask;              // hashed: table capacity - 1 (nslots == capacity)
+  uint32_t ndist;              // COUNT(DISTINCT) presence structures (distinct columns)
+  uint32_t _pad_dist;
+  DevDistinct dist[kMaxAggs];
 };
 
 // Accumulator table layout (device, 8-byte cells, struct of arrays over nslots):

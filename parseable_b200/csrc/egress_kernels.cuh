@@ -98,6 +98,7 @@ __global__ void k_agg_finish(const __grid_constant__ FinishArgs f) {
     switch (ag.fn) {
       case AG_COUNT_STAR: v = rows; break;
       case AG_COUNT: v = nn; break;
+      case AG_COUNT_DISTINCT: v = cell; break;   // first sightings of the group's values: 0 when every input was NULL
       case AG_SUM: valid = nn > 0; v = cell; break;
       case AG_AVG:
         valid = nn > 0;

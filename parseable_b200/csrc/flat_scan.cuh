@@ -285,6 +285,26 @@ __device__ __forceinline__ bool col_valid(const ColCtx& c, uint32_t row) {
   return (c.vw[b >> 5] >> (b & 31)) & 1u;
 }
 
+// GROUP BY id of one non-NULL row (the key pass of k_flat_agg and its COUNT(DISTINCT) pass): a boolean's bit, the
+// staged id of a page without a dictionary (FK_IDS), or the gid LUT entry of the row's dictionary index
+// (`gid` already points at the chunk's lut_base)
+__device__ __forceinline__ uint32_t row_id_bool(const ColCtx& c, uint32_t row) {
+  const uint32_t pb = c.phase + row;
+  return (c.colw[pb >> 5] >> (pb & 31)) & 1u;
+}
+__device__ __forceinline__ uint32_t row_id_ids(const ColCtx& c, uint32_t card, uint32_t row) {
+  const uint32_t g = bits32_at(c.colw, c.phase + row * 32u);
+  return g < card ? g : card - 1u;   // never out of the table
+}
+__device__ __forceinline__ uint32_t row_id_lut(const ColCtx& c, const uint32_t* __restrict__ gid, uint32_t row) {
+  return __ldg(gid + col_index(c, row));
+}
+__device__ __forceinline__ uint32_t row_id(const ColCtx& c, bool is_bool, const uint32_t* __restrict__ gid, uint32_t card, uint32_t row) {
+  if (is_bool) return row_id_bool(c, row);
+  if (c.fkind == FK_IDS) return row_id_ids(c, card, row);
+  return row_id_lut(c, gid, row);
+}
+
 // ---- leaves -------------------------------------------------------------------------------------
 // Everything a consumer needs about one leaf for the CURRENT slab; built once per slab (warp uniform)
 // so that the row loops below carry no interpretation: the switch on the page kind sits outside them.
@@ -748,7 +768,66 @@ __device__ __forceinline__ uint32_t agg_hash_slot(unsigned long long* __restrict
   return 0u;
 }
 
-template <int KR, bool HASHED>
+// ---- COUNT(DISTINCT): presence of (group slot, value id) pairs; a first sighting bumps the group's count cell ----
+constexpr unsigned long long kDistinctFull = 101ull;   // counters[1]: the pair set ran full (the host refuses the query)
+__device__ __forceinline__ void count_cell_add(unsigned long long* scell, unsigned long long* gcell, uint32_t cell, uint32_t Hw, uint32_t n) {
+  if (cell < Hw) atomicAdd(reinterpret_cast<uint32_t*>(&scell[cell]), n);   // a CTA sees < 2^32 rows: the low word never wraps
+  else atomicAdd(&gcell[cell], (unsigned long long)n);
+}
+// pair set: true when this call inserted the pair (keys only ever go from EMPTY to one value, as in agg_hash_slot)
+__device__ __forceinline__ bool distinct_pair_insert(unsigned long long* __restrict__ keys, uint32_t mask, uint64_t pair, unsigned long long* counters) {
+  uint32_t h = uint32_t(mix64(pair)) & mask;
+  for (uint32_t probes = 0; probes <= mask; probes++) {
+    const unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(keys + h);
+    if (cur == pair) return false;
+    if (cur == kHashEmpty) {
+      const unsigned long long prev = atomicCAS(keys + h, kHashEmpty, (unsigned long long)pair);
+      if (prev == kHashEmpty) return true;
+      if (prev == pair) return false;
+    }
+    h = (h + 1) & mask;
+  }
+  atomicExch(&counters[1], kDistinctFull);
+  return false;
+}
+// One COUNT(DISTINCT) over the thread's KR rows.  Called by every lane of the warp (the dense form matches lanes).
+// `gs`: the group slot of each row (the hash-table cell under a hashed GROUP BY), `cell`: its count cell.
+template <int KR, bool HASHED, typename slot_t>
+__device__ __forceinline__ void distinct_pass(const DevDistinct& ds, const ColCtx& c, const uint32_t* __restrict__ gid, uint32_t sel,
+                                              const slot_t* gs, const uint32_t* cell, unsigned long long* scell,
+                                              unsigned long long* gcell, uint32_t Hw, unsigned long long* counters) {
+  const uint32_t tc = threadIdx.x, lane = threadIdx.x & 31;
+  const bool is_bool = ds.kind == KK_BOOL;
+#pragma unroll
+  for (int i = 0; i < KR; i++) {
+    const uint32_t r = tc + i * kAggConsumers;
+    const bool on = ((sel >> i) & 1u) && (!c.vw || col_valid(c, r));   // NULL inputs do not count
+    const uint32_t vid = on ? row_id(c, is_bool, gid, ds.card, r) : 0u;
+    if (HASHED || ds.hashed) {
+      if (on && distinct_pair_insert(ds.pairs, ds.hmask, (uint64_t(gs[i]) << 32) | vid, counters)) count_cell_add(scell, gcell, cell[i], Hw, 1u);
+    } else {
+      // dense: test before set (bits only go 0 -> 1: a stale read costs a redundant atomic, never a missed one), then
+      // one atomicOr per distinct word of the warp.  Lanes with nothing to set carry the null address and drop out.
+      unsigned int* w = nullptr;
+      uint32_t bit = 0;
+      if (on) {
+        w = ds.bits + size_t(gs[i]) * ds.row_words + (vid >> 5);
+        bit = 1u << (vid & 31);
+        if (*reinterpret_cast<volatile unsigned int*>(w) & bit) { w = nullptr; bit = 0; }
+      }
+      if (!__any_sync(0xffffffffu, w != nullptr)) continue;   // once the values have been seen, most rows end here
+      const uint32_t peers = __match_any_sync(0xffffffffu, reinterpret_cast<unsigned long long>(w));
+      const uint32_t m = __reduce_or_sync(peers, bit);
+      if (w && lane == uint32_t(__ffs(peers) - 1)) {
+        const uint32_t fresh = __popc(m & ~atomicOr(w, m));   // every lane of the word has the same slot: rows are word-padded
+        if (fresh) count_cell_add(scell, gcell, cell[i], Hw, fresh);
+      }
+    }
+  }
+}
+
+// DIST: the instantiation with the COUNT(DISTINCT) pass (queries without one run code that does not contain it)
+template <int KR, bool HASHED, bool DIST = false>
 __global__ void __launch_bounds__(kAggThreads, 1)
 k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLayout L, const __grid_constant__ DevScanArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -853,8 +932,7 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
             if ((sel >> i) & 1u) {
               const uint32_t r = tc + i * kAggConsumers;
               if (nullable && !col_valid(c, r)) { slot[i] += nullslot; continue; }
-              const uint32_t pb = c.phase + r;
-              slot[i] += ((c.colw[pb >> 5] >> (pb & 31)) & 1u) * stride;
+              slot[i] += row_id_bool(c, r) * stride;
             }
         } else if (key.kind == KK_BIN) {
           // DATE_BIN: the key is computed from the value.  value - bin_base >= 0 and < 2^53 (checked on the host from the
@@ -885,13 +963,12 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
               if ((sel >> i) & 1u) {
                 const uint32_t r = tc + i * kAggConsumers;
                 if (nullable && !col_valid(c, r)) { slot[i] += nullslot; continue; }
-                const uint32_t g = bits32_at(c.colw, c.phase + r * 32u);
-                slot[i] += (g < key.card ? g : key.card - 1u) * stride;   // never out of the table
+                slot[i] += row_id_ids(c, key.card, r) * stride;
               }
           } else if (!nullable) {   // the loads of all rows in flight together
             uint32_t g[KR];
 #pragma unroll
-            for (int i = 0; i < KR; i++) g[i] = ((sel >> i) & 1u) ? __ldg(gid + col_index(c, tc + i * kAggConsumers)) : 0u;
+            for (int i = 0; i < KR; i++) g[i] = ((sel >> i) & 1u) ? row_id_lut(c, gid, tc + i * kAggConsumers) : 0u;
 #pragma unroll
             for (int i = 0; i < KR; i++) slot[i] += g[i] * stride;
           } else {
@@ -900,7 +977,7 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
               if ((sel >> i) & 1u) {
                 const uint32_t r = tc + i * kAggConsumers;
                 if (!col_valid(c, r)) { slot[i] += nullslot; continue; }
-                slot[i] += __ldg(gid + col_index(c, r)) * stride;
+                slot[i] += row_id_lut(c, gid, r) * stride;
               }
           }
         }
@@ -926,6 +1003,19 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
         ColCtx c;
         col_ctx<true>(c, st, base, L, ag.col, a.flat);
         if (c.absent) continue;
+        if constexpr (DIST) {
+          if (ag.fn == AG_COUNT_DISTINCT) {   // a second COUNT(DISTINCT) over the same column shares the first one's cell
+            if (ag.dset_owner) {
+              const DevDistinct& ds = plan.dist[ag.dset];
+              const uint32_t* gid = ds.gid ? ds.gid + st.col[ag.col].lut_base : nullptr;
+              unsigned long long* scell = sacc + size_t(1 + ag.acc_slot) * Hs;
+              unsigned long long* gcell = gadj + size_t(1 + ag.acc_slot) * nslots;
+              if constexpr (HASHED) distinct_pass<KR, HASHED>(ds, c, gid, sel, cell, cell, scell, gcell, Hw, a.counters);   // the hash-table cell is the group
+              else distinct_pass<KR, HASHED>(ds, c, gid, sel, slot, cell, scell, gcell, Hw, a.counters);
+            }
+            continue;
+          }
+        }
         uint32_t vsel = sel;   // selected rows whose input is not NULL
         if (c.vw) {
 #pragma unroll

@@ -53,6 +53,10 @@ struct DevBuf {
 };
 
 constexpr uint64_t kKeepDeviceResult = 1ull << 30;   // result blocks up to this size stay on the device until the query closes
+// COUNT(DISTINCT): the dense presence bitmap of one distinct column may take this much HBM (and at most a quarter of
+// the free HBM); above it the column gets a pair set, of at most kDistinctPairsMax 8-byte entries (2 GiB)
+constexpr uint64_t kDistinctDenseBudget = 1ull << 30;
+constexpr uint64_t kDistinctPairsMax = 1ull << 28;
 
 struct Timer {
   cudaEvent_t a, b;
@@ -852,10 +856,34 @@ void Query::run(const PqQueryDesc& d) {
       ag = DevAgg{};
       ag.fn = uint8_t(d.aggs[a].fn);
       if (ag.fn == AG_COUNT_STAR) { agg_out_type[a] = PQ_T_I64; continue; }
-      if (ag.fn > AG_AVG) throw Error(PQ_ERR_INVALID_ARG, "unknown aggregate function");
+      if (ag.fn > AG_COUNT_DISTINCT) throw Error(PQ_ERR_INVALID_ARG, "unknown aggregate function");
       uint32_t qc = uint32_t(d.aggs[a].col);
       ag.col = uint8_t(slot_of[qc]);
       ag.kind = plan.cols[ag.col].kind;
+      if (ag.fn == AG_COUNT_DISTINCT) {
+        // the count of first sightings is an integer-add cell; COUNT(DISTINCT) twice over one column shares the first
+        // one's presence structure and cell
+        if (ag.kind != DK_I64 && ag.kind != DK_F64 && ag.kind != DK_STR && ag.kind != DK_BOOL)
+          throw Error(PQ_ERR_UNSUPPORTED, std::string("COUNT(DISTINCT) over ") + type_name(out_type_of(qc)) + " is not on the GPU path");
+        agg_out_type[a] = PQ_T_I64;
+        uint32_t first = a;
+        for (uint32_t b = 0; b < a; b++)
+          if (plan.aggs[b].fn == AG_COUNT_DISTINCT && plan.aggs[b].col == ag.col) { first = b; break; }
+        if (first != a) {
+          ag.acc_slot = plan.aggs[first].acc_slot;
+          ag.dset = plan.aggs[first].dset;
+          ag.dset_owner = 0;
+          continue;
+        }
+        ag.acc_slot = uint8_t(n_acc);
+        plan.acc_init[n_acc++] = 0;
+        ag.dset = uint8_t(plan.ndist);
+        ag.dset_owner = 1;
+        plan.dist[plan.ndist] = DevDistinct{};
+        plan.dist[plan.ndist].col = ag.col;
+        plan.ndist++;
+        continue;
+      }
       if (ag.fn != AG_COUNT && ag.kind != DK_I64 && ag.kind != DK_F64)
         throw Error(PQ_ERR_UNSUPPORTED, std::string("SUM/MIN/MAX/AVG over ") + type_name(out_type_of(qc)) + " is not on the GPU path");
       if (ag.fn == AG_COUNT) { agg_out_type[a] = PQ_T_I64; continue; }
@@ -868,6 +896,10 @@ void Query::run(const PqQueryDesc& d) {
       agg_out_type[a] = ag.fn == AG_AVG ? PQ_T_F64 : out_type_of(qc);
     }
     plan.n_acc = n_acc;
+    for (uint32_t a = 0; a < d.n_aggs; a++)
+      if (plan.aggs[a].fn == AG_COUNT_DISTINCT && (d.flags & PQ_QUERY_ALLREDUCE))
+        throw Error(PQ_ERR_UNSUPPORTED, std::string("COUNT(DISTINCT ") + d.columns[d.aggs[a].col].name +
+                                            ") under PQ_QUERY_ALLREDUCE: per-rank distinct counts cannot be summed");
   }
 
   mark("plan compiled");
@@ -939,6 +971,7 @@ void Query::run(const PqQueryDesc& d) {
       DevAgg& ag = plan.aggs[a];
       if (ag.fn == AG_COUNT_STAR) continue;
       ag.update_nn = 0;
+      if (ag.fn == AG_COUNT_DISTINCT) { nn_is_rows[a] = 1; continue; }   // no non-null counter: k_agg_finish reads only its count cell
       if (!col_has_nulls[ag.col]) { nn_is_rows[a] = 1; continue; }
       auto it = nn_of_col.find(int(ag.col));
       if (it == nn_of_col.end()) { it = nn_of_col.emplace(int(ag.col), int(nn_of_col.size())).first; ag.update_nn = 1; }
@@ -1039,7 +1072,7 @@ void Query::run(const PqQueryDesc& d) {
         if (plan.leaves[l].col == key.col && (plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE))
           throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[tcol[d.group_by[k]]].name + "' has pages without a dictionary and is also filtered on: not on the GPU path");
       for (uint32_t a = 0; a < d.n_aggs; a++)
-        if (plan.aggs[a].fn >= AG_SUM && plan.aggs[a].col == key.col)
+        if (plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG && plan.aggs[a].col == key.col)
           throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[tcol[d.group_by[k]]].name + "' has pages without a dictionary and is also aggregated: not on the GPU path");
       row_keys[k] = 1;
     }
@@ -1066,29 +1099,57 @@ void Query::run(const PqQueryDesc& d) {
       qk[k].card = cs.glob_card;
     }
   }
-  // ---- id pages of key columns with pages that have no dictionary: this query's copy of the flat page table, with
-  // those pages pointing into the column's id array (local or agreed numbering) ----
+  // ---- COUNT(DISTINCT) columns: value ids are the column's GROUP BY ids (interned like a key column, NULL excluded) ----
+  std::vector<const uint32_t*> ids_gid(ncols, nullptr);   // column slots whose pages without a dictionary are read as id pages
+  for (uint32_t k = 0; k < d.n_group_by; k++)
+    if (row_keys[k]) ids_gid[plan.keys[k].col] = plan.keys[k].gid;
+  for (uint32_t i = 0; agg_kernel && i < plan.ndist; i++) {
+    DevDistinct& ds = plan.dist[i];
+    const int tc_i = shape_cols[ds.col];
+    const std::string& cname = table->columns[tc_i].name;
+    if (plan.cols[ds.col].kind == DK_BOOL) { ds.kind = KK_BOOL; ds.card = 2; continue; }
+    ds.kind = KK_DICT_LUT;
+    if (table->columns[tc_i].kind == 0xfe) { ds.card = 0; continue; }   // in no file: every row NULL, nothing to count
+    if (plan.cols[ds.col].has_plain || plan.cols[ds.col].has_delta) {
+      // the id pages stand in for the values, as for a key column: nothing else of this query may read them
+      for (uint32_t l = 0; l < nleaves; l++)
+        if (plan.leaves[l].col == ds.col && (plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE))
+          throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + cname + "): the column has pages without a dictionary and is also filtered on: not on the GPU path");
+      for (uint32_t a = 0; a < d.n_aggs; a++)
+        if (plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG && plan.aggs[a].col == ds.col)
+          throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + cname + "): the column has pages without a dictionary and is also aggregated: not on the GPU path");
+      for (uint32_t k = 0; k < d.n_group_by; k++)
+        if (plan.keys[k].kind == KK_BIN && plan.keys[k].col == ds.col)
+          throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + cname + "): the column has pages without a dictionary and is also a DATE_BIN key: not on the GPU path");
+    }
+    table->ensure_key(tc_i, stream);
+    const ColSide& cs = table->sides[tc_i];
+    ds.gid = cs.d_gid;
+    ds.card = cs.card;
+    if (plan.cols[ds.col].has_plain || plan.cols[ds.col].has_delta) ids_gid[ds.col] = ds.gid;
+  }
+  // ---- id pages of key / COUNT(DISTINCT) columns with pages that have no dictionary: this query's copy of the flat
+  // page table, with those pages pointing into the column's id array (local or agreed numbering) ----
   DevBuf<FlatPageRec> d_kpages;
   std::vector<uint32_t> key_bw32(ncols, 0);
   {
     bool any = false;
-    for (uint32_t k = 0; k < d.n_group_by; k++) any = any || row_keys[k];
+    for (uint32_t s = 0; s < ncols; s++) any = any || ids_gid[s];
     if (any) {
       std::vector<FlatPageRec> fp;
       {
         std::lock_guard<std::mutex> lk(table->side_mu);
         fp = table->flat_pages;
-        for (uint32_t k = 0; k < d.n_group_by; k++) {
-          if (!row_keys[k]) continue;
-          const DevKey& key = plan.keys[k];
-          const ColSide& cs = table->sides[shape_cols[key.col]];
-          key_bw32[key.col] = 32;
+        for (uint32_t s = 0; s < ncols; s++) {
+          if (!ids_gid[s]) continue;
+          const ColSide& cs = table->sides[shape_cols[s]];
+          key_bw32[s] = 32;
           for (const ColSide::KeyRowPage& rp : cs.key_row_pages) {
             FlatPageRec& r = fp[rp.page];
             r.fkind = FK_IDS;
             r.bw = 32;
             // relative to d_flat like every flat page (the subtraction may wrap, base + offset does not); 16-byte aligned: ebase is a multiple of 4
-            r.off = uint64_t(key.gid) + 4ull * (uint64_t(cs.n_dict_pad) + rp.ebase) - uint64_t(table->d_flat);
+            r.off = uint64_t(ids_gid[s]) + 4ull * (uint64_t(cs.n_dict_pad) + rp.ebase) - uint64_t(table->d_flat);
           }
         }
       }
@@ -1114,6 +1175,7 @@ void Query::run(const PqQueryDesc& d) {
   // A key space wider than the dense table (2^26 slots): the groups that actually occur are found through a hash
   // table on the wide id (DataFusion's GroupValues hashes the key tuple, SURVEY §8 a12); its capacity is twice the
   // groups that can occur (<= rows scanned, <= combinations), so it never runs full below the 2^27-slot ceiling.
+  const uint64_t key_space = nslots64;   // group-id combinations (the dense table, or the groups a hashed table may meet)
   plan.hashed = 0;
   plan.hmask = 0;
   if (nslots64 > (1ull << 26)) {
@@ -1130,6 +1192,39 @@ void Query::run(const PqQueryDesc& d) {
   }
   plan.nslots = uint32_t(nslots64);
   const uint32_t cells = 1 + plan.n_acc + plan.n_nn;
+  // ---- COUNT(DISTINCT) presence structures: a dense bitmap (row_words words per group slot) while it fits
+  // kDistinctDenseBudget and a quarter of the free HBM; above that, and always under a hashed GROUP BY (whose slots are
+  // hash-table cells), a pair set on (slot << 32 | value id) with room for twice the pairs that can occur ----
+  std::vector<DevBuf<unsigned int>> d_dist_bits(plan.ndist);
+  std::vector<DevBuf<unsigned long long>> d_dist_pairs(plan.ndist);
+  if (plan.ndist) {
+    const char* fh = getenv("PQB_DISTINCT_HASH");   // experiment switch: always the pair set
+    const bool force_hash = fh && fh[0] == '1';
+    size_t free_b = 0, total_b = 0;
+    PQB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const uint64_t budget = std::min<uint64_t>(kDistinctDenseBudget, free_b / 4);
+    uint64_t rows_bound = 0;
+    for (uint32_t g = 0; g < nrg_table; g++) if (rg_live[g]) rows_bound += table->row_groups[g].num_rows;
+    for (uint32_t i = 0; i < plan.ndist; i++) {
+      DevDistinct& ds = plan.dist[i];
+      ds.row_words = std::max<uint32_t>(1, (ds.card + 31) / 32);
+      const uint64_t dense_bytes = uint64_t(plan.nslots) * ds.row_words * 4;
+      ds.hashed = (plan.hashed || force_hash || dense_bytes > budget) ? 1 : 0;
+      if (!ds.hashed) {
+        d_dist_bits[i].alloc(size_t(plan.nslots) * ds.row_words, stream);
+        d_dist_bits[i].zero();
+        ds.bits = d_dist_bits[i].p;
+        continue;
+      }
+      const uint64_t pairs = std::min<uint64_t>(std::max<uint64_t>(rows_bound, 1), key_space * std::max<uint32_t>(ds.card, 1));
+      uint64_t cap = 1024;
+      while (cap < 2 * pairs && cap < kDistinctPairsMax) cap <<= 1;
+      ds.hmask = uint32_t(cap - 1);
+      d_dist_pairs[i].alloc(cap, stream);
+      PQB_CUDA(cudaMemsetAsync(d_dist_pairs[i].p, 0xff, cap * 8, stream));
+      ds.pairs = d_dist_pairs[i].p;
+    }
+  }
 
   // ---- which kernels run ----
   (void)has_null_const;   // the flat kernels evaluate SQL three-valued logic, NULL literals included
@@ -1144,6 +1239,10 @@ void Query::run(const PqQueryDesc& d) {
       throw Error(PQ_ERR_UNSUPPORTED, "DATE_BIN keys need a flat-store copy of every page the query reads: " + shape->why_general);
   if (agg_kernel && plan.hashed && n_general)
     throw Error(PQ_ERR_UNSUPPORTED, "a hashed GROUP BY needs a flat-store copy of every page the query reads: " + shape->why_general);
+  for (uint32_t i = 0; agg_kernel && i < plan.ndist; i++)
+    if (n_general)
+      throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + table->columns[shape_cols[plan.dist[i].col]].name +
+                                          ") needs a flat-store copy of every page the query reads: " + shape->why_general);
   mark("side tables ready");
   // ---- shared-memory layout of k_scan (items the flat kernels do not take) ----
   SmemLayout L{};
@@ -1368,7 +1467,13 @@ void Query::run(const PqQueryDesc& d) {
         PQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(ctx.smem_optin())));
         kern<<<grid, kAggThreads, FL.total, stream>>>(plan, FL, sa);
       };
-      if (plan.hashed) go(k_flat_agg<4, true>);           // key space wider than the dense table: cells through the hash table
+      if (plan.ndist) {   // COUNT(DISTINCT): the instantiations with the presence pass
+        if (plan.hashed) go(k_flat_agg<4, true, true>);
+        else if (plan.flat_krows >= 8) go(k_flat_agg<8, false, true>);
+        else if (plan.flat_krows >= 4) go(k_flat_agg<4, false, true>);
+        else go(k_flat_agg<2, false, true>);
+      }
+      else if (plan.hashed) go(k_flat_agg<4, true>);           // key space wider than the dense table: cells through the hash table
       else if (plan.flat_krows >= 8) go(k_flat_agg<8, false>);   // rows per thread and slab: the widest instantiation the stages leave room for
       else if (plan.flat_krows >= 4) go(k_flat_agg<4, false>);
       else go(k_flat_agg<2, false>);
@@ -1467,14 +1572,16 @@ void Query::run(const PqQueryDesc& d) {
     PQB_CUDA(cudaStreamSynchronize(stream));
     metrics.d2h_bytes += 16 + sizeof(h_counters);
     if (plan.hashed && h_counters[1] == 100) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: more distinct groups than the hashed accumulator table holds (2^26)");
+    if (plan.ndist && h_counters[1] == kDistinctFull) throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT): more distinct (group, value) pairs than the pair set holds (2^27)");
     if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
     const uint32_t n_out = uint32_t(totals[0]);
     metrics.rows_selected = totals[1];
     if (allreduce) { float ms = 0; cudaEventElapsedTime(&ms, t_ar.a, t_ar.b); metrics.allreduce_ms = ms; }
-    static const char* fn_names[] = {"count(*)", "count", "sum", "min", "max", "avg"};
+    static const char* fn_names[] = {"count(*)", "count", "sum", "min", "max", "avg", "count(distinct"};
     auto agg_name = [&](uint32_t a) {
       const DevAgg& ag = plan.aggs[a];
-      return ag.fn == AG_COUNT_STAR ? std::string("count(*)") : std::string(fn_names[ag.fn]) + "(" + d.columns[d.aggs[a].col].name + ")";
+      return ag.fn == AG_COUNT_STAR ? std::string("count(*)")
+                                    : std::string(fn_names[ag.fn]) + (ag.fn == AG_COUNT_DISTINCT ? " " : "(") + d.columns[d.aggs[a].col].name + ")";
     };
     if (d.n_group_by == 0 && n_out == 0) {
       // SQL: a global aggregate over zero rows still yields one row: COUNT = 0, everything else NULL
@@ -1485,7 +1592,7 @@ void Query::run(const PqQueryDesc& d) {
         oc.name = agg_name(a);
         oc.type = agg_out_type[a];
         oc.values.assign(8, 0);
-        const bool is_count = plan.aggs[a].fn == AG_COUNT_STAR || plan.aggs[a].fn == AG_COUNT;
+        const bool is_count = plan.aggs[a].fn == AG_COUNT_STAR || plan.aggs[a].fn == AG_COUNT || plan.aggs[a].fn == AG_COUNT_DISTINCT;
         if (!is_count) { oc.validity.assign(1, 0); oc.null_count = 1; }
         ob.cols.push_back(std::move(oc));
       }

@@ -90,12 +90,21 @@ _FLIP = {L.PQ_LT: L.PQ_GT, L.PQ_GT: L.PQ_LT, L.PQ_LE: L.PQ_GE, L.PQ_GE: L.PQ_LE,
 
 @dataclass
 class Agg:
-    fn: str           # count_star count sum min max avg
+    fn: str           # count_star count sum min max avg count_distinct
     column: str | None = None
+
+    @property
+    def name(self) -> str:
+        """The result column's name (DataFusion's display names, lower case)."""
+        if self.fn == "count_star":
+            return "count(*)"
+        if self.fn == "count_distinct":
+            return f"count(distinct {self.column})"
+        return f"{self.fn}({self.column})"
 
 
 _AGG_CODE = {"count_star": L.PQ_AGG_COUNT_STAR, "count": L.PQ_AGG_COUNT, "sum": L.PQ_AGG_SUM,
-             "min": L.PQ_AGG_MIN, "max": L.PQ_AGG_MAX, "avg": L.PQ_AGG_AVG}
+             "min": L.PQ_AGG_MIN, "max": L.PQ_AGG_MAX, "avg": L.PQ_AGG_AVG, "count_distinct": L.PQ_AGG_COUNT_DISTINCT}
 
 
 @dataclass(frozen=True)
@@ -127,6 +136,7 @@ def sum_(c): return Agg("sum", c)
 def min_(c): return Agg("min", c)
 def max_(c): return Agg("max", c)
 def avg(c): return Agg("avg", c)
+def count_distinct(c): return Agg("count_distinct", c)
 
 
 # ----------------------------------------------------------------------------- descriptor builder
@@ -407,24 +417,13 @@ class StandardTableProvider:
         return self._run(list(filters), list(group_by), list(aggs), [], None, batch_size, flags, json=json)
 
     def count_distinct(self, group_by: Sequence[str], column: str, filters: Iterable[Expr] = ()) -> pa.Table:
-        """``SELECT keys, COUNT(DISTINCT column)`` (Parseable's alerts use it: src/alerts/alert_enums.rs:216-223).
-        The distinct values of a dictionary-encoded column are its interned ids: the GPU runs
-        ``GROUP BY keys, column -> COUNT(*)`` (every row, one pass) and the per-key number of non-NULL ``column`` groups is
-        counted over that small result above the scan.  NULLs do not count, an empty input yields 0 for the global form."""
-        t = self.aggregate(list(group_by) + [column], [count_star()], filters).table()
+        """``SELECT keys, COUNT(DISTINCT column)`` (Parseable's alerts use it: src/alerts/alert_enums.rs:216-223), one
+        native aggregate (PQ_AGG_COUNT_DISTINCT).  NULLs do not count, an empty input yields 0 for the global form."""
         name = f"count(distinct {column})"
-        if not group_by:
-            n = sum(1 for v in t[column].to_pylist() if v is not None) if t.num_rows else 0
-            return pa.table({name: pa.array([n], pa.int64())})
-        if t.num_rows == 0:
-            return pa.table({**{k: t[k] for k in group_by}, name: pa.array([], pa.int64())})
-        seen: dict = {}
-        for row in zip(*[t[k].to_pylist() for k in group_by], t[column].to_pylist()):
-            key, v = row[:-1], row[-1]
-            seen[key] = seen.get(key, 0) + (0 if v is None else 1)
-        cols = {k: pa.array([key[i] for key in seen], t[k].type) for i, k in enumerate(group_by)}
-        cols[name] = pa.array(list(seen.values()), pa.int64())
-        return pa.table(cols)
+        res = self.aggregate(list(group_by), [count_distinct(column)], filters)
+        if res.batches:
+            return res.table()
+        return pa.table({**{k: pa.array([], pa.null()) for k in group_by}, name: pa.array([], pa.int64())})
 
     def _run(self, filters, group_by, aggs, projection, limit, batch_size, flags, poll: bool = False, json: str | None = None) -> QueryResult:
         lib = L.load()
@@ -626,6 +625,8 @@ class Query:
             self._expect("op", "(")
             if t[1] == "COUNT" and self._accept("op", "*"):
                 item = Agg("count_star")
+            elif t[1] == "COUNT" and self._accept("kw", "DISTINCT"):
+                item = Agg("count_distinct", self._next("id")[1])
             else:
                 item = Agg(t[1].lower(), self._next("id")[1])
             self._expect("op", ")")
@@ -707,7 +708,8 @@ class Query:
 
 
 _KEYWORDS = {"SELECT", "FROM", "WHERE", "GROUP", "BY", "AND", "OR", "NOT", "LIKE", "ILIKE", "IS", "NULL", "COUNT",
-             "SUM", "MIN", "MAX", "AVG", "AS", "LIMIT", "TRUE", "FALSE", "ESCAPE"}
+             "SUM", "MIN", "MAX", "AVG", "AS", "LIMIT", "TRUE", "FALSE", "ESCAPE",
+             "DISTINCT"}
 _CMP = {"=": L.PQ_EQ, "!=": L.PQ_NE, "<>": L.PQ_NE, "<": L.PQ_LT, "<=": L.PQ_LE, ">": L.PQ_GT, ">=": L.PQ_GE}
 
 
@@ -741,8 +743,7 @@ def execute(query: Query, provider: StandardTableProvider, is_streaming: bool = 
                 if it[0] == "col":
                     src = it[1]
                 else:
-                    a = it[1]
-                    src = "count(*)" if a.fn == "count_star" else f"{a.fn}({a.column})"
+                    src = it[1].name
                 picked.append(t.column(src))
                 names.append(it[2] or src)
             t = pa.table(picked, names=names)

@@ -37,7 +37,9 @@ oracle: oracle/liboracle.so
 oracle/liboracle.so: oracle/oracle.c
 	$(CC) -O2 -std=c11 -fPIC -shared -Wall -o $@ $< -lm
 
-tools: tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so
+tools: tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so
+tools/liborder_keys_host.so: tools/order_keys_host.cpp $(CSRC)/order_keys.cuh $(CSRC)/decode_core.cuh $(CSRC)/device_structs.hpp
+	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 tools/libjson_host.so: tools/json_host.cpp $(CSRC)/json_egress.cuh $(CSRC)/ryu_f64.cuh $(CSRC)/ryu_tables.inc
 	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -Wno-maybe-uninitialized -I$(CSRC) -o $@ $<
 tools/libzstd_host.so: tools/zstd_host.cpp $(CSRC)/zstd_decode.cuh $(CSRC)/inflate_decode.cuh
@@ -46,6 +48,6 @@ tools/libdecode_core_host.so: tools/decode_core_host.cpp $(CSRC)/decode_core.cuh
 	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 
 clean:
-	rm -rf $(OBJDIR) $(LIB) oracle/liboracle.so tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/libjson_host.so
+	rm -rf $(OBJDIR) $(LIB) oracle/liboracle.so tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so
 
 .PHONY: all oracle tools clean

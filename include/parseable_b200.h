@@ -167,9 +167,36 @@ typedef struct {
   int64_t origin_ms;  /* DATE_BIN: origin, milliseconds since the epoch (the reference passes 1970-01-01) */
 } PqKeyExpr;
 
+/* ---- ORDER BY over aggregate results (the SortExec / TopK DataFusion puts above the AggregateExec) ----
+ * Scope: aggregate queries only (n_aggs > 0), with or without GROUP BY and PQ_QUERY_ALLREDUCE.  n_order_by > 0 on a
+ * filter / projection scan returns PQ_ERR_UNSUPPORTED; an out-of-range index or an unknown target PQ_ERR_INVALID_ARG;
+ * more than 8 terms PQ_ERR_UNSUPPORTED.
+ * LIMIT: with n_order_by > 0, limit >= 0 keeps the first `limit` rows of the ordered result (LIMIT 0: no rows, also for
+ * a global aggregate).  Without ORDER BY an aggregate query ignores `limit`.
+ * Value order (arrow-ord's sort, restated): Int64 / Timestamp(ms) signed; Float64 by IEEE totalOrder (-NaN < -inf <
+ * ... < -0.0 < +0.0 < ... < +inf < +NaN); Utf8 bytewise, a prefix before any longer string; Boolean false < true; a
+ * DATE_BIN key by bin start; an aggregate by its output value (AVG: the Float64 the result holds).  NULL keys and NULL
+ * aggregates (all-NULL groups) go first with PQ_ORDER_NULLS_FIRST and last without it, in either direction.
+ * Ties: rows equal on every term keep the order the same query returns without ORDER BY (ascending group slot), and
+ * at the LIMIT boundary the earlier of them are kept: the result is a stable sort of the unordered result, cut to the
+ * limit, and every rank of an all-reduced query returns the same rows.  Slot order follows the group ids a table
+ * numbers when it is opened (a resident table keeps them); under a hashed GROUP BY (a key space wider than 2^26) the
+ * slots are hash-table cells and their order, so the order of tied rows, may differ from one query to the next.
+ * Paths (all stable on slot order): <= 4096 groups one CTA sorts them; a key that packs into one 64-bit word with
+ * LIMIT <= 4096 takes a radix select of the LIMIT-th key; anything else an LSD radix sort. */
+typedef enum { PQ_ORDER_KEY = 0, PQ_ORDER_AGG = 1 } PqOrderTarget;
+#define PQ_ORDER_DESC 1u
+#define PQ_ORDER_NULLS_FIRST 2u
+typedef struct {
+  int32_t target;  /* PqOrderTarget */
+  int32_t index;   /* into group_by[] (PQ_ORDER_KEY) or aggs[] (PQ_ORDER_AGG) */
+  uint32_t flags;  /* PQ_ORDER_DESC | PQ_ORDER_NULLS_FIRST */
+  int32_t _pad;
+} PqOrderBy;
+
 /* ---- inputs ---- */
 typedef struct {
-  const char* path;   /* file to read, or NULL when buf is given */
+  const char* path;  /* file to read, or NULL when buf is given */
   const uint8_t* buf; /* whole Parquet file image in host memory, or NULL */
   uint64_t size;      /* bytes of buf (ignored for path) */
 } PqFile;
@@ -219,6 +246,11 @@ typedef struct {
   /* NULL, or n_group_by entries: how group_by[k] becomes a key (plain column | DATE_BIN of a Timestamp / Int64 column);
    * a DATE_BIN key comes back as a Timestamp(ms) column named date_bin(<column>) holding the bin start */
   const PqKeyExpr* group_exprs;
+
+  /* ORDER BY terms of an aggregate query, most significant first (see PqOrderBy); n_order_by == 0: none */
+  const PqOrderBy* order_by;
+  uint32_t n_order_by;
+  uint32_t _pad2;
 } PqQueryDesc;
 
 #define PQ_QUERY_COUNT_ONLY 1u    /* filter scan: only rows_selected is wanted, emit no batches */
@@ -241,6 +273,9 @@ typedef struct {
   double host_ms;           /* wall time of pq_query_open (planning + uploads + device work + result copy) */
   double upload_ms;         /* of which: footer parse, page walk and H2D of the column chunks (file-list queries) */
   double allreduce_ms;      /* CUDA-event time of the NCCL all-reduce of the partial tables (PQ_QUERY_ALLREDUCE) */
+  uint64_t groups_total;    /* aggregate queries: groups before the ORDER BY ... LIMIT cut (== groups without ORDER BY) */
+  double order_ms;          /* CUDA-event time of the ORDER BY kernels, without the one host round trip between them
+                               (0 without ORDER BY) */
 } PqMetrics;
 
 /* ---- lifecycle ---- */

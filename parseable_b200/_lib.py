@@ -55,6 +55,14 @@ class PqKeyExpr(C.Structure):
     _fields_ = [("kind", C.c_int32), ("_pad", C.c_int32), ("width_ms", C.c_int64), ("origin_ms", C.c_int64)]
 
 
+PQ_ORDER_KEY, PQ_ORDER_AGG = 0, 1
+PQ_ORDER_DESC, PQ_ORDER_NULLS_FIRST = 1, 2
+
+
+class PqOrderBy(C.Structure):
+    _fields_ = [("target", C.c_int32), ("index", C.c_int32), ("flags", C.c_uint32), ("_pad", C.c_int32)]
+
+
 class PqQueryDesc(C.Structure):
     _fields_ = [
         ("table", C.c_void_p), ("files", C.POINTER(PqFile)), ("n_files", C.c_uint32),
@@ -66,6 +74,7 @@ class PqQueryDesc(C.Structure):
         ("limit", C.c_int64), ("batch_size", C.c_uint32),
         ("shard_index", C.c_uint32), ("shard_count", C.c_uint32), ("flags", C.c_uint32),
         ("group_exprs", C.POINTER(PqKeyExpr)),
+        ("order_by", C.POINTER(PqOrderBy)), ("n_order_by", C.c_uint32), ("_pad2", C.c_uint32),
     ]
 
 
@@ -107,6 +116,7 @@ class PqMetrics(C.Structure):
         ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("kernel_launches", C.c_uint64),
         ("device_ms", C.c_double), ("scan_kernel_ms", C.c_double), ("groups", C.c_uint64),
         ("host_ms", C.c_double), ("upload_ms", C.c_double), ("allreduce_ms", C.c_double),
+        ("groups_total", C.c_uint64), ("order_ms", C.c_double),
     ]
 
     def as_dict(self) -> dict:

@@ -80,6 +80,37 @@ struct FinishArgs {
   FinishKey keys[kMaxKeys];
 };
 
+// The output value of one aggregate of one group slot: the bits of its Int64 / Float64 result, valid == false for NULL.
+// k_agg_finish writes it and k_order_encode sorts by it, so an ORDER BY on an aggregate and its output cannot disagree.
+__device__ __forceinline__ unsigned long long agg_output_value(const unsigned long long* __restrict__ acc, uint32_t nslots, uint32_t n_acc,
+                                                               const DevAgg ag, uint8_t nn_is_rows, uint32_t slot,
+                                                               unsigned long long rows, bool& valid) {
+  unsigned long long nn = 0, cell = 0;
+  if (ag.fn != AG_COUNT_STAR) nn = nn_is_rows ? rows : acc[size_t(1 + n_acc + ag.nn_slot) * nslots + slot];
+  if (ag.fn >= AG_SUM) cell = acc[size_t(1 + ag.acc_slot) * nslots + slot];
+  valid = true;
+  unsigned long long v = 0;
+  switch (ag.fn) {
+    case AG_COUNT_STAR: v = rows; break;
+    case AG_COUNT: v = nn; break;
+    case AG_COUNT_DISTINCT: v = cell; break;   // first sightings of the group's values: 0 when every input was NULL
+    case AG_SUM: valid = nn > 0; v = cell; break;
+    case AG_AVG:
+      valid = nn > 0;
+      if (valid) v = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cell) / double(nn));
+      break;
+    default:
+      valid = nn > 0;
+      v = ag.kind == DK_F64 ? f64_from_order_key((int64_t)cell) : cell;
+  }
+  return v;
+}
+
+// the group id of one GROUP BY key of a group slot (hashed GROUP BY: decoded from the slot's wide id); card: NULL
+__device__ __forceinline__ uint32_t key_gid_of_slot(const unsigned long long* __restrict__ wide, uint32_t slot, uint64_t wstride, uint32_t card) {
+  return uint32_t(((wide ? wide[slot] : uint64_t(slot)) / wstride) % (card + 1));
+}
+
 // one thread per output row: aggregate values + validity, numeric / boolean key values, string key lengths
 __global__ void k_agg_finish(const __grid_constant__ FinishArgs f) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -89,32 +120,15 @@ __global__ void k_agg_finish(const __grid_constant__ FinishArgs f) {
   const uint32_t word = batch * f.words_per_batch + (pos >> 5), bit = 1u << (pos & 31);
   const unsigned long long rows = f.acc[slot];
   for (uint32_t a = 0; a < f.naggs; a++) {
-    const DevAgg ag = f.aggs[a];
-    unsigned long long nn = 0, cell = 0;
-    if (ag.fn != AG_COUNT_STAR) nn = f.nn_is_rows[a] ? rows : f.acc[size_t(1 + f.n_acc + ag.nn_slot) * f.nslots + slot];
-    if (ag.fn >= AG_SUM) cell = f.acc[size_t(1 + ag.acc_slot) * f.nslots + slot];
-    bool valid = true;
-    unsigned long long v = 0;
-    switch (ag.fn) {
-      case AG_COUNT_STAR: v = rows; break;
-      case AG_COUNT: v = nn; break;
-      case AG_COUNT_DISTINCT: v = cell; break;   // first sightings of the group's values: 0 when every input was NULL
-      case AG_SUM: valid = nn > 0; v = cell; break;
-      case AG_AVG:
-        valid = nn > 0;
-        if (valid) v = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cell) / double(nn));
-        break;
-      default:
-        valid = nn > 0;
-        v = ag.kind == DK_F64 ? f64_from_order_key((int64_t)cell) : cell;
-    }
+    bool valid;
+    const unsigned long long v = agg_output_value(f.acc, f.nslots, f.n_acc, f.aggs[a], f.nn_is_rows[a], slot, rows, valid);
     reinterpret_cast<unsigned long long*>(f.out + f.val_off[a])[i] = valid ? v : 0ull;
     if (valid) atomicOr(reinterpret_cast<uint32_t*>(f.out + f.valid_off[a]) + word, bit);
     else atomicAdd(&f.nulls[(f.nkeys + a) * f.nbatches + batch], 1u);
   }
   for (uint32_t k = 0; k < f.nkeys; k++) {
     const FinishKey& key = f.keys[k];
-    const uint32_t gid = uint32_t(((f.wide ? f.wide[slot] : uint64_t(slot)) / key.wstride) % (key.card + 1));
+    const uint32_t gid = key_gid_of_slot(f.wide, slot, key.wstride, key.card);
     const bool valid = gid != key.card;   // NULL is its own group (field_stats.rs:1009-1037)
     if (valid) atomicOr(reinterpret_cast<uint32_t*>(f.out + key.valid_off) + word, bit);
     else atomicAdd(&f.nulls[k * f.nbatches + batch], 1u);

@@ -130,6 +130,7 @@ struct ColSide {
   uint32_t* d_kd_offs = nullptr;       // the same on the device (result assembly)
   uint8_t* d_kd_bytes = nullptr;
   uint32_t kd_max_len = 0;
+  std::shared_ptr<const uint32_t> kd_rank;   // ORDER BY on a Utf8 key: bytewise rank of every group id, on the device (ensure_kd_rank)
   // multi-GPU: the numbering every rank of the communicator agreed on (unify_key), tagged with the communicator's epoch
   bool glob_ready = false;
   uint64_t glob_epoch = 0;
@@ -138,6 +139,7 @@ struct ColSide {
   uint32_t* d_glob_gid = nullptr;
   uint32_t* d_glob_kd_offs = nullptr;
   uint8_t* d_glob_kd_bytes = nullptr;
+  std::shared_ptr<const uint32_t> glob_kd_rank;   // the same ranks over the agreed numbering (dropped by every unify_key)
   uint64_t* d_key_hash = nullptr;
   // GROUP BY on a column with pages that have no dictionary (PLAIN fallback, PLAIN / DELTA numerics): every ROW of those
   // pages is an entry behind the dictionary entries; d_gid / d_glob_gid then hold, per such page, one group id per row --
@@ -213,6 +215,9 @@ class Table {
   void ensure_ent_off(int tcol, cudaStream_t stream) const;
   void ensure_key(int tcol, cudaStream_t stream) const;
   void unify_key(int tcol, cudaStream_t stream) const;        // collective over the pq_comm communicator
+  // bytewise rank per group id of a Utf8 key column, local or agreed numbering (after ensure_key / unify_key)
+  // (shared: a query keeps the ranks it sorts with alive even if unify_key replaces them meanwhile)
+  std::shared_ptr<const uint32_t> ensure_kd_rank(int tcol, bool agreed, cudaStream_t stream) const;
   void ensure_plain8(int tcol, cudaStream_t stream) const;   // DELTA_BINARY_PACKED pages -> row-addressable 8-byte values
 
  private:

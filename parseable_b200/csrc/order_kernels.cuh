@@ -1,0 +1,317 @@
+// ORDER BY [... LIMIT n] over the groups of an aggregate query, on the device.  The result path lists the non-empty
+// group slots in ascending slot order (out_slot, k_slot_compact); ordering permutes and cuts that list before
+// k_agg_finish assembles the rows, so the batches, the Arrow stream and the JSON egress follow the new order unchanged.
+//
+//   k_order_encode   one thread per row: every term's order-preserving u64 (order_keys.cuh) + NULL flag, and the
+//                    value range of every term (one small D2H: the pack plan is sized from it)
+//   k_order_pack     the terms packed MSB-first into the fewest 64-bit words their ranges need
+//   k_order_cta      rows <= kOrderCta: one CTA sorts (word 0, row) pairs in shared memory (bitonic, the row index as the
+//                    last key: stable), then writes the kept slots
+//   k_topk_hist / k_topk_pick / k_topk_tile_eq / k_item_prefix / k_topk_compact, then k_order_cta
+//                    one packed word and LIMIT <= kOrderCta over more rows: radix select of the LIMIT-th key T, MSB
+//                    digit first over the used bits, each digit's histogram over the rows that still match the prefix
+//                    and the digit picked on the device; then the rows below T and, in row order, the first rows equal
+//                    to T (exactly LIMIT candidates) are sorted by the one-CTA sort
+//   k_radix_hist / k_item_prefix / k_radix_scatter
+//                    anything larger: LSD radix sort of the row indices, 8-bit digits over the used bits of each word
+//                    from the least significant word up; per pass tile histograms, one scan of the digit x tile matrix
+//                    and a stable scatter (in-tile ranks from a __match_any_sync multisplit)
+//   k_order_gather   the first `keep` rows' slots in the new order
+// Rows equal on every term keep their slot order (the row index breaks every tie), so the ordered result is a stable
+// sort of the unordered one.
+#pragma once
+#include <cuda_runtime.h>
+
+#include "../../include/parseable_b200.h"
+#include "egress_kernels.cuh"
+#include "order_keys.cuh"
+
+namespace pqb {
+
+enum OrderSource : uint8_t { OS_VALUE = 0, OS_RANK = 1, OS_GID = 2 };   // key terms: 8-byte dictionary value | rank[gid] | gid
+
+struct OrderTerm {
+  uint8_t target;       // PQ_ORDER_KEY / PQ_ORDER_AGG
+  uint8_t enc;          // OrderEnc
+  uint8_t desc;
+  uint8_t source;       // key terms: OrderSource
+  uint8_t nn_is_rows;   // aggregate terms: as FinishArgs.nn_is_rows
+  uint8_t _pad[3];
+  uint32_t card;        // key terms: NULL is gid == card
+  uint64_t wstride;
+  const uint32_t* kd_offs;
+  const uint8_t* kd_bytes;
+  const uint32_t* rank;
+  DevAgg agg;
+};
+struct OrderArgs {
+  const unsigned long long* acc;
+  const unsigned long long* wide;
+  const uint32_t* out_slot;
+  uint32_t n, nslots, n_acc, nterms;
+  unsigned long long* vals;   // [nterms][n] encoded values
+  uint8_t* nulls;             // [nterms][n]
+  OrderRange* ranges;         // [nterms], min = ~0 / max = 0 / flags 0 on entry
+  OrderTerm t[kMaxOrder];
+};
+
+constexpr int kRadixThreads = 256;
+constexpr int kRadixItems = 8;
+constexpr uint32_t kRadixTile = kRadixThreads * kRadixItems;
+
+__global__ void __launch_bounds__(256) k_order_encode(const __grid_constant__ OrderArgs o) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool live = i < o.n;
+  const uint32_t slot = live ? o.out_slot[i] : 0u;
+  const unsigned long long rows = live ? o.acc[slot] : 0ull;
+  for (uint32_t t = 0; t < o.nterms; t++) {
+    const OrderTerm& ot = o.t[t];
+    bool valid = false;
+    unsigned long long bits = 0;
+    if (live) {
+      if (ot.target == PQ_ORDER_AGG) {
+        bits = agg_output_value(o.acc, o.nslots, o.n_acc, ot.agg, ot.nn_is_rows, slot, rows, valid);
+      } else {
+        const uint32_t gid = key_gid_of_slot(o.wide, slot, ot.wstride, ot.card);
+        valid = gid != ot.card;
+        if (valid) {
+          if (ot.source == OS_RANK) bits = ot.rank[gid];
+          else if (ot.source == OS_GID) bits = gid;
+          else {
+            const uint8_t* p = ot.kd_bytes + ot.kd_offs[gid];
+            for (int b = 0; b < 8; b++) bits |= (unsigned long long)p[b] << (8 * b);
+          }
+        }
+      }
+    }
+    const unsigned long long v = order_encode(bits, ot.enc, ot.desc != 0);
+    if (live) {
+      o.vals[size_t(t) * o.n + i] = v;
+      o.nulls[size_t(t) * o.n + i] = valid ? 0 : 1;
+    }
+    unsigned long long mn = (live && valid) ? v : ~0ull, mx = (live && valid) ? v : 0ull;
+    for (int s = 16; s > 0; s >>= 1) {
+      mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, s));
+      mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, s));
+    }
+    const bool any_null = __any_sync(0xffffffffu, live && !valid), any_value = __any_sync(0xffffffffu, live && valid);
+    if ((threadIdx.x & 31) == 0) {
+      if (any_value) {
+        atomicMin(&o.ranges[t].min, mn);
+        atomicMax(&o.ranges[t].max, mx);
+        atomicOr(&o.ranges[t].has_value, 1u);
+      }
+      if (any_null) atomicOr(&o.ranges[t].has_null, 1u);
+    }
+  }
+}
+
+// words[w][n]: the packed key of every row
+__global__ void __launch_bounds__(256) k_order_pack(const __grid_constant__ OrderPack p, const unsigned long long* __restrict__ vals,
+                                                    const uint8_t* __restrict__ nulls, uint32_t n, unsigned long long* __restrict__ words) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint64_t v[kMaxOrder];
+  uint8_t nl[kMaxOrder];
+  for (uint32_t t = 0; t < p.nterms; t++) { v[t] = vals[size_t(t) * n + i]; nl[t] = nulls[size_t(t) * n + i]; }
+  uint64_t w[kMaxOrderWords];
+  for (int k = 0; k < kMaxOrderWords; k++) w[k] = 0;
+  order_pack_row(p, v, nl, w);
+  for (uint32_t k = 0; k < p.nwords; k++) words[size_t(k) * n + i] = w[k];
+}
+
+// row a before row b?  Word 0 is given, the other words are read from the packed keys; padding (row ~0u) goes last.
+__device__ __forceinline__ bool order_row_less(const unsigned long long* __restrict__ words, uint32_t n, uint32_t nwords,
+                                               unsigned long long ka, uint32_t a, unsigned long long kb, uint32_t b) {
+  if (ka != kb) return ka < kb;
+  if (a == ~0u || b == ~0u) return a < b;
+  for (uint32_t w = 1; w < nwords; w++) {
+    const unsigned long long x = words[size_t(w) * n + a], y = words[size_t(w) * n + b];
+    if (x != y) return x < y;
+  }
+  return a < b;
+}
+
+// m <= kOrderCta rows (all n rows, or the top-K candidates cand[0, m)): bitonic sort of (word 0, row) in shared memory
+// by one CTA, then the first `keep` slots
+__global__ void __launch_bounds__(1024) k_order_cta(const unsigned long long* __restrict__ words, uint32_t n, uint32_t nwords,
+                                                    const uint32_t* __restrict__ cand, uint32_t m, uint32_t keep,
+                                                    const uint32_t* __restrict__ out_slot, uint32_t* __restrict__ new_slot) {
+  extern __shared__ __align__(16) unsigned char order_smem[];
+  unsigned long long* key = reinterpret_cast<unsigned long long*>(order_smem);
+  uint32_t* row = reinterpret_cast<uint32_t*>(key + kOrderCta);
+  uint32_t N = 2;
+  while (N < m) N <<= 1;
+  for (uint32_t i = threadIdx.x; i < N; i += blockDim.x) {
+    const uint32_t r = i < m ? (cand ? cand[i] : i) : ~0u;
+    key[i] = i < m ? words[r] : ~0ull;
+    row[i] = r;
+  }
+  __syncthreads();
+  for (uint32_t k = 2; k <= N; k <<= 1) {
+    for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+      for (uint32_t i = threadIdx.x; i < N; i += blockDim.x) {
+        const uint32_t l = i ^ j;
+        if (l <= i) continue;
+        const bool up = (i & k) == 0;
+        const bool l_before_i = order_row_less(words, n, nwords, key[l], row[l], key[i], row[i]);
+        if (l_before_i == up) {
+          const unsigned long long tk = key[i]; key[i] = key[l]; key[l] = tk;
+          const uint32_t tr = row[i]; row[i] = row[l]; row[l] = tr;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  for (uint32_t r = threadIdx.x; r < keep; r += blockDim.x) new_slot[r] = out_slot[row[r]];
+}
+
+// one radix pass: digit counts of every tile of kRadixTile positions, digit-major (hist[d * ntiles + tile])
+__global__ void __launch_bounds__(kRadixThreads) k_radix_hist(const unsigned long long* __restrict__ key, const uint32_t* __restrict__ idx,
+                                                              uint32_t n, uint32_t shift, uint32_t* __restrict__ hist, uint32_t ntiles) {
+  __shared__ uint32_t h[256];
+  h[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t p0 = blockIdx.x * kRadixTile;
+  for (int r = 0; r < kRadixItems; r++) {
+    const uint32_t pos = p0 + r * kRadixThreads + threadIdx.x;
+    if (pos < n) atomicAdd(&h[uint32_t(key[idx ? idx[pos] : pos] >> shift) & 255u], 1u);
+  }
+  __syncthreads();
+  hist[threadIdx.x * ntiles + blockIdx.x] = h[threadIdx.x];
+}
+
+// one radix pass: the rows of a tile go to base[digit, tile] + their rank among the tile's rows with that digit, in
+// position order (stable).  Per round of 256 positions: a warp's lanes with the same digit find each other with
+// __match_any_sync, the per-warp counts are scanned across the 8 warps per digit.
+__global__ void __launch_bounds__(kRadixThreads) k_radix_scatter(const unsigned long long* __restrict__ key, const uint32_t* __restrict__ idx,
+                                                                 uint32_t n, uint32_t shift, const unsigned long long* __restrict__ base,
+                                                                 uint32_t ntiles, uint32_t* __restrict__ idx_out) {
+  constexpr int kWarps = kRadixThreads / 32;
+  __shared__ uint32_t cnt[kWarps][256];
+  __shared__ unsigned long long gbase[256];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  gbase[threadIdx.x] = base[threadIdx.x * ntiles + blockIdx.x];
+  const uint32_t p0 = blockIdx.x * kRadixTile;
+  for (int r = 0; r < kRadixItems; r++) {
+    for (int w = 0; w < kWarps; w++) cnt[w][threadIdx.x] = 0;
+    __syncthreads();
+    const uint32_t pos = p0 + r * kRadixThreads + threadIdx.x;
+    const bool valid = pos < n;
+    const uint32_t row = valid ? (idx ? idx[pos] : pos) : 0u;
+    const uint32_t d = valid ? uint32_t(key[row] >> shift) & 255u : 256u;
+    const uint32_t peers = __match_any_sync(0xffffffffu, d);
+    const uint32_t rank = __popc(peers & ((1u << lane) - 1u));
+    if (valid && rank == 0) cnt[warp][d] = __popc(peers);
+    __syncthreads();
+    uint32_t run = 0;
+    for (int w = 0; w < kWarps; w++) { const uint32_t c = cnt[w][threadIdx.x]; cnt[w][threadIdx.x] = run; run += c; }
+    __syncthreads();
+    if (valid) idx_out[gbase[d] + cnt[warp][d] + rank] = row;
+    __syncthreads();
+    gbase[threadIdx.x] += run;
+  }
+}
+
+// ---- top-K (one packed word, keep <= kOrderCta): radix select of the keep-th smallest key T, MSB digit first, then the
+// candidates = every row below T + the first rows (in row order) equal to T, finished by k_order_cta ----
+struct TopkSel {
+  unsigned long long prefix, mask;   // digits of T found so far
+  uint32_t k;                        // rows still wanted among those matching the prefix (1-based rank of T among them)
+  uint32_t less;                     // rows known to lie strictly below T
+  uint32_t hist[256];
+};
+
+// digit histogram of the rows whose key matches the prefix found so far
+__global__ void __launch_bounds__(256) k_topk_hist(const unsigned long long* __restrict__ key, uint32_t n, uint32_t shift, TopkSel* sel) {
+  __shared__ uint32_t h[256];
+  h[threadIdx.x] = 0;
+  __syncthreads();
+  const unsigned long long prefix = sel->prefix, mask = sel->mask;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const unsigned long long k = key[i];
+    if ((k & mask) == prefix) atomicAdd(&h[uint32_t(k >> shift) & 255u], 1u);
+  }
+  __syncthreads();
+  if (h[threadIdx.x]) atomicAdd(&sel->hist[threadIdx.x], h[threadIdx.x]);
+}
+
+// pick the digit holding the k-th matching row; no host round trip
+__global__ void k_topk_pick(uint32_t shift, TopkSel* sel) {
+  __shared__ uint32_t h[256];
+  h[threadIdx.x] = sel->hist[threadIdx.x];
+  sel->hist[threadIdx.x] = 0;   // ready for the next digit
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t before = 0, d = 0;
+    for (; d < 255; d++) {
+      if (before + h[d] >= sel->k) break;
+      before += h[d];
+    }
+    sel->prefix |= (unsigned long long)d << shift;
+    sel->mask |= 255ull << shift;
+    sel->less += before;
+    sel->k -= before;
+  }
+}
+
+// rows equal to T per tile of kSlotTile rows
+__global__ void __launch_bounds__(256) k_topk_tile_eq(const unsigned long long* __restrict__ key, uint32_t n, const TopkSel* __restrict__ sel,
+                                                      uint32_t* __restrict__ tile_counts) {
+  __shared__ uint32_t ws[8];
+  const unsigned long long T = sel->prefix;
+  const uint32_t s0 = blockIdx.x * kSlotTile;
+  uint32_t c = 0;
+  for (uint32_t i = threadIdx.x; i < (uint32_t)kSlotTile; i += blockDim.x) c += (s0 + i < n && key[s0 + i] == T) ? 1u : 0u;
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t t = 0;
+    for (int w = 0; w < 8; w++) t += ws[w];
+    tile_counts[blockIdx.x] = t;
+  }
+}
+
+// the candidates: every row below T, and the rows equal to T whose rank among them in row order is below sel->k;
+// their order in cand is arbitrary (k_order_cta sorts them by (key, row))
+__global__ void __launch_bounds__(256) k_topk_compact(const unsigned long long* __restrict__ key, uint32_t n, const TopkSel* __restrict__ sel,
+                                                      const unsigned long long* __restrict__ tile_base, uint32_t* __restrict__ cand,
+                                                      uint32_t* __restrict__ count) {
+  __shared__ uint32_t ws[8];
+  const unsigned long long T = sel->prefix;
+  const uint32_t need_eq = sel->k;
+  const uint32_t s0 = blockIdx.x * kSlotTile + threadIdx.x * 4;
+  uint32_t f[4], c = 0;
+#pragma unroll
+  for (int k = 0; k < 4; k++) { f[k] = (s0 + k < n && key[s0 + k] == T) ? 1u : 0u; c += f[k]; }
+  uint32_t incl = c;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+    if ((int)lane >= o) incl += t;
+  }
+  if (lane == 31) ws[warp] = incl;
+  __syncthreads();
+  uint32_t wbase = 0;
+  for (uint32_t w = 0; w < warp; w++) wbase += ws[w];
+  unsigned long long rank = tile_base[blockIdx.x] + wbase + incl - c;   // rank of this thread's first equal row
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    if (s0 + k >= n) break;
+    if (f[k]) {
+      if (rank < need_eq) cand[atomicAdd(count, 1u)] = s0 + k;
+      rank++;
+    } else if (key[s0 + k] < T) {
+      cand[atomicAdd(count, 1u)] = s0 + k;
+    }
+  }
+}
+
+__global__ void k_order_gather(const uint32_t* __restrict__ idx, uint32_t keep, const uint32_t* __restrict__ out_slot,
+                               uint32_t* __restrict__ new_slot) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < keep) new_slot[r] = out_slot[idx[r]];
+}
+
+}  // namespace pqb

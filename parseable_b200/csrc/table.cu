@@ -16,6 +16,7 @@
 
 #include "decomp_kernels.cuh"
 #include "engine.hpp"
+#include "order_keys.cuh"
 
 namespace pqb {
 
@@ -1384,6 +1385,25 @@ void Table::ensure_plain8(int tcol, cudaStream_t stream) const {
 void Table::unify_key(int tcol, cudaStream_t stream) const {
   std::lock_guard<std::mutex> lk(side_mu);
   unify_key_side(*this, tcol, sides[tcol], stream);
+}
+
+// Query-independent prep like the hot-first numbering of ensure_key: the host copy of the key dictionary is sorted once
+// per column (and once per agreement of the ranks); keys interned from pages without a dictionary are in it too.
+std::shared_ptr<const uint32_t> Table::ensure_kd_rank(int tcol, bool agreed, cudaStream_t stream) const {
+  std::lock_guard<std::mutex> lk(side_mu);
+  ColSide& cs = sides[tcol];
+  std::shared_ptr<const uint32_t>& r = agreed ? cs.glob_kd_rank : cs.kd_rank;
+  if (r) return r;
+  const KeyDict& kd = agreed ? cs.glob_kd : cs.kd;
+  const uint32_t card = kd.offs.empty() ? 0u : uint32_t(kd.offs.size() - 1);
+  std::vector<uint32_t> rank(std::max<uint32_t>(card, 1), 0);
+  order_string_ranks(kd.offs.data(), kd.bytes.data(), card, rank.data());
+  uint32_t* d = nullptr;
+  PQB_CUDA(cudaMallocAsync((void**)&d, rank.size() * 4, stream));
+  r = std::shared_ptr<const uint32_t>(d, [](const uint32_t* p) { cudaFree(const_cast<uint32_t*>(p)); });
+  PQB_CUDA(cudaMemcpyAsync(d, rank.data(), rank.size() * 4, cudaMemcpyHostToDevice, stream));
+  PQB_CUDA(cudaStreamSynchronize(stream));
+  return r;
 }
 
 void Table::ensure_key(int tcol, cudaStream_t stream) const {

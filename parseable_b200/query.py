@@ -209,6 +209,29 @@ class _Desc:
             raise QueryError(L.PQ_ERR_UNSUPPORTED, f"expression {e.kind} in a predicate")
 
 
+def _order_term(group_by: list, aggs: list, term) -> tuple[int, int, int]:
+    """One ORDER BY term of ``aggregate`` -> (PqOrderTarget, index, PqOrderBy flags)."""
+    item, direction, *rest = term
+    nulls_first = rest[0] if rest else None
+    if str(direction).lower() not in ("asc", "desc"):
+        raise QueryError(L.PQ_ERR_INVALID_ARG, f"ORDER BY direction {direction!r}: asc or desc")
+    desc = str(direction).lower() == "desc"
+    if nulls_first is None:
+        nulls_first = desc               # DataFusion: ASC -> NULLS LAST, DESC -> NULLS FIRST
+    flags = (L.PQ_ORDER_DESC if desc else 0) | (L.PQ_ORDER_NULLS_FIRST if nulls_first else 0)
+    if isinstance(item, Agg):
+        if item in aggs:
+            return L.PQ_ORDER_AGG, aggs.index(item), flags
+    else:
+        for i, k in enumerate(group_by):
+            if item == k or (isinstance(k, DateBin) and item == k.name):
+                return L.PQ_ORDER_KEY, i, flags
+        for i, a in enumerate(aggs):
+            if item == a.name:
+                return L.PQ_ORDER_AGG, i, flags
+    raise QueryError(L.PQ_ERR_INVALID_ARG, f"ORDER BY {item!r}: neither a GROUP BY key nor an aggregate of the query")
+
+
 _ARROW_TO_PQ = {pa.int64(): L.PQ_T_I64, pa.float64(): L.PQ_T_F64, pa.string(): L.PQ_T_UTF8,
                 pa.large_string(): L.PQ_T_UTF8, pa.bool_(): L.PQ_T_BOOL, pa.timestamp("ms"): L.PQ_T_TS_MS}
 
@@ -293,13 +316,16 @@ def _staging_image(batches: list) -> "HostFile":
 
 def field_stats(provider: "StandardTableProvider", field: str, max_field_statistics: int = 50, filters: Iterable[Expr] = ()):
     """Field statistics of one column like the reference's per-upload job (src/storage/field_stats.rs:298-330):
-    ``GROUP BY field -> COUNT(*)`` runs on the GPU over every row; the window functions of the SQL (SUM / COUNT OVER (),
-    ROW_NUMBER() OVER (ORDER BY value_count DESC)) range over the grouped result and stay above the scan.
+    ``GROUP BY field -> COUNT(*) ORDER BY count(*) DESC LIMIT max_field_statistics`` is one GPU query: the groups are
+    ordered and cut on the device (ties keep the scan's order, as ROW_NUMBER() over a stable sort does), the total is
+    the selected rows and the distinct count the groups before the cut -- what SUM / COUNT OVER () compute.
     Returns (total_count, distinct_count, [(value, count), ...] for the max_field_statistics most frequent values)."""
-    t = provider.aggregate([field], [count_star()], list(filters)).table()
-    vals, cnts = t[field].to_pylist(), t["count(*)"].to_pylist()
-    order = sorted(range(len(vals)), key=lambda i: -cnts[i])          # stable: ties keep the scan's (dictionary) order
-    return sum(cnts), len(vals), [(vals[i], cnts[i]) for i in order[:max_field_statistics]]
+    res = provider.aggregate([field], [count_star()], list(filters), order_by=[(count_star(), "desc")], limit=max_field_statistics)
+    top = []
+    if res.batches:
+        t = res.table()
+        top = list(zip(t[field].to_pylist(), t["count(*)"].to_pylist()))
+    return res.metrics["rows_selected"], res.metrics["groups_total"], top
 
 
 class DeviceTable:
@@ -413,8 +439,16 @@ class StandardTableProvider:
 
     # -- FilterExec + AggregateExec folded into the same call ----------------
     def aggregate(self, group_by: Sequence[str], aggs: Sequence[Agg], filters: Iterable[Expr] = (),
-                  batch_size: int = 0, flags: int = 0, json: str | None = None) -> QueryResult:
-        return self._run(list(filters), list(group_by), list(aggs), [], None, batch_size, flags, json=json)
+                  batch_size: int = 0, flags: int = 0, json: str | None = None, order_by: Sequence | None = None,
+                  limit: int | None = None) -> QueryResult:
+        """``order_by``: ``[(item, "asc" | "desc"[, nulls_first]), ...]``, most significant first, sorted on the GPU
+        (the SortExec / TopK above the AggregateExec).  An item is a GROUP BY key (its name or DateBin), an aggregate
+        (an Agg of ``aggs`` or its output name).  ``nulls_first=None`` follows DataFusion's default (restated, not
+        checked here): ASC puts NULLs last, DESC first.  With ``order_by``, ``limit`` keeps the first rows of the
+        ordered result; without it the C ABI ignores ``limit`` on an aggregate."""
+        group_by, aggs = list(group_by), list(aggs)
+        order = [_order_term(group_by, aggs, t) for t in (order_by or [])]
+        return self._run(list(filters), group_by, aggs, [], limit, batch_size, flags, json=json, order=order)
 
     def count_distinct(self, group_by: Sequence[str], column: str, filters: Iterable[Expr] = ()) -> pa.Table:
         """``SELECT keys, COUNT(DISTINCT column)`` (Parseable's alerts use it: src/alerts/alert_enums.rs:216-223), one
@@ -425,7 +459,8 @@ class StandardTableProvider:
             return res.table()
         return pa.table({**{k: pa.array([], pa.null()) for k in group_by}, name: pa.array([], pa.int64())})
 
-    def _run(self, filters, group_by, aggs, projection, limit, batch_size, flags, poll: bool = False, json: str | None = None) -> QueryResult:
+    def _run(self, filters, group_by, aggs, projection, limit, batch_size, flags, poll: bool = False, json: str | None = None,
+             order: Sequence[tuple] = ()) -> QueryResult:
         lib = L.load()
         d = _Desc()
         ops: list = []
@@ -473,6 +508,11 @@ class StandardTableProvider:
         if proj:
             arr_pj = (C.c_int32 * len(proj))(*proj)
             desc.projection, desc.n_projection = arr_pj, len(proj)
+        if order:
+            arr_ob = (L.PqOrderBy * len(order))()
+            for i, (target, index, fl) in enumerate(order):
+                arr_ob[i].target, arr_ob[i].index, arr_ob[i].flags = target, index, fl
+            desc.order_by, desc.n_order_by = arr_ob, len(order)
         desc.limit = -1 if limit is None else int(limit)
         desc.batch_size = batch_size
         desc.shard_index, desc.shard_count = self.shard_index, self.shard_count
@@ -537,7 +577,7 @@ class TimeRange:
 
 
 class Query:
-    """``SELECT <cols | aggs> FROM <stream> [WHERE ...] [GROUP BY ...] [LIMIT n]`` — the subset of SQL the
+    """``SELECT <cols | aggs> FROM <stream> [WHERE ...] [GROUP BY ...] [ORDER BY ...] [LIMIT n]`` — the subset of SQL the
     GPU path executes.  The reference hands SQL to DataFusion's planner (src/query/mod.rs:261-264);
     that planner is out of scope (SURVEY §2), so this small recursive-descent parser only exists
     to let tests and the bench state their queries the way Parseable users do."""
@@ -589,13 +629,59 @@ class Query:
                 self.group_by.append(self._next("id")[1])
                 if not self._accept("op", ","):
                     break
+        # ORDER BY item [ASC | DESC] [NULLS FIRST | LAST], ...: these words are matched here only, never reserved, so
+        # columns named `order`, `last`, ... keep parsing everywhere else
+        self.order_by: list = []
+        if self._word() == "ORDER" and self._peek(1) == ("kw", "BY"):
+            self._i += 2
+            while True:
+                self.order_by.append(self._order_item())
+                if not self._accept("op", ","):
+                    break
+            if not any(it[0] == "agg" for it in self.select):
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, "ORDER BY on a query without aggregates: row-level sorting is not on the GPU path")
         if self._accept("kw", "LIMIT"):
             self.limit = int(self._next("num")[1])
         if self._i != len(self._t):
             raise QueryError(L.PQ_ERR_UNSUPPORTED, f"unsupported SQL near {self._t[self._i]!r}")
 
-    def _peek(self):
-        return self._t[self._i] if self._i < len(self._t) else (None, None)
+    def _peek(self, k: int = 0):
+        return self._t[self._i + k] if self._i + k < len(self._t) else (None, None)
+
+    def _word(self, k: int = 0):
+        """The upper-cased identifier k tokens ahead (a non-reserved word such as ORDER or NULLS), else None."""
+        t = self._peek(k)
+        return t[1].upper() if t[0] == "id" else None
+
+    def _order_item(self):
+        t = self._peek()
+        if t[0] == "num" and t[1].isdigit():
+            self._i += 1
+            item = ("pos", int(t[1]))                       # 1-based position in the SELECT list
+        elif t[0] == "kw" and t[1] in ("COUNT", "SUM", "MIN", "MAX", "AVG"):
+            item = ("agg", self._agg_call())
+        else:
+            item = ("name", self._next("id")[1])            # a SELECT alias or a GROUP BY column
+        direction = "asc"
+        if self._word() in ("ASC", "DESC"):
+            direction = self._next("id")[1].lower()
+        nulls_first = None
+        if self._word() == "NULLS" and self._word(1) in ("FIRST", "LAST"):
+            self._i += 1
+            nulls_first = self._next("id")[1].upper() == "FIRST"
+        return (item, direction, nulls_first)
+
+    def _agg_call(self) -> Agg:
+        t = self._next("kw")
+        self._expect("op", "(")
+        if t[1] == "COUNT" and self._accept("op", "*"):
+            item = Agg("count_star")
+        elif t[1] == "COUNT" and self._accept("kw", "DISTINCT"):
+            item = Agg("count_distinct", self._next("id")[1])
+        else:
+            item = Agg(t[1].lower(), self._next("id")[1])
+        self._expect("op", ")")
+        return item
 
     def _next(self, kind):
         t = self._peek()
@@ -621,15 +707,7 @@ class Query:
             self._i += 1
             return ("star",)
         if t[0] == "kw" and t[1] in ("COUNT", "SUM", "MIN", "MAX", "AVG"):
-            self._i += 1
-            self._expect("op", "(")
-            if t[1] == "COUNT" and self._accept("op", "*"):
-                item = Agg("count_star")
-            elif t[1] == "COUNT" and self._accept("kw", "DISTINCT"):
-                item = Agg("count_distinct", self._next("id")[1])
-            else:
-                item = Agg(t[1].lower(), self._next("id")[1])
-            self._expect("op", ")")
+            item = self._agg_call()
             alias = self._next("id")[1] if self._accept("kw", "AS") else None
             return ("agg", item, alias)
         name = self._next("id")[1]
@@ -734,8 +812,25 @@ def execute(query: Query, provider: StandardTableProvider, is_streaming: bool = 
         extra = [c for c in cols if c not in query.group_by]
         if extra:
             raise QueryError(L.PQ_ERR_INVALID_ARG, f"column {extra[0]} must appear in GROUP BY")
-        res = provider.aggregate(query.group_by, aggs, filters)
-        # output columns in SELECT order under their aliases; LIMIT applies to the groups
+        # ORDER BY items -> GROUP BY keys / aggregates; an aggregate only ORDER BY names is computed and then dropped
+        order, hidden = [], []
+        for (kind, v), direction, nulls_first in query.order_by:
+            if kind == "pos":
+                if not 1 <= v <= len(query.select):
+                    raise QueryError(L.PQ_ERR_INVALID_ARG, f"ORDER BY {v}: the SELECT list has {len(query.select)} items")
+                target = query.select[v - 1][1]
+            elif kind == "agg":
+                target = v
+                if v not in aggs and v not in hidden:
+                    hidden.append(v)
+            else:
+                alias = [it[1] for it in query.select if it[0] != "star" and it[2] == v]
+                target = alias[0] if alias else v
+            order.append((target, direction, nulls_first))
+        # ORDER BY ... LIMIT runs on the GPU; a grouped LIMIT without ORDER BY keeps n groups in the unordered result
+        res = provider.aggregate(query.group_by, aggs + hidden, filters, order_by=order or None,
+                                 limit=query.limit if order else None)
+        # output columns in SELECT order under their aliases
         if res.batches:
             t = res.table()
             names, picked = [], []
@@ -747,7 +842,7 @@ def execute(query: Query, provider: StandardTableProvider, is_streaming: bool = 
                 picked.append(t.column(src))
                 names.append(it[2] or src)
             t = pa.table(picked, names=names)
-            if query.limit is not None:
+            if query.limit is not None and not order:
                 t = t.slice(0, query.limit)
             res.batches = t.to_batches(max_chunksize=20000) or res.batches[:1]
             res.fields = names

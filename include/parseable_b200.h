@@ -167,29 +167,40 @@ typedef struct {
   int64_t origin_ms;  /* DATE_BIN: origin, milliseconds since the epoch (the reference passes 1970-01-01) */
 } PqKeyExpr;
 
-/* ---- ORDER BY over aggregate results (the SortExec / TopK DataFusion puts above the AggregateExec) ----
- * Scope: aggregate queries only (n_aggs > 0), with or without GROUP BY and PQ_QUERY_ALLREDUCE.  n_order_by > 0 on a
- * filter / projection scan returns PQ_ERR_UNSUPPORTED; an out-of-range index or an unknown target PQ_ERR_INVALID_ARG;
- * more than 8 terms PQ_ERR_UNSUPPORTED.
- * LIMIT: with n_order_by > 0, limit >= 0 keeps the first `limit` rows of the ordered result (LIMIT 0: no rows, also for
- * a global aggregate).  Without ORDER BY an aggregate query ignores `limit`.
+/* ---- ORDER BY on the device: over aggregate results (the SortExec / TopK DataFusion puts above the AggregateExec), and
+ *      ORDER BY ... LIMIT over the selected rows of a filter / projection scan (SortExec(fetch) above the scan) ----
+ * Aggregate queries (n_aggs > 0, with or without GROUP BY and PQ_QUERY_ALLREDUCE) order by PQ_ORDER_KEY and
+ * PQ_ORDER_AGG terms; a PQ_ORDER_COLUMN term there returns PQ_ERR_INVALID_ARG.  With ORDER BY, limit >= 0 keeps the
+ * first `limit` rows of the ordered result (LIMIT 0: no rows, also for a global aggregate).  Without ORDER BY an
+ * aggregate query ignores `limit`.
+ * Scans (n_aggs == 0, with or without a projection) order by PQ_ORDER_COLUMN terms, whose column need not be projected,
+ * and need a LIMIT: limit < 0 returns PQ_ERR_UNSUPPORTED.  The result is the first `limit` rows of the ordered
+ * selection (LIMIT 0: no rows); the __row_id column of PQ_QUERY_EMIT_ROW_IDS follows the order, and without a
+ * projection the result is the selected __row_ids in order.  rows_selected counts the rows before the cut.  Under
+ * row-group or file sharding every shard orders and cuts its own selection; merging the shards' rows is the caller's.
+ * A PQ_ORDER_KEY / PQ_ORDER_AGG term on a scan returns PQ_ERR_UNSUPPORTED; ORDER BY with PQ_QUERY_COUNT_ONLY
+ * PQ_ERR_INVALID_ARG; more than 2^32 - 1 selected rows, or pages without a flat-store copy, PQ_ERR_UNSUPPORTED.
+ * Every query: an out-of-range index or an unknown target returns PQ_ERR_INVALID_ARG, more than 8 terms
+ * PQ_ERR_UNSUPPORTED.
  * Value order (arrow-ord's sort, restated): Int64 / Timestamp(ms) signed; Float64 by IEEE totalOrder (-NaN < -inf <
  * ... < -0.0 < +0.0 < ... < +inf < +NaN); Utf8 bytewise, a prefix before any longer string; Boolean false < true; a
- * DATE_BIN key by bin start; an aggregate by its output value (AVG: the Float64 the result holds).  NULL keys and NULL
- * aggregates (all-NULL groups) go first with PQ_ORDER_NULLS_FIRST and last without it, in either direction.
- * Ties: rows equal on every term keep the order the same query returns without ORDER BY (ascending group slot), and
- * at the LIMIT boundary the earlier of them are kept: the result is a stable sort of the unordered result, cut to the
- * limit, and every rank of an all-reduced query returns the same rows.  Slot order follows the group ids a table
- * numbers when it is opened (a resident table keeps them); under a hashed GROUP BY (a key space wider than 2^26) the
- * slots are hash-table cells and their order, so the order of tied rows, may differ from one query to the next.
- * Paths (all stable on slot order): <= 4096 groups one CTA sorts them; a key that packs into one 64-bit word with
+ * DATE_BIN key by bin start; an aggregate by its output value (AVG: the Float64 the result holds).  NULLs (NULL keys,
+ * NULL aggregates of all-NULL groups, NULL column values, a column missing from a file) go first with
+ * PQ_ORDER_NULLS_FIRST and last without it, in either direction.
+ * Ties: rows equal on every term keep the order the same query returns without ORDER BY, and at the LIMIT boundary the
+ * earlier of them are kept: the result is a stable sort of the unordered result, cut to the limit.  For a scan that
+ * order is file order, then row order.  For an aggregate it is ascending group slot, and every rank of an all-reduced
+ * query returns the same rows.  Slot order follows the group ids a table numbers when it is opened (a resident table
+ * keeps them); under a hashed GROUP BY (a key space wider than 2^26) the slots are hash-table cells and their order, so
+ * the order of tied rows, may differ from one query to the next.
+ * Paths (all stable on that order): <= 4096 rows one CTA sorts them; a key that packs into one 64-bit word with
  * LIMIT <= 4096 takes a radix select of the LIMIT-th key; anything else an LSD radix sort. */
-typedef enum { PQ_ORDER_KEY = 0, PQ_ORDER_AGG = 1 } PqOrderTarget;
+typedef enum { PQ_ORDER_KEY = 0, PQ_ORDER_AGG = 1, PQ_ORDER_COLUMN = 2 } PqOrderTarget;
 #define PQ_ORDER_DESC 1u
 #define PQ_ORDER_NULLS_FIRST 2u
 typedef struct {
   int32_t target;  /* PqOrderTarget */
-  int32_t index;   /* into group_by[] (PQ_ORDER_KEY) or aggs[] (PQ_ORDER_AGG) */
+  int32_t index;   /* into group_by[] (PQ_ORDER_KEY), aggs[] (PQ_ORDER_AGG) or columns[] (PQ_ORDER_COLUMN) */
   uint32_t flags;  /* PQ_ORDER_DESC | PQ_ORDER_NULLS_FIRST */
   int32_t _pad;
 } PqOrderBy;
@@ -247,7 +258,7 @@ typedef struct {
    * a DATE_BIN key comes back as a Timestamp(ms) column named date_bin(<column>) holding the bin start */
   const PqKeyExpr* group_exprs;
 
-  /* ORDER BY terms of an aggregate query, most significant first (see PqOrderBy); n_order_by == 0: none */
+  /* ORDER BY terms, most significant first (see PqOrderBy); n_order_by == 0: none */
   const PqOrderBy* order_by;
   uint32_t n_order_by;
   uint32_t _pad2;
@@ -260,7 +271,7 @@ typedef struct {
 typedef struct {
   uint64_t bytes_scanned;   /* compressed bytes of the column chunks read (plan metric "bytes_scanned") */
   uint64_t rows_scanned;    /* rows in the row groups that survived pruning */
-  uint64_t rows_selected;   /* rows passing the predicate */
+  uint64_t rows_selected;   /* rows passing the predicate (before an ORDER BY ... LIMIT cut) */
   uint64_t row_groups_total;
   uint64_t row_groups_pruned;
   uint64_t algorithmic_bytes; /* uncompressed encoded bytes of the pages read + bitmap bytes written */

@@ -55,7 +55,7 @@ class PqKeyExpr(C.Structure):
     _fields_ = [("kind", C.c_int32), ("_pad", C.c_int32), ("width_ms", C.c_int64), ("origin_ms", C.c_int64)]
 
 
-PQ_ORDER_KEY, PQ_ORDER_AGG = 0, 1
+PQ_ORDER_KEY, PQ_ORDER_AGG, PQ_ORDER_COLUMN = 0, 1, 2
 PQ_ORDER_DESC, PQ_ORDER_NULLS_FIRST = 1, 2
 
 

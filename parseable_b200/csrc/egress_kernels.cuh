@@ -235,20 +235,25 @@ __device__ __forceinline__ uint32_t flat_bits_at(const uint8_t* flat, uint64_t o
   return bw >= 32 ? v : (v & ((1u << bw) - 1u));
 }
 
-// one CTA per work item (grid-strided): bitmap words -> output positions -> values of every projected column
-__global__ void __launch_bounds__(256) k_project(const __grid_constant__ ProjArgs f) {
+// Every selected row of the work items this CTA takes (one CTA per item, grid-strided; <= 256 threads), in scan order:
+// fn(item, item index, row inside the item, position in the selection = item_base + the in-item prefix).  Every thread
+// of the CTA returns from it.
+template <class Fn>
+__device__ __forceinline__ void for_each_selected(const DevItem* __restrict__ items, const uint32_t* __restrict__ bitmap,
+                                                  const uint32_t* __restrict__ item_counts, const unsigned long long* __restrict__ item_base,
+                                                  uint32_t n_items, Fn&& fn) {
   __shared__ uint32_t warp_sums[8];
   __shared__ uint32_t carry;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-  for (uint32_t it = blockIdx.x; it < f.n_items; it += gridDim.x) {
-    if (f.item_counts[it] == 0) continue;   // uniform per block
-    const DevItem& item = f.items[it];
+  for (uint32_t it = blockIdx.x; it < n_items; it += gridDim.x) {
+    if (item_counts[it] == 0) continue;   // uniform per block
+    const DevItem& item = items[it];
     const uint32_t nwords = (item.nrows + 31) >> 5;
     if (threadIdx.x == 0) carry = 0;
     __syncthreads();
     for (uint32_t w0 = 0; w0 < nwords; w0 += blockDim.x) {
       const uint32_t w = w0 + threadIdx.x;
-      uint32_t word = w < nwords ? f.bitmap[item.bitmap_word0 + w] : 0;
+      uint32_t word = w < nwords ? bitmap[item.bitmap_word0 + w] : 0;
       const uint32_t c = __popc(word);
       uint32_t incl = c;
       for (int o = 1; o < 32; o <<= 1) {
@@ -266,54 +271,11 @@ __global__ void __launch_bounds__(256) k_project(const __grid_constant__ ProjArg
         if (lane < nwarps) warp_sums[lane] = si - s;
       }
       __syncthreads();
-      unsigned long long pos = f.item_base[it] + carry + warp_sums[warp] + incl - c;
+      unsigned long long pos = item_base[it] + carry + warp_sums[warp] + incl - c;
       while (word) {
         const uint32_t b = __ffs(word) - 1;
         word &= word - 1;
-        if (pos < f.n_out) {
-          const uint32_t r = w * 32 + b;   // row inside the item
-          const uint32_t batch = uint32_t(pos / f.batch_rows), bp = uint32_t(pos - uint64_t(batch) * f.batch_rows);
-          const uint32_t vword = batch * f.words_per_batch + (bp >> 5), vbit = 1u << (bp & 31);
-          for (uint32_t ci = 0; ci < f.ncols; ci++) {
-            const ProjCol& pc = f.cols[ci];
-            if (pc.slot == 0xffffffffu) {   // __row_id: ordinal of the row in the scanned table
-              reinterpret_cast<unsigned long long*>(f.out + pc.val_off)[pos] = item.global_row0 + r;
-              continue;
-            }
-            if ((item.absent >> pc.slot) & 1u) {   // column missing from this file: NULL
-              atomicAdd(&f.nulls[ci * f.nbatches + batch], 1u);
-              continue;
-            }
-            const FlatPageRec fp = f.fpages[item.page[pc.slot]];
-            const uint64_t row = uint64_t(item.poff[pc.slot]) + r;
-            if (fp.voff != ~0ull && !((reinterpret_cast<const uint32_t*>(f.flat + fp.voff)[row >> 5] >> (row & 31)) & 1u)) {
-              atomicAdd(&f.nulls[ci * f.nbatches + batch], 1u);   // NULL row: value slot stays 0, string length 0
-              continue;
-            }
-            atomicOr(reinterpret_cast<uint32_t*>(f.out + pc.valid_off) + vword, vbit);
-            if (fp.fkind == FK_BYTES) {   // PLAIN byte array: the row's bytes inside the page
-              const uint64_t e = fp.base + reinterpret_cast<const uint32_t*>(f.flat + fp.off)[row];
-              reinterpret_cast<unsigned long long*>(f.out + pc.src_off)[pos] = e;
-              reinterpret_cast<uint32_t*>(f.out + pc.len_off)[pos] = load_u32_unaligned(f.arena + e - 4);
-            } else if (fp.fkind == FK_PLAIN8) {
-              reinterpret_cast<unsigned long long*>(f.out + pc.val_off)[pos] = reinterpret_cast<const unsigned long long*>(f.flat + fp.off)[row];
-            } else if (fp.fkind == FK_BITS) {
-              const uint32_t v = (reinterpret_cast<const uint32_t*>(f.flat + fp.off)[row >> 5] >> (row & 31)) & 1u;
-              if (v) atomicOr(reinterpret_cast<uint32_t*>(f.out + pc.val_off) + vword, vbit);
-            } else {
-              const DevChunk& ch = f.chunks[item.rg * f.plan_ncols + pc.slot];
-              uint32_t idx = flat_bits_at(f.flat, fp.off, row * fp.bw, fp.bw);
-              idx = idx < ch.dict_n ? idx : (ch.dict_n ? ch.dict_n - 1 : 0);
-              if (pc.kind == DK_STR) {
-                const uint64_t e = pc.ent[ch.lut_base + idx];
-                reinterpret_cast<unsigned long long*>(f.out + pc.src_off)[pos] = e;
-                reinterpret_cast<uint32_t*>(f.out + pc.len_off)[pos] = load_u32_unaligned(f.arena + e - 4);
-              } else {
-                reinterpret_cast<unsigned long long*>(f.out + pc.val_off)[pos] = reinterpret_cast<const unsigned long long*>(f.flat + ch.dict8_off)[idx];
-              }
-            }
-          }
-        }
+        fn(item, it, w * 32 + b, pos);
         pos++;
       }
       __syncthreads();
@@ -321,6 +283,94 @@ __global__ void __launch_bounds__(256) k_project(const __grid_constant__ ProjArg
       __syncthreads();
     }
   }
+}
+
+// The value of row r of a work item in one column slot, straight out of the flat store (row r of a page is bits
+// [r*bw, (r+1)*bw) / 8-byte slot r); false for NULL (a NULL row, or the column is missing from the file).  v is the
+// 8-byte value (Int64 / Timestamp / Float64 bits, a numeric dictionary through the chunk's aligned copy) or 0 / 1
+// (Boolean).  Utf8: the arena offset of the value's bytes, their length in len; with IDS instead the value's id in the
+// column's GROUP BY numbering (ensure_key): gid[entry] of a dictionary entry, or the u32 of an FK_IDS page.
+template <bool IDS>
+__device__ __forceinline__ bool flat_value_at(const uint8_t* __restrict__ arena, const uint8_t* __restrict__ flat,
+                                              const FlatPageRec* __restrict__ fpages, const DevChunk* __restrict__ chunks,
+                                              uint32_t plan_ncols, const DevItem& item, uint32_t slot, uint32_t kind,
+                                              const uint64_t* __restrict__ ent, const uint32_t* __restrict__ gid, uint32_t r,
+                                              unsigned long long& v, uint32_t& len) {
+  if ((item.absent >> slot) & 1u) return false;
+  const FlatPageRec fp = fpages[item.page[slot]];
+  const uint64_t row = uint64_t(item.poff[slot]) + r;
+  if (fp.voff != ~0ull && !((reinterpret_cast<const uint32_t*>(flat + fp.voff)[row >> 5] >> (row & 31)) & 1u)) return false;
+  if (IDS && fp.fkind == FK_IDS) {
+    v = reinterpret_cast<const uint32_t*>(flat + fp.off)[row];
+  } else if (fp.fkind == FK_BYTES) {   // PLAIN byte array: the row's bytes inside the page
+    const uint64_t e = fp.base + reinterpret_cast<const uint32_t*>(flat + fp.off)[row];
+    v = e;
+    len = load_u32_unaligned(arena + e - 4);
+  } else if (fp.fkind == FK_PLAIN8) {
+    v = reinterpret_cast<const unsigned long long*>(flat + fp.off)[row];
+  } else if (fp.fkind == FK_BITS) {
+    v = (reinterpret_cast<const uint32_t*>(flat + fp.off)[row >> 5] >> (row & 31)) & 1u;
+  } else {
+    const DevChunk& ch = chunks[item.rg * plan_ncols + slot];
+    uint32_t idx = flat_bits_at(flat, fp.off, row * fp.bw, fp.bw);
+    idx = idx < ch.dict_n ? idx : (ch.dict_n ? ch.dict_n - 1 : 0);
+    if (kind == DK_STR && IDS) {
+      v = gid[ch.lut_base + idx];
+    } else if (kind == DK_STR) {
+      const uint64_t e = ent[ch.lut_base + idx];
+      v = e;
+      len = load_u32_unaligned(arena + e - 4);
+    } else {
+      v = reinterpret_cast<const unsigned long long*>(flat + ch.dict8_off)[idx];
+    }
+  }
+  return true;
+}
+
+// every projected column of one selected row (row r of `item`) at output position pos < n_out
+__device__ __forceinline__ void project_row(const ProjArgs& f, const DevItem& item, uint32_t r, unsigned long long pos) {
+  const uint32_t batch = uint32_t(pos / f.batch_rows), bp = uint32_t(pos - uint64_t(batch) * f.batch_rows);
+  const uint32_t vword = batch * f.words_per_batch + (bp >> 5), vbit = 1u << (bp & 31);
+  for (uint32_t ci = 0; ci < f.ncols; ci++) {
+    const ProjCol& pc = f.cols[ci];
+    if (pc.slot == 0xffffffffu) {   // __row_id: ordinal of the row in the scanned table
+      reinterpret_cast<unsigned long long*>(f.out + pc.val_off)[pos] = item.global_row0 + r;
+      continue;
+    }
+    unsigned long long v = 0;
+    uint32_t len = 0;
+    if (!flat_value_at<false>(f.arena, f.flat, f.fpages, f.chunks, f.plan_ncols, item, pc.slot, pc.kind, pc.ent, nullptr, r, v, len)) {
+      atomicAdd(&f.nulls[ci * f.nbatches + batch], 1u);   // NULL: value slot stays 0, string length 0
+      continue;
+    }
+    atomicOr(reinterpret_cast<uint32_t*>(f.out + pc.valid_off) + vword, vbit);
+    if (pc.kind == DK_STR) {
+      reinterpret_cast<unsigned long long*>(f.out + pc.src_off)[pos] = v;
+      reinterpret_cast<uint32_t*>(f.out + pc.len_off)[pos] = len;
+    } else if (pc.kind == DK_BOOL) {
+      if (v) atomicOr(reinterpret_cast<uint32_t*>(f.out + pc.val_off) + vword, vbit);
+    } else {
+      reinterpret_cast<unsigned long long*>(f.out + pc.val_off)[pos] = v;
+    }
+  }
+}
+
+// one CTA per work item (grid-strided): bitmap words -> output positions -> values of every projected column
+__global__ void __launch_bounds__(256) k_project(const __grid_constant__ ProjArgs f) {
+  for_each_selected(f.items, f.bitmap, f.item_counts, f.item_base, f.n_items,
+                    [&](const DevItem& item, uint32_t, uint32_t r, unsigned long long pos) {
+                      if (pos < f.n_out) project_row(f, item, r, pos);
+                    });
+}
+
+// ORDER BY ... LIMIT on a scan: output row i is the selected row at position kept[i] of the selection (kept == nullptr:
+// i), reached through its handle (item index << 32 | row inside the item); one thread per output row
+__global__ void __launch_bounds__(256) k_project_rows(const __grid_constant__ ProjArgs f, const unsigned long long* __restrict__ handles,
+                                                      const uint32_t* __restrict__ kept) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= f.n_out) return;
+  const unsigned long long h = handles[kept ? kept[i] : i];
+  project_row(f, f.items[uint32_t(h >> 32)], uint32_t(h), i);
 }
 
 // string bytes of one projected column: one warp per output row

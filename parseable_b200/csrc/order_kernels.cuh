@@ -1,9 +1,14 @@
-// ORDER BY [... LIMIT n] over the groups of an aggregate query, on the device.  The result path lists the non-empty
-// group slots in ascending slot order (out_slot, k_slot_compact); ordering permutes and cuts that list before
-// k_agg_finish assembles the rows, so the batches, the Arrow stream and the JSON egress follow the new order unchanged.
+// ORDER BY [... LIMIT n] on the device, over the groups of an aggregate query or the selected rows of a scan.  The
+// aggregate result path lists the non-empty group slots in ascending slot order (out_slot, k_slot_compact); ordering
+// permutes and cuts that list before k_agg_finish assembles the rows, so the batches, the Arrow stream and the JSON
+// egress follow the new order unchanged.  A scan orders the positions of its selected rows and k_project_rows gathers
+// the kept ones into the projection's result block.
 //
-//   k_order_encode   one thread per row: every term's order-preserving u64 (order_keys.cuh) + NULL flag, and the
+//   k_order_encode   one thread per group: every term's order-preserving u64 (order_keys.cuh) + NULL flag, and the
 //                    value range of every term (one small D2H: the pack plan is sized from it)
+//   k_order_rows_encode
+//                    the same for every selected row of a scan (a CTA per work item, positions as k_project finds
+//                    them), plus the row's handle (item, row inside the item)
 //   k_order_pack     the terms packed MSB-first into the fewest 64-bit words their ranges need
 //   k_order_cta      rows <= kOrderCta: one CTA sorts (word 0, row) pairs in shared memory (bitonic, the row index as the
 //                    last key: stable), then writes the kept slots
@@ -16,9 +21,9 @@
 //                    anything larger: LSD radix sort of the row indices, 8-bit digits over the used bits of each word
 //                    from the least significant word up; per pass tile histograms, one scan of the digit x tile matrix
 //                    and a stable scatter (in-tile ranks from a __match_any_sync multisplit)
-//   k_order_gather   the first `keep` rows' slots in the new order
-// Rows equal on every term keep their slot order (the row index breaks every tie), so the ordered result is a stable
-// sort of the unordered one.
+//   k_order_gather   the first `keep` rows' slots in the new order (no slot list: the row indices themselves)
+// Rows equal on every term keep their slot order, or for a scan their selection order (the row index breaks every tie),
+// so the ordered result is a stable sort of the unordered one.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -106,6 +111,82 @@ __global__ void __launch_bounds__(256) k_order_encode(const __grid_constant__ Or
   }
 }
 
+// ---- scans: the terms are columns, read for the selected rows only ----
+struct RowOrderTerm {
+  uint32_t slot;          // column slot of the plan
+  uint8_t kind;           // DevKind
+  uint8_t enc;            // OrderEnc
+  uint8_t desc;
+  uint8_t _pad;
+  const uint32_t* gid;    // Utf8: the column's GROUP BY id of every dictionary entry (the per-row ids come as FK_IDS pages)
+  const uint32_t* rank;   // Utf8: bytewise rank of every id
+};
+struct RowOrderArgs {
+  const uint8_t* arena;
+  const uint8_t* flat;
+  const FlatPageRec* fpages;   // the table's flat pages; Utf8 term pages without a dictionary as FK_IDS pages
+  const DevChunk* chunks;
+  const DevItem* items;
+  const uint32_t* bitmap;
+  const uint32_t* item_counts;
+  const unsigned long long* item_base;
+  uint32_t n_items, plan_ncols, n, nterms;   // n: selected rows
+  unsigned long long* vals;    // [nterms][n] encoded values
+  uint8_t* nulls;              // [nterms][n]
+  OrderRange* ranges;          // [nterms], min = ~0 / max = 0 / flags 0 on entry
+  unsigned long long* handles; // [n]: item index << 32 | row inside the item
+  RowOrderTerm t[kMaxOrder];
+};
+
+__global__ void __launch_bounds__(256) k_order_rows_encode(const __grid_constant__ RowOrderArgs o) {
+  unsigned long long mn[kMaxOrder], mx[kMaxOrder];   // this thread's value range per term (registers: indexed by constants only)
+  uint32_t met_null = 0, met_value = 0;              // bit t: term t met a NULL / a value
+#pragma unroll
+  for (int k = 0; k < kMaxOrder; k++) { mn[k] = ~0ull; mx[k] = 0ull; }
+  for_each_selected(o.items, o.bitmap, o.item_counts, o.item_base, o.n_items,
+                    [&](const DevItem& item, uint32_t it, uint32_t r, unsigned long long pos) {
+    o.handles[pos] = (unsigned long long)it << 32 | r;
+    for (uint32_t t = 0; t < o.nterms; t++) {
+      const RowOrderTerm& ot = o.t[t];
+      unsigned long long bits = 0;
+      uint32_t len = 0;
+      const bool valid = flat_value_at<true>(o.arena, o.flat, o.fpages, o.chunks, o.plan_ncols, item, ot.slot, ot.kind, nullptr, ot.gid, r,
+                                             bits, len);
+      if (valid && ot.rank) bits = ot.rank[bits];
+      const unsigned long long v = order_encode(bits, ot.enc, ot.desc != 0);
+      o.vals[size_t(t) * o.n + pos] = v;
+      o.nulls[size_t(t) * o.n + pos] = valid ? 0 : 1;
+      if (valid) {
+        met_value |= 1u << t;
+#pragma unroll
+        for (int k = 0; k < kMaxOrder; k++)
+          if (k == int(t)) { mn[k] = min(mn[k], v); mx[k] = max(mx[k], v); }
+      } else {
+        met_null |= 1u << t;
+      }
+    }
+  });
+  // one warp reduction per term, one set of atomics per warp
+#pragma unroll
+  for (int k = 0; k < kMaxOrder; k++) {
+    if (k >= int(o.nterms)) break;
+    unsigned long long a = mn[k], b = mx[k];
+    for (int s = 16; s > 0; s >>= 1) {
+      a = min(a, __shfl_xor_sync(0xffffffffu, a, s));
+      b = max(b, __shfl_xor_sync(0xffffffffu, b, s));
+    }
+    const bool any_value = __any_sync(0xffffffffu, (met_value >> k) & 1u), any_null = __any_sync(0xffffffffu, (met_null >> k) & 1u);
+    if ((threadIdx.x & 31) == 0) {
+      if (any_value) {
+        atomicMin(&o.ranges[k].min, a);
+        atomicMax(&o.ranges[k].max, b);
+        atomicOr(&o.ranges[k].has_value, 1u);
+      }
+      if (any_null) atomicOr(&o.ranges[k].has_null, 1u);
+    }
+  }
+}
+
 // words[w][n]: the packed key of every row
 __global__ void __launch_bounds__(256) k_order_pack(const __grid_constant__ OrderPack p, const unsigned long long* __restrict__ vals,
                                                     const uint8_t* __restrict__ nulls, uint32_t n, unsigned long long* __restrict__ words) {
@@ -163,7 +244,7 @@ __global__ void __launch_bounds__(1024) k_order_cta(const unsigned long long* __
       __syncthreads();
     }
   }
-  for (uint32_t r = threadIdx.x; r < keep; r += blockDim.x) new_slot[r] = out_slot[row[r]];
+  for (uint32_t r = threadIdx.x; r < keep; r += blockDim.x) new_slot[r] = out_slot ? out_slot[row[r]] : row[r];
 }
 
 // one radix pass: digit counts of every tile of kRadixTile positions, digit-major (hist[d * ntiles + tile])
@@ -311,7 +392,7 @@ __global__ void __launch_bounds__(256) k_topk_compact(const unsigned long long* 
 __global__ void k_order_gather(const uint32_t* __restrict__ idx, uint32_t keep, const uint32_t* __restrict__ out_slot,
                                uint32_t* __restrict__ new_slot) {
   const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r < keep) new_slot[r] = out_slot[idx[r]];
+  if (r < keep) new_slot[r] = out_slot ? out_slot[idx[r]] : idx[r];
 }
 
 }  // namespace pqb

@@ -523,36 +523,36 @@ void unify_key_side(const Table& t, int tcol, ColSide& cs, cudaStream_t stream) 
 
 namespace {
 
-// ORDER BY [LIMIT]: out_slot[0, n) becomes the first `keep` slots in the query's order (order_kernels.cuh).  One round
-// trip: the value ranges the pack plan is sized from.  The kernels before it are timed by `t_enc`, those after it by
-// `t_sort` (every buffer is allocated before the events, so the spans hold device work only); *sort_timed says whether
-// the second span was recorded.  Returns the kernels it launched.
-uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, DevBuf<uint32_t>& out_slot, cudaStream_t stream,
-                      PqMetrics& m, Timer& t_enc, Timer& t_sort, bool* sort_timed) {
-  const uint32_t n = oa.n;
-  uint64_t launches = 0;
-  *sort_timed = false;
+// What an ORDER BY encode step writes for n rows: [nterms][n] order-preserving values and NULL flags, and the value range
+// of every term (reset here: min = ~0, max = 0, no flags).
+struct OrderBufs {
   DevBuf<unsigned long long> vals;
   DevBuf<uint8_t> nulls;
   DevBuf<OrderRange> ranges;
-  vals.alloc(size_t(oa.nterms) * n, stream);
-  nulls.alloc(size_t(oa.nterms) * n, stream);
-  std::vector<OrderRange> hr(oa.nterms, OrderRange{~0ull, 0ull, 0u, 0u});
-  ranges.upload(hr, stream);
-  oa.vals = vals.p;
-  oa.nulls = nulls.p;
-  oa.ranges = ranges.p;
-  PQB_CUDA(cudaEventRecord(t_enc.a, stream));
-  k_order_encode<<<(n + 255) / 256, 256, 0, stream>>>(oa);
-  PQB_CUDA(cudaEventRecord(t_enc.b, stream));
-  launches++;
-  PQB_CUDA(cudaMemcpyAsync(hr.data(), ranges.p, hr.size() * sizeof(OrderRange), cudaMemcpyDeviceToHost, stream));
+  OrderBufs(uint32_t nterms, uint32_t n, cudaStream_t stream, PqMetrics& m) {
+    vals.alloc(size_t(nterms) * n, stream);
+    nulls.alloc(size_t(nterms) * n, stream);
+    ranges.upload(std::vector<OrderRange>(nterms, OrderRange{~0ull, 0ull, 0u, 0u}), stream);
+    m.h2d_bytes += nterms * sizeof(OrderRange);
+  }
+};
+
+// ORDER BY [LIMIT] of n encoded rows (groups or selected scan rows), after the caller's encode step.  One round trip: the
+// value ranges the pack plan is sized from.  Then `kept` becomes the first `keep` rows in the query's order, as their
+// entries of `rows` (nullptr: the row indices themselves); it stays empty when every term is one value for every row
+// (the row order is the order).  The kernels are timed by `t_sort` (every buffer is allocated before the events, so the
+// span holds device work only); *sort_timed says whether it was recorded.  Returns the kernels it launched.
+uint64_t order_sort(const OrderBufs& ob, uint32_t nterms, uint32_t n, const uint8_t* nulls_first, uint32_t keep, const uint32_t* rows,
+                    DevBuf<uint32_t>& kept, cudaStream_t stream, PqMetrics& m, Timer& t_sort, bool* sort_timed) {
+  uint64_t launches = 0;
+  *sort_timed = false;
+  std::vector<OrderRange> hr(nterms);
+  PQB_CUDA(cudaMemcpyAsync(hr.data(), ob.ranges.p, hr.size() * sizeof(OrderRange), cudaMemcpyDeviceToHost, stream));
   PQB_CUDA(cudaStreamSynchronize(stream));
-  m.h2d_bytes += hr.size() * sizeof(OrderRange);
   m.d2h_bytes += hr.size() * sizeof(OrderRange);
   OrderPack pk{};
-  order_pack_plan(hr.data(), nulls_first, oa.nterms, pk);
-  if (pk.nwords == 0) return launches;   // every term is one value for every row: the slot order is the order
+  order_pack_plan(hr.data(), nulls_first, nterms, pk);
+  if (pk.nwords == 0) return launches;   // every term is one value for every row: the row order is the order
   // the path: the one-CTA sort when every row fits it, top-K when one word holds the key and the kept rows fit the CTA
   // sort, else the radix sort.  PQB_ORDER_PATH=cta|topk|sort (experiment switch) forces a path where it is legal.
   const char* e = getenv("PQB_ORDER_PATH");
@@ -562,19 +562,19 @@ uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, D
   if (want == "sort") path = P_SORT;
   else if (want == "topk" && topk_ok) path = P_TOPK;
   else if (want == "cta" && cta_ok) path = P_CTA;
+  const uint32_t grid_n = uint32_t((uint64_t(n) + 255) / 256);
   DevBuf<unsigned long long> words;
   words.alloc(size_t(pk.nwords) * n, stream);
-  DevBuf<uint32_t> slots;
-  slots.alloc(keep, stream);
+  kept.alloc(keep, stream);
   const int smem = int(kOrderCta * (8 + 4));
   if (path != P_SORT) PQB_CUDA(cudaFuncSetAttribute(k_order_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   if (path == P_CTA) {
     PQB_CUDA(cudaEventRecord(t_sort.a, stream));
-    k_order_pack<<<(n + 255) / 256, 256, 0, stream>>>(pk, vals.p, nulls.p, n, words.p);
-    k_order_cta<<<1, 1024, smem, stream>>>(words.p, n, pk.nwords, nullptr, n, keep, out_slot.p, slots.p);
+    k_order_pack<<<grid_n, 256, 0, stream>>>(pk, ob.vals.p, ob.nulls.p, n, words.p);
+    k_order_cta<<<1, 1024, smem, stream>>>(words.p, n, pk.nwords, nullptr, n, keep, rows, kept.p);
     launches += 2;
   } else if (path == P_TOPK) {
-    const uint32_t ntiles = (n + kSlotTile - 1) / kSlotTile;
+    const uint32_t ntiles = uint32_t((uint64_t(n) + kSlotTile - 1) / kSlotTile);
     DevBuf<TopkSel> sel;
     DevBuf<uint32_t> tile_counts, cand, count;
     DevBuf<unsigned long long> tile_base, total;
@@ -589,9 +589,9 @@ uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, D
     PQB_CUDA(cudaMemcpyAsync(sel.p, &init, sizeof(TopkSel), cudaMemcpyHostToDevice, stream));
     count.zero();
     m.h2d_bytes += sizeof(TopkSel);
-    const uint32_t hgrid = std::min<uint32_t>((n + 255) / 256, uint32_t(Context::get().sm_count()) * 8);
+    const uint32_t hgrid = std::min<uint32_t>(grid_n, uint32_t(Context::get().sm_count()) * 8);
     PQB_CUDA(cudaEventRecord(t_sort.a, stream));
-    k_order_pack<<<(n + 255) / 256, 256, 0, stream>>>(pk, vals.p, nulls.p, n, words.p);
+    k_order_pack<<<grid_n, 256, 0, stream>>>(pk, ob.vals.p, ob.nulls.p, n, words.p);
     launches++;
     // MSB digit first over the used bits only (MSB-first packing: bits [64 - total_bits, 64)); the lowest digit starts at
     // the lowest used bit, the highest may reach past bit 63 (those bits are zero)
@@ -605,12 +605,10 @@ uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, D
     k_topk_tile_eq<<<ntiles, 256, 0, stream>>>(words.p, n, sel.p, tile_counts.p);
     k_item_prefix<<<1, 1024, 0, stream>>>(tile_counts.p, ntiles, tile_base.p, total.p);
     k_topk_compact<<<ntiles, 256, 0, stream>>>(words.p, n, sel.p, tile_base.p, cand.p, count.p);
-    k_order_cta<<<1, 1024, smem, stream>>>(words.p, n, 1, cand.p, keep, keep, out_slot.p, slots.p);
+    k_order_cta<<<1, 1024, smem, stream>>>(words.p, n, 1, cand.p, keep, keep, rows, kept.p);
     launches += 4;
-    PQB_CUDA(cudaEventRecord(t_sort.b, stream));
-    *sort_timed = true;
   } else {
-    const uint32_t ntiles = (n + kRadixTile - 1) / kRadixTile;
+    const uint32_t ntiles = uint32_t((uint64_t(n) + kRadixTile - 1) / kRadixTile);
     DevBuf<uint32_t> hist, ia, ib;
     DevBuf<unsigned long long> base, total;
     hist.alloc(size_t(256) * ntiles, stream);
@@ -619,9 +617,9 @@ uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, D
     ia.alloc(n, stream);
     ib.alloc(n, stream);
     PQB_CUDA(cudaEventRecord(t_sort.a, stream));
-    k_order_pack<<<(n + 255) / 256, 256, 0, stream>>>(pk, vals.p, nulls.p, n, words.p);
+    k_order_pack<<<grid_n, 256, 0, stream>>>(pk, ob.vals.p, ob.nulls.p, n, words.p);
     launches++;
-    const uint32_t* cur = nullptr;   // the first pass reads the rows in slot order
+    const uint32_t* cur = nullptr;   // the first pass reads the rows in row order
     uint32_t* out = ia.p;
     for (int w = int(pk.nwords) - 1; w >= 0; w--) {   // least significant word first
       const unsigned long long* key = words.p + size_t(w) * n;
@@ -635,15 +633,32 @@ uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, D
         out = out == ia.p ? ib.p : ia.p;
       }
     }
-    k_order_gather<<<(keep + 255) / 256, 256, 0, stream>>>(cur, keep, out_slot.p, slots.p);
+    k_order_gather<<<(keep + 255) / 256, 256, 0, stream>>>(cur, keep, rows, kept.p);
     launches++;
-    PQB_CUDA(cudaEventRecord(t_sort.b, stream));
-    *sort_timed = true;
   }
-  if (path == P_CTA) { PQB_CUDA(cudaEventRecord(t_sort.b, stream)); *sort_timed = true; }
+  PQB_CUDA(cudaEventRecord(t_sort.b, stream));
+  *sort_timed = true;
   PQB_CUDA(cudaGetLastError());
-  std::swap(out_slot.p, slots.p);   // the old list is freed with `slots`
-  std::swap(out_slot.n, slots.n);
+  return launches;
+}
+
+// ORDER BY [LIMIT] of an aggregate result: out_slot[0, n) becomes the first `keep` slots in the query's order.  The
+// encode kernel is timed by `t_enc`, the sort by `t_sort` (order_sort).  Returns the kernels it launched.
+uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, DevBuf<uint32_t>& out_slot, cudaStream_t stream,
+                      PqMetrics& m, Timer& t_enc, Timer& t_sort, bool* sort_timed) {
+  OrderBufs ob(oa.nterms, oa.n, stream, m);
+  oa.vals = ob.vals.p;
+  oa.nulls = ob.nulls.p;
+  oa.ranges = ob.ranges.p;
+  PQB_CUDA(cudaEventRecord(t_enc.a, stream));
+  k_order_encode<<<(oa.n + 255) / 256, 256, 0, stream>>>(oa);
+  PQB_CUDA(cudaEventRecord(t_enc.b, stream));
+  DevBuf<uint32_t> slots;
+  const uint64_t launches = 1 + order_sort(ob, oa.nterms, oa.n, nulls_first, keep, out_slot.p, slots, stream, m, t_sort, sort_timed);
+  if (slots.p) {
+    std::swap(out_slot.p, slots.p);   // the old list is freed with `slots`
+    std::swap(out_slot.n, slots.n);
+  }
   return launches;
 }
 
@@ -669,17 +684,24 @@ void Query::run(const PqQueryDesc& d) {
   if (d.n_pred > (uint32_t)kMaxPredOps) throw Error(PQ_ERR_UNSUPPORTED, "predicate program too long");
   if (d.n_group_by && !d.n_aggs) throw Error(PQ_ERR_INVALID_ARG, "GROUP BY without aggregates");
   const bool ordered = d.n_order_by > 0;
+  const bool row_order = ordered && !d.n_aggs;   // ORDER BY ... LIMIT on a filter / projection scan: the terms are columns
   if (ordered) {
-    if (!d.n_aggs) throw Error(PQ_ERR_UNSUPPORTED, "ORDER BY on a filter / projection scan: only aggregate results are sorted on the GPU");
     if (d.n_order_by > uint32_t(kMaxOrder)) throw Error(PQ_ERR_UNSUPPORTED, "more than 8 ORDER BY terms");
     if (!d.order_by) throw Error(PQ_ERR_INVALID_ARG, "n_order_by > 0 without order_by");
     for (uint32_t t = 0; t < d.n_order_by; t++) {
       const PqOrderBy& ob = d.order_by[t];
-      const uint32_t n = ob.target == PQ_ORDER_KEY ? d.n_group_by : ob.target == PQ_ORDER_AGG ? d.n_aggs : 0;
-      if (ob.target != PQ_ORDER_KEY && ob.target != PQ_ORDER_AGG) throw Error(PQ_ERR_INVALID_ARG, "ORDER BY term " + std::to_string(t) + ": unknown target");
+      const std::string term = "ORDER BY term " + std::to_string(t) + ": ";
+      if (ob.target != PQ_ORDER_KEY && ob.target != PQ_ORDER_AGG && ob.target != PQ_ORDER_COLUMN) throw Error(PQ_ERR_INVALID_ARG, term + "unknown target");
+      if (row_order && ob.target != PQ_ORDER_COLUMN)
+        throw Error(PQ_ERR_UNSUPPORTED, term + "ORDER BY on a filter / projection scan orders by columns (PQ_ORDER_COLUMN), not by a GROUP BY key or an aggregate");
+      if (!row_order && ob.target == PQ_ORDER_COLUMN)
+        throw Error(PQ_ERR_INVALID_ARG, term + "an aggregate query orders by its GROUP BY keys and aggregates, not by a column (PQ_ORDER_COLUMN)");
+      const uint32_t n = ob.target == PQ_ORDER_KEY ? d.n_group_by : ob.target == PQ_ORDER_AGG ? d.n_aggs : d.n_columns;
       if (ob.index < 0 || uint32_t(ob.index) >= n)
-        throw Error(PQ_ERR_INVALID_ARG, "ORDER BY term " + std::to_string(t) + ": " + (ob.target == PQ_ORDER_KEY ? "GROUP BY" : "aggregate") + " index out of range");
+        throw Error(PQ_ERR_INVALID_ARG, term + (ob.target == PQ_ORDER_KEY ? "GROUP BY" : ob.target == PQ_ORDER_AGG ? "aggregate" : "column") + " index out of range");
     }
+    if (row_order && (d.flags & PQ_QUERY_COUNT_ONLY)) throw Error(PQ_ERR_INVALID_ARG, "ORDER BY with PQ_QUERY_COUNT_ONLY: a count has no rows to order");
+    if (row_order && d.limit < 0) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY needs a LIMIT (limit >= 0)");
   }
 
   cudaStream_t stream;
@@ -905,6 +927,7 @@ void Query::run(const PqQueryDesc& d) {
     if (d.projection[i] < 0 || uint32_t(d.projection[i]) >= d.n_columns) throw Error(PQ_ERR_INVALID_ARG, "projection column out of range");
     col_used[d.projection[i]] = true;        // only gathered for the selected rows
   }
+  for (uint32_t t = 0; row_order && t < d.n_order_by; t++) col_used[d.order_by[t].index] = true;   // likewise: read for the selected rows
   // compact to kernel column slots
   std::vector<int> slot_of(d.n_columns, -1);
   std::vector<uint32_t> qcol_of_slot;
@@ -1386,6 +1409,53 @@ void Query::run(const PqQueryDesc& d) {
     if (n_general)
       throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + table->columns[shape_cols[plan.dist[i].col]].name +
                                           ") needs a flat-store copy of every page the query reads: " + shape->why_general);
+  if (row_order && n_general)
+    throw Error(PQ_ERR_UNSUPPORTED, "ORDER BY on a scan needs a flat-store copy of every page the query reads: " + shape->why_general);
+  // ---- ORDER BY on a scan: a Utf8 term sorts by the bytewise rank of the column's GROUP BY ids (ensure_key, cached with
+  // the table); its pages without a dictionary are read as their id pages, through this query's copy of the flat page
+  // table that only the encode kernel sees ----
+  RowOrderArgs roa{};
+  uint8_t row_nulls_first[kMaxOrder] = {};
+  std::vector<std::shared_ptr<const uint32_t>> row_rank_hold;   // a query keeps the ranks it sorts with alive
+  DevBuf<FlatPageRec> d_opages;
+  if (row_order) {
+    std::vector<int> id_cols;   // table columns whose pages without a dictionary are read as id pages
+    roa.nterms = d.n_order_by;
+    for (uint32_t t = 0; t < d.n_order_by; t++) {
+      const PqOrderBy& ob = d.order_by[t];
+      RowOrderTerm& ot = roa.t[t];
+      ot.slot = uint32_t(slot_of[ob.index]);
+      ot.kind = plan.cols[ot.slot].kind;
+      ot.desc = (ob.flags & PQ_ORDER_DESC) ? 1 : 0;
+      row_nulls_first[t] = (ob.flags & PQ_ORDER_NULLS_FIRST) ? 1 : 0;
+      ot.enc = ot.kind == DK_F64 ? OE_F64 : ot.kind == DK_I64 ? OE_I64 : OE_RAW;   // Boolean: 0 / 1; Utf8: the rank
+      const int tc_i = shape_cols[ot.slot];
+      if (ot.kind != DK_STR || table->columns[tc_i].kind == 0xfe) continue;   // in no file: every row NULL, nothing to rank
+      table->ensure_key(tc_i, stream);
+      row_rank_hold.push_back(table->ensure_kd_rank(tc_i, false, stream));
+      ot.gid = table->sides[tc_i].d_gid;
+      ot.rank = row_rank_hold.back().get();
+      if (!table->sides[tc_i].key_row_pages.empty()) id_cols.push_back(tc_i);
+    }
+    if (!id_cols.empty()) {
+      std::vector<FlatPageRec> fp;
+      {
+        std::lock_guard<std::mutex> lk(table->side_mu);
+        fp = table->flat_pages;
+        for (int tc_i : id_cols) {
+          const ColSide& cs = table->sides[tc_i];
+          for (const ColSide::KeyRowPage& rp : cs.key_row_pages) {
+            FlatPageRec& r = fp[rp.page];
+            r.fkind = FK_IDS;
+            r.bw = 32;
+            r.off = uint64_t(cs.d_gid) + 4ull * (uint64_t(cs.n_dict_pad) + rp.ebase) - uint64_t(table->d_flat);   // as for key columns
+          }
+        }
+      }
+      d_opages.upload(fp, stream);
+      metrics.h2d_bytes += fp.size() * sizeof(FlatPageRec);
+    }
+  }
   mark("side tables ready");
   // ---- shared-memory layout of k_scan (items the flat kernels do not take) ----
   SmemLayout L{};
@@ -1958,7 +2028,7 @@ void Query::run(const PqQueryDesc& d) {
     PQB_CUDA(cudaMemcpyAsync(&total, d_total.p, 8, cudaMemcpyDeviceToHost, stream));
     metrics.d2h_bytes += 8 + sizeof(h_counters);
     const unsigned long long lim = d.limit >= 0 ? (unsigned long long)d.limit : ~0ull;
-    if (projecting) {
+    if (projecting || row_order) {
       // ---- TableProvider::scan(projection): gather the projected columns of the selected rows ----
       struct PC { uint32_t qcol; uint32_t slot; uint8_t kind; std::string name; int type; };
       std::vector<PC> pcs;
@@ -1967,7 +2037,8 @@ void Query::run(const PqQueryDesc& d) {
         pcs.push_back({qc, uint32_t(slot_of[qc]), plan.cols[slot_of[qc]].kind, d.columns[qc].name, out_type_of(qc)});
         if (pcs.back().kind == DK_STR) table->ensure_ent_off(shape_cols[slot_of[qc]], stream);
       }
-      if (d.flags & PQ_QUERY_EMIT_ROW_IDS) pcs.push_back({0, 0xffffffffu, DK_I64, "__row_id", PQ_T_I64});
+      // an ordered scan without a projection returns its selected row ordinals in order
+      if ((d.flags & PQ_QUERY_EMIT_ROW_IDS) || !projecting) pcs.push_back({0, 0xffffffffu, DK_I64, "__row_id", PQ_T_I64});
       const uint32_t npc = uint32_t(pcs.size());
       std::shared_ptr<PinnedBlock> block;
       ProjArgs pj{};
@@ -1976,7 +2047,8 @@ void Query::run(const PqQueryDesc& d) {
       const uint32_t wpb = (batch_rows + 31) / 32;
       unsigned long long n_rows = 0;
       DevBuf<uint8_t> d_block;
-      auto gather = [&](unsigned long long cap) {
+      // the first `cap` selected rows, or with `handles` the rows at positions kept[0, cap) (ORDER BY ... LIMIT)
+      auto gather = [&](unsigned long long cap, const unsigned long long* handles, const uint32_t* kept) {
         nbatches = uint32_t((cap + batch_rows - 1) / batch_rows);
         uint64_t off = 0;
         auto take = [&](uint64_t bytes) { uint64_t o = off; off = (off + bytes + 63) & ~63ull; return o; };
@@ -2022,8 +2094,12 @@ void Query::run(const PqQueryDesc& d) {
         pj.batch_rows = batch_rows;
         pj.words_per_batch = wpb;
         pj.nbatches = nbatches;
-        const uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
-        k_project<<<grid, 256, 0, stream>>>(pj);
+        if (handles) {
+          k_project_rows<<<uint32_t((cap + 255) / 256), 256, 0, stream>>>(pj, handles, kept);
+        } else {
+          const uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
+          k_project<<<grid, 256, 0, stream>>>(pj);
+        }
         launches++;
         for (uint32_t c = 0; c < npc; c++) {
           if (pj.cols[c].kind != DK_STR) continue;
@@ -2039,13 +2115,60 @@ void Query::run(const PqQueryDesc& d) {
         block->bytes = copy_bytes;
         PQB_CUDA(cudaMemcpyAsync(block->p, d_block.p, copy_bytes, cudaMemcpyDeviceToHost, stream));
       };
-      if (!items.empty()) {
+      if (row_order && !items.empty()) {
+        // ---- ORDER BY ... LIMIT: every selected row's terms and handle (k_order_rows_encode), the positions of the first
+        // `keep` rows in order (order_sort), then their projection.  Per shard: the merge of the shards' rows is above.
+        PQB_CUDA(cudaStreamSynchronize(stream));   // the selected-row total sizes the sort
+        if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
+        if (total > 0xffffffffull) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY over more than 2^32 - 1 selected rows");
+        const unsigned long long keep = std::min(total, lim);
+        if (keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
+        if (keep) {
+          const uint32_t n = uint32_t(total);
+          OrderBufs ob(roa.nterms, n, stream, metrics);
+          DevBuf<unsigned long long> handles;
+          DevBuf<uint32_t> kept;
+          handles.alloc(n, stream);
+          roa.arena = table->d_arena;
+          roa.flat = table->d_flat;
+          roa.fpages = d_opages.p ? d_opages.p : table->d_flat_pages;
+          roa.chunks = shape->d_chunks;
+          roa.items = shape->d_items;
+          roa.bitmap = d_bitmap.p;
+          roa.item_counts = d_item_counts.p;
+          roa.item_base = d_item_base.p;
+          roa.n_items = uint32_t(items.size());
+          roa.plan_ncols = ncols;
+          roa.n = n;
+          roa.vals = ob.vals.p;
+          roa.nulls = ob.nulls.p;
+          roa.ranges = ob.ranges.p;
+          roa.handles = handles.p;
+          uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
+          if (const char* g = getenv("PQB_GRID")) grid = std::max(1, atoi(g));   // debugging aid: several items per CTA
+          Timer t_enc, t_sort;
+          bool sort_timed = false;
+          PQB_CUDA(cudaEventRecord(t_enc.a, stream));
+          k_order_rows_encode<<<grid, 256, 0, stream>>>(roa);
+          PQB_CUDA(cudaEventRecord(t_enc.b, stream));
+          launches += 1 + order_sort(ob, roa.nterms, n, row_nulls_first, uint32_t(keep), nullptr, kept, stream, metrics, t_sort, &sort_timed);
+          gather(keep, handles.p, kept.p);
+          PQB_CUDA(cudaStreamSynchronize(stream));
+          metrics.d2h_bytes += copy_bytes;
+          float ms = 0, ms2 = 0;
+          cudaEventElapsedTime(&ms, t_enc.a, t_enc.b);
+          if (sort_timed) cudaEventElapsedTime(&ms2, t_sort.a, t_sort.b);
+          metrics.order_ms = double(ms) + double(ms2);
+        }
+        n_rows = keep;
+        shape->last_total.store(total);
+      } else if (!items.empty()) {
         const unsigned long long hint = shape->last_total.load();
         bool done = false;
         if (hint != ~0ull) {
           const unsigned long long cap = std::max<unsigned long long>(1, std::min(lim, hint + hint / 8 + 1024));
           if (cap > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
-          gather(cap);
+          gather(cap, nullptr, nullptr);
           PQB_CUDA(cudaStreamSynchronize(stream));
           if (std::min(total, lim) <= cap) { done = true; n_rows = std::min(total, lim); metrics.d2h_bytes += copy_bytes; }
           else block.reset();
@@ -2056,7 +2179,7 @@ void Query::run(const PqQueryDesc& d) {
           const unsigned long long keep = std::min(total, lim);
           if (keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
           if (keep) {
-            gather(keep);
+            gather(keep, nullptr, nullptr);
             PQB_CUDA(cudaStreamSynchronize(stream));
             metrics.d2h_bytes += copy_bytes;
           }

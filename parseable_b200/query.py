@@ -209,16 +209,20 @@ class _Desc:
             raise QueryError(L.PQ_ERR_UNSUPPORTED, f"expression {e.kind} in a predicate")
 
 
-def _order_term(group_by: list, aggs: list, term) -> tuple[int, int, int]:
-    """One ORDER BY term of ``aggregate`` -> (PqOrderTarget, index, PqOrderBy flags)."""
-    item, direction, *rest = term
-    nulls_first = rest[0] if rest else None
+def _order_flags(direction, nulls_first) -> int:
+    """PqOrderBy flags of ``asc`` / ``desc`` and NULLS FIRST (True) / LAST (False) / the default (None)."""
     if str(direction).lower() not in ("asc", "desc"):
         raise QueryError(L.PQ_ERR_INVALID_ARG, f"ORDER BY direction {direction!r}: asc or desc")
     desc = str(direction).lower() == "desc"
     if nulls_first is None:
         nulls_first = desc               # DataFusion: ASC -> NULLS LAST, DESC -> NULLS FIRST
-    flags = (L.PQ_ORDER_DESC if desc else 0) | (L.PQ_ORDER_NULLS_FIRST if nulls_first else 0)
+    return (L.PQ_ORDER_DESC if desc else 0) | (L.PQ_ORDER_NULLS_FIRST if nulls_first else 0)
+
+
+def _order_term(group_by: list, aggs: list, term) -> tuple[int, int, int]:
+    """One ORDER BY term of ``aggregate`` -> (PqOrderTarget, index, PqOrderBy flags)."""
+    item, direction, *rest = term
+    flags = _order_flags(direction, rest[0] if rest else None)
     if isinstance(item, Agg):
         if item in aggs:
             return L.PQ_ORDER_AGG, aggs.index(item), flags
@@ -424,10 +428,14 @@ class StandardTableProvider:
     # -- TableProvider::scan -------------------------------------------------
     def scan(self, projection: Sequence[str] | None = None, filters: Iterable[Expr] = (), limit: int | None = None,
              count_only: bool = False, row_ids: bool | None = None, batch_size: int = 0, flags: int = 0,
-             poll: bool = False, json: str | None = None) -> QueryResult:
+             poll: bool = False, json: str | None = None, order_by: Sequence | None = None) -> QueryResult:
         """``projection``: the columns to return for the selected rows (TableProvider::scan's projection);
         without one the scan returns the selected row ordinals (``__row_id``).  ``row_ids=True`` appends
-        ``__row_id`` to a projection."""
+        ``__row_id`` to a projection.  ``order_by``: ``[(column, "asc" | "desc"[, nulls_first]), ...]``, most
+        significant first, with a ``limit``: the first ``limit`` selected rows in that order, selected and sorted on
+        the GPU (the SortExec(fetch) / TopK above the scan); the columns need not be projected.  ``nulls_first=None``
+        follows the same default as ``aggregate``."""
+        order = [(L.PQ_ORDER_COLUMN, c, _order_flags(direction, rest[0] if rest else None)) for c, direction, *rest in (order_by or [])]
         f = 0
         if row_ids is None:
             row_ids = not projection
@@ -435,7 +443,7 @@ class StandardTableProvider:
             f |= L.PQ_QUERY_COUNT_ONLY
         elif row_ids:
             f |= L.PQ_QUERY_EMIT_ROW_IDS
-        return self._run(list(filters), [], [], list(projection or []), limit, batch_size, f | flags, poll=poll, json=json)
+        return self._run(list(filters), [], [], list(projection or []), limit, batch_size, f | flags, poll=poll, json=json, order=order)
 
     # -- FilterExec + AggregateExec folded into the same call ----------------
     def aggregate(self, group_by: Sequence[str], aggs: Sequence[Agg], filters: Iterable[Expr] = (),
@@ -480,6 +488,8 @@ class StandardTableProvider:
         for a in aggs:
             ag.append(L.PqAgg(fn=_AGG_CODE[a.fn], col=d.col_index(a.column) if a.column is not None else -1))
         proj = [d.col_index(c) for c in projection]
+        # PQ_ORDER_COLUMN terms name their column: it joins the referenced columns
+        order = [(t, d.col_index(i) if isinstance(i, str) else i, fl) for t, i, fl in order]
 
         desc = L.PqQueryDesc()
         hfs = None
@@ -578,7 +588,7 @@ class TimeRange:
 
 class Query:
     """``SELECT <cols | aggs> FROM <stream> [WHERE ...] [GROUP BY ...] [ORDER BY ...] [LIMIT n]`` — the subset of SQL the
-    GPU path executes.  The reference hands SQL to DataFusion's planner (src/query/mod.rs:261-264);
+    GPU path executes (ORDER BY on a query without aggregates only with a LIMIT).  The reference hands SQL to DataFusion's planner (src/query/mod.rs:261-264);
     that planner is out of scope (SURVEY §2), so this small recursive-descent parser only exists
     to let tests and the bench state their queries the way Parseable users do."""
 
@@ -638,10 +648,14 @@ class Query:
                 self.order_by.append(self._order_item())
                 if not self._accept("op", ","):
                     break
-            if not any(it[0] == "agg" for it in self.select):
-                raise QueryError(L.PQ_ERR_UNSUPPORTED, "ORDER BY on a query without aggregates: row-level sorting is not on the GPU path")
         if self._accept("kw", "LIMIT"):
             self.limit = int(self._next("num")[1])
+        if self.order_by and not any(it[0] == "agg" for it in self.select):
+            # rows are ordered on the GPU as a top-K of the selection (SortExec(fetch)), never as a full sort
+            if self.limit is None:
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, "ORDER BY on a query without aggregates needs a LIMIT: a full row-level sort is not on the GPU path")
+            if any(item[0] == "agg" for item, _, _ in self.order_by):
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, "an aggregate in ORDER BY of a query without aggregates")
         if self._i != len(self._t):
             raise QueryError(L.PQ_ERR_UNSUPPORTED, f"unsupported SQL near {self._t[self._i]!r}")
 
@@ -853,7 +867,20 @@ def execute(query: Query, provider: StandardTableProvider, is_streaming: bool = 
         if not provider.schema:
             raise QueryError(L.PQ_ERR_INVALID_ARG, "SELECT * needs the table schema")
         cols = list(provider.schema.keys())
-    res = provider.scan(cols, filters, query.limit)
+    # ORDER BY items -> columns: a position in the SELECT list (SELECT * counts as the schema's columns), a SELECT alias,
+    # or any column of the stream
+    listed = [c for it in query.select for c in (list(provider.schema.keys()) if it[0] == "star" else [it[1]])]
+    order = []
+    for (kind, v), direction, nulls_first in query.order_by:
+        if kind == "pos":
+            if not 1 <= v <= len(listed):
+                raise QueryError(L.PQ_ERR_INVALID_ARG, f"ORDER BY {v}: the SELECT list has {len(listed)} items")
+            target = listed[v - 1]
+        else:
+            alias = [it[1] for it in query.select if it[0] == "col" and it[2] == v]
+            target = alias[0] if alias else v
+        order.append((target, direction, nulls_first))
+    res = provider.scan(cols, filters, query.limit, order_by=order or None)
     aliases = {it[1]: it[2] for it in query.select if it[0] == "col" and it[2]}
     if aliases and res.batches:
         names = [aliases.get(n, n) for n in res.batches[0].schema.names]

@@ -8,7 +8,9 @@
 // on the CPU by tests/test_decode_core.py through tools/decode_core_host.cpp
 // (test harness only; it is never linked into libparseable_b200.so).
 #pragma once
+#include <cmath>
 #include <cstdint>
+#include <cstring>
 
 #include "device_structs.hpp"
 
@@ -387,6 +389,49 @@ PQ_HD int64_t f64_order_key(uint64_t bits) {
 }
 PQ_HD uint64_t f64_from_order_key(int64_t k) {
   return uint64_t(k ^ int64_t(uint64_t(k >> 63) >> 1));
+}
+
+// ---- value pages (FK_FOR): numeric dictionary pages as bit-packed values ----
+// An Int64 value v is stored as the w-bit offset v - base (64-bit wrapping: base + bits gives v back exactly).  A Float64
+// value v is first written as an integer k with dec_decode_f64(k, e) == v bit for bit (|k| < 2^53), then stored like an
+// Int64.  A value without such a k (NaN, infinities, -0.0, subnormals, most random doubles) refuses the encoding, and its
+// chunk keeps the dictionary.
+//
+// The decode is k / 10^e rounded to nearest: the quotient through the correctly rounded reciprocal, plus one exact FMA
+// correction step (q0 = k * r, rem = k - q0 * 10^e exactly, q = q0 + rem * r).  That is the IEEE quotient for decimal
+// values (tests/test_agg_forms.py compares it with IEEE division), costs two FMAs and a multiply instead of the
+// division's slow-path call -- which spilled the aggregate kernel's registers -- and, above all, the encoder accepts k
+// only when THIS function gives v back, so no value ever changes whatever the rounding of a corner case.
+constexpr uint32_t kForMaxExp = 9;      // decimal exponents 0 .. 9 are tried
+constexpr uint32_t kForMaxBits = 32;    // a chunk whose offsets need more bits keeps the dictionary
+struct DecScale { double p10, rinv; };
+PQ_HD DecScale dec_scale(uint32_t e) {   // 10^e is exact for e <= 22
+  double p = 1.0;
+  for (uint32_t i = 0; i < e; i++) p *= 10.0;
+  return DecScale{p, 1.0 / p};
+}
+PQ_HD double f64_of_bits(uint64_t b) { double d; memcpy(&d, &b, 8); return d; }
+PQ_HD uint64_t bits_of_f64(double d) { uint64_t b; memcpy(&b, &d, 8); return b; }
+PQ_HD uint64_t dec_decode_f64(int64_t k, DecScale s) {
+  const double x = double(k), q0 = x * s.rinv;
+  return bits_of_f64(fma(fma(-q0, s.p10, x), s.rinv, q0));
+}
+// false: v has no k at this exponent
+PQ_HD bool dec_encode_f64(uint64_t bits, DecScale s, int64_t& k) {
+  if (bits == 0x8000000000000000ull) return false;   // -0.0 would come back as +0.0
+  const double v = f64_of_bits(bits);
+  if (!(v - v == 0.0)) return false;                 // NaN, +-inf
+  const double r = rint(v * s.p10);
+  if (!(fabs(r) < 9007199254740992.0)) return false; // |k| < 2^53: double(k) is exact
+  k = int64_t(r);
+  return dec_decode_f64(k, s) == bits;
+}
+PQ_HD uint64_t for_encode(int64_t v, int64_t base) { return uint64_t(v) - uint64_t(base); }
+PQ_HD int64_t for_decode(int64_t base, uint32_t bits) { return int64_t(uint64_t(base) + bits); }
+PQ_HD uint32_t bit_width_u64(uint64_t x) {
+  uint32_t n = 0;
+  while (x) { n++; x >>= 1; }
+  return n;
 }
 
 // compare with PqCmp codes: 0 EQ 1 NE 2 LT 3 LE 4 GT 5 GE

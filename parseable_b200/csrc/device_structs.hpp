@@ -69,16 +69,19 @@ struct DevChunk {              // one column chunk (row group x referenced colum
 
 // Flat store (flat_store.cuh): the scan-ready copy of one data page.
 enum FlatKind : uint8_t { FK_NONE = 0, FK_INDEX = 1, FK_PLAIN8 = 2, FK_BITS = 3, FK_BYTES = 4,
-                          FK_IDS = 5 };   // FK_IDS (per query): u32 group id per row of a GROUP BY column's page without a dictionary
+                          FK_IDS = 5,    // group id per row of a GROUP BY column: u32 for a page without a dictionary (per
+                                         // query), bit-packed at bits(card - 1) for a dictionary page (the table's agg pages)
+                          FK_FOR = 6 };  // value page of a numeric dictionary page: row value = base + bits (f64: / 10^e)
 struct FlatPageRec {           // parallel to pages[]
   uint64_t off;                // byte offset in the flat buffer, 16-byte aligned: one slot per ROW (NULL rows hold 0)
   uint64_t voff;               // validity bitmap (1 bit per row, LSB first like Arrow), or ~0: the page holds no NULLs
   uint32_t rows;
-  uint8_t bw;                  // FK_INDEX: bits per dictionary index; FK_BITS: 1
+  uint8_t bw;                  // FK_INDEX: bits per dictionary index; FK_BITS: 1; FK_IDS / FK_FOR: bits per row
   uint8_t fkind;               // FlatKind: FK_INDEX dictionary indices, FK_PLAIN8 8-byte values, FK_BITS boolean values,
                                // FK_BYTES PLAIN byte arrays: one u32 per row = where the row's bytes start, relative to `base`
-  uint16_t _pad;
-  uint64_t base;               // FK_BYTES: arena offset of the page's values section (a value's 4-byte length sits right before its bytes)
+  uint16_t dexp;               // FK_FOR of a Float64 column: the decimal exponent e
+  uint64_t base;               // FK_BYTES: arena offset of the page's values section (a value's 4-byte length sits right before its bytes);
+                               // FK_FOR: the frame of reference (the chunk's smallest value, or smallest k of a Float64 chunk)
 };
 
 struct DevItem {               // unit of CTA work: rows between two page boundaries common to all columns
@@ -220,7 +223,7 @@ struct DevPlan {
   uint32_t hashed;             // 1: the key space is wider than the dense table: group cells are found through DevScanArgs.hkeys
   uint32_t hmask;              // hashed: table capacity - 1 (nslots == capacity)
   uint32_t ndist;              // COUNT(DISTINCT) presence structures (distinct columns)
-  uint32_t _pad_dist;
+  uint32_t agg_forms;          // k_flat_agg: bit s = column slot s reads a page's agg page (DevScanArgs.apages) where it has one
   DevDistinct dist[kMaxAggs];
 };
 
@@ -239,6 +242,7 @@ struct DevScanArgs {
   const uint8_t* rg_live;      // per row group: 0 = pruned by statistics for this query (nullptr: all live)
   const uint8_t* flat;         // flat store (flat_store.cuh)
   const FlatPageRec* fpages;   // parallel to pages[]
+  const FlatPageRec* apages;   // the table's agg pages (Table::agg_pages), parallel to pages[]; read for plan.agg_forms slots
   uint32_t* bitmap;            // selection bitmap, per-item word regions
   uint32_t* item_counts;       // selected rows per item
   unsigned long long* acc;     // accumulator table (global)

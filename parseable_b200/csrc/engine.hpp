@@ -149,6 +149,21 @@ struct ColSide {
   uint64_t* d_row_ent = nullptr;       // where every row entry's value sits (relative to the arena, ~0: NULL / padding)
   struct KeyRowPage { uint32_t page; uint32_t ebase; };   // page index, first entry of its rows relative to n_dict_pad
   std::vector<KeyRowPage> key_row_pages;
+  // agg pages (Table::agg_pages): value pages of a numeric column's dictionary pages, or id pages of a GROUP BY key's.
+  // A page has one other form at most: the first one a query asks for stays.
+  bool for_ready = false;
+  uint8_t* d_for = nullptr;
+  uint32_t for_pages = 0;              // dictionary pages that have a value page
+  uint32_t for_bw = 0;                 // widest value page
+  uint32_t for_rest_bw = 0;            // widest index page left without one (chunks that do not qualify)
+  uint64_t for_bytes = 0;
+  // Id pages hold the LOCAL numbering (d_gid) only: it is fixed for the table's life, so the pages are built once and never
+  // rewritten under a query that reads them.  An agreed numbering (d_glob_gid) changes with every agreement of the ranks
+  // (unify_key), and a table may serve both numberings at the same time; its queries keep the gid LUT.
+  bool ids_ready = false;
+  uint8_t* d_ids = nullptr;
+  uint32_t ids_bw = 0;
+  uint64_t ids_bytes = 0;
 };
 
 // What a query needs per SET of referenced columns, built once per (table, column set): the chunk
@@ -219,6 +234,15 @@ class Table {
   // (shared: a query keeps the ranks it sorts with alive even if unify_key replaces them meanwhile)
   std::shared_ptr<const uint32_t> ensure_kd_rank(int tcol, bool agreed, cudaStream_t stream) const;
   void ensure_plain8(int tcol, cudaStream_t stream) const;   // DELTA_BINARY_PACKED pages -> row-addressable 8-byte values
+  // agg pages: a second flat page table parallel to pages[] (FK_NONE: the page has no other form), read by k_flat_agg's
+  // producer for the column slots a query marks.  ensure_for_pages: value pages of a numeric column; ensure_id_pages: id
+  // pages of a GROUP BY key in its local numbering (after ensure_key).  Both return false when the column has no such
+  // pages (no chunk qualifies, its pages hold the other form, or the device memory for them is not there: the agg pages
+  // are optional, the query then reads the index pages).  Records only ever go from FK_NONE to a form, once.
+  mutable std::vector<FlatPageRec> agg_pages;
+  mutable FlatPageRec* d_agg_pages = nullptr;
+  bool ensure_for_pages(int tcol, bool f64, cudaStream_t stream) const;
+  bool ensure_id_pages(int tcol, cudaStream_t stream) const;
 
  private:
   void build_flat_store(cudaStream_t stream);

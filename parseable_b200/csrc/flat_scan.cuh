@@ -85,7 +85,7 @@ struct FlatStageCol {
                                  // page at a row that is not a multiple of 128: the copy starts at the 16 bytes below)
   uint32_t vphase;               // the same for the validity bits
   uint32_t flags;                // kColHasValid: the page holds NULLs (validity staged); kColAbsent: column missing from the file
-  uint32_t _pad;
+  uint32_t dexp;                 // FK_FOR of a Float64 column: decimal exponent (dict8 then carries the page's base)
 };
 struct FlatStage {
   uint32_t item;                 // 0xffffffff: the queue is empty, consumers leave
@@ -159,10 +159,15 @@ __device__ __noinline__ void flat_producer(const DevPlan& plan, const FlatLayout
         mycol.flags = kColAbsent;
         mycol.fkind = FK_NONE;
       } else {
-        const FlatPageRec fp = a.fpages[item.page[lane]];
+        FlatPageRec fp = a.fpages[item.page[lane]];
+        if ((plan.agg_forms >> lane) & 1u) {   // the page's agg page, where it has one (value page / id page)
+          const FlatPageRec ap = a.apages[item.page[lane]];
+          if (ap.fkind != FK_NONE) fp = ap;
+        }
         mycol.bw = fp.bw;
         mycol.fkind = fp.fkind;
         if (fp.fkind == FK_BYTES) mycol.dict8 = fp.base;   // PLAIN byte arrays: arena offset of the page's values section
+        if (fp.fkind == FK_FOR) { mycol.dict8 = fp.base; mycol.dexp = fp.dexp; }   // value pages: the frame of reference
         mysrc = fp.off;
         mypoff = item.poff[lane];
         if (fp.voff != ~0ull) { mycol.flags = kColHasValid; myvsrc = fp.voff; }
@@ -286,14 +291,16 @@ __device__ __forceinline__ bool col_valid(const ColCtx& c, uint32_t row) {
 }
 
 // GROUP BY id of one non-NULL row (the key pass of k_flat_agg and its COUNT(DISTINCT) pass): a boolean's bit, the
-// staged id of a page without a dictionary (FK_IDS), or the gid LUT entry of the row's dictionary index
-// (`gid` already points at the chunk's lut_base)
+// staged id of an id page (FK_IDS: u32 ids of a page without a dictionary, or a dictionary page's agg page at
+// bits(card - 1) bits), or the gid LUT entry of the row's dictionary index (`gid` already points at the chunk's lut_base)
 __device__ __forceinline__ uint32_t row_id_bool(const ColCtx& c, uint32_t row) {
   const uint32_t pb = c.phase + row;
   return (c.colw[pb >> 5] >> (pb & 31)) & 1u;
 }
+// PACKED = false: u32 ids only (the COUNT(DISTINCT) instantiations, whose queries get no agg pages)
+template <bool PACKED = true>
 __device__ __forceinline__ uint32_t row_id_ids(const ColCtx& c, uint32_t card, uint32_t row) {
-  const uint32_t g = bits32_at(c.colw, c.phase + row * 32u);
+  const uint32_t g = PACKED ? bits32_at(c.colw, c.phase + row * c.bw) & c.mask : bits32_at(c.colw, c.phase + row * 32u);
   return g < card ? g : card - 1u;   // never out of the table
 }
 __device__ __forceinline__ uint32_t row_id_lut(const ColCtx& c, const uint32_t* __restrict__ gid, uint32_t row) {
@@ -301,7 +308,7 @@ __device__ __forceinline__ uint32_t row_id_lut(const ColCtx& c, const uint32_t* 
 }
 __device__ __forceinline__ uint32_t row_id(const ColCtx& c, bool is_bool, const uint32_t* __restrict__ gid, uint32_t card, uint32_t row) {
   if (is_bool) return row_id_bool(c, row);
-  if (c.fkind == FK_IDS) return row_id_ids(c, card, row);
+  if (c.fkind == FK_IDS) return row_id_ids<false>(c, card, row);   // COUNT(DISTINCT) columns never read agg pages
   return row_id_lut(c, gid, row);
 }
 
@@ -963,7 +970,7 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
               if ((sel >> i) & 1u) {
                 const uint32_t r = tc + i * kAggConsumers;
                 if (nullable && !col_valid(c, r)) { slot[i] += nullslot; continue; }
-                slot[i] += row_id_ids(c, key.card, r) * stride;
+                slot[i] += row_id_ids<!DIST>(c, key.card, r) * stride;
               }
           } else if (!nullable) {   // the loads of all rows in flight together
             uint32_t g[KR];
@@ -1044,9 +1051,21 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
         // the values first (all loads in flight together: a dictionary value is an L2 round trip), then the updates,
         // one straight-line loop per aggregate function
         uint64_t bits[KR];
+        // a value page (FK_FOR): the values are in the stage, no load at all.  Not in the COUNT(DISTINCT) instantiations
+        // (the planner gives those queries no agg pages): there it spilled registers at the 64-register cap
         if (plain) {
 #pragma unroll
           for (int i = 0; i < KR; i++) bits[i] = ((vsel >> i) & 1u) ? __ldg(v8 + tc + i * kAggConsumers) : 0ull;   // in place in the flat store (global)
+        } else if (!DIST && c.fkind == FK_FOR) {
+          const int64_t fbase = int64_t(st.col[ag.col].dict8);
+#pragma unroll
+          for (int i = 0; i < KR; i++)
+            bits[i] = uint64_t(for_decode(fbase, bits32_at(c.colw, c.phase + (tc + i * kAggConsumers) * c.bw) & c.mask));
+          if (f64) {
+            const DecScale p10 = dec_scale(st.col[ag.col].dexp);
+#pragma unroll
+            for (int i = 0; i < KR; i++) bits[i] = dec_decode_f64(int64_t(bits[i]), p10);
+          }
         } else {
 #pragma unroll
           for (int i = 0; i < KR; i++) bits[i] = ((vsel >> i) & 1u) ? __ldg(dict + col_index(c, tc + i * kAggConsumers)) : 0ull;

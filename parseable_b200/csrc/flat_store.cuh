@@ -20,6 +20,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <climits>
+
 #include "decode_core.cuh"
 #include "device_structs.hpp"
 
@@ -385,6 +387,116 @@ __global__ void __launch_bounds__(128) k_check_flat_indices(const uint8_t* __res
   bool bad = false;
   for (uint32_t i = lane; i < fp.rows; i += 32) bad |= (bits32_at(w, i * fp.bw) & mask) >= limit;
   if (__any_sync(0xffffffffu, bad) && lane == 0) atomicMin(first_bad, pi);
+}
+
+// ---- agg pages: what k_flat_agg reads instead of a dictionary index when the index only ever looks something up ----
+// Built once per table column (Table::ensure_for_pages / ensure_id_pages) and kept with the table:
+//   FK_FOR  value page of a numeric dictionary page: base + w-bit offset per row (decode_core.cuh: for_* / dec_*)
+//   FK_IDS  id page of a GROUP BY key's dictionary page: the row's group id at bits(card - 1) bits
+// Both follow the flat store's conventions: 16-byte aligned, row r at bits [r*w, (r+1)*w), NULL rows hold 0, the index
+// page's validity bitmap is reused.
+struct ForChunkJob { uint64_t dict8; uint32_t n; uint32_t f64; };
+struct ForChunkInfo { int64_t base; uint32_t w; uint32_t e; uint32_t ok; uint32_t _pad; };
+
+template <typename T, typename Op>
+__device__ __forceinline__ T block_reduce_256(T v, T* s, Op op) {   // 256 threads; s holds 8 T
+  for (int o = 16; o; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = v;
+  __syncthreads();
+  v = s[0];
+  for (int w = 1; w < 8; w++) v = op(v, s[w]);
+  return v;
+}
+
+// One block per chunk: can every dictionary entry be written as base + w bits (w <= 32)?  Float64: the smallest decimal
+// exponent e at which every entry has its k.
+__global__ void __launch_bounds__(256) k_for_classify(const uint8_t* __restrict__ flat, const ForChunkJob* __restrict__ jobs,
+                                                      ForChunkInfo* __restrict__ out) {
+  __shared__ long long s_ll[8];
+  __shared__ uint32_t s_u[8];
+  const ForChunkJob j = jobs[blockIdx.x];
+  const uint64_t* __restrict__ d = reinterpret_cast<const uint64_t*>(flat + j.dict8);
+  uint32_t e = 0;
+  if (j.f64) {
+    uint32_t fail = 0;   // bit e: some entry has no k at exponent e
+    for (uint32_t i = threadIdx.x; i < j.n && fail != (2u << kForMaxExp) - 1u; i += 256) {
+      const uint64_t b = d[i];
+      for (uint32_t x = 0; x <= kForMaxExp; x++) {
+        int64_t k;
+        if (!((fail >> x) & 1u) && !dec_encode_f64(b, dec_scale(x), k)) fail |= 1u << x;
+      }
+    }
+    fail = block_reduce_256<uint32_t>(fail, s_u, [](uint32_t a, uint32_t b) { return a | b; });
+    e = __ffs(~fail) - 1;
+    if (e > kForMaxExp) {
+      if (threadIdx.x == 0) out[blockIdx.x] = ForChunkInfo{0, 0, 0, 0, 0};
+      return;
+    }
+  }
+  const DecScale p10 = dec_scale(e);
+  long long lo = LLONG_MAX, hi = LLONG_MIN;
+  for (uint32_t i = threadIdx.x; i < j.n; i += 256) {
+    int64_t k = int64_t(d[i]);
+    if (j.f64) dec_encode_f64(d[i], p10, k);
+    lo = k < lo ? k : lo;
+    hi = k > hi ? k : hi;
+  }
+  __syncthreads();
+  lo = block_reduce_256<long long>(lo, s_ll, [](long long a, long long b) { return a < b ? a : b; });
+  __syncthreads();
+  hi = block_reduce_256<long long>(hi, s_ll, [](long long a, long long b) { return a > b ? a : b; });
+  if (threadIdx.x == 0) {
+    const uint32_t w = j.n ? bit_width_u64(for_encode(hi, lo)) : 0u;
+    out[blockIdx.x] = ForChunkInfo{j.n ? lo : 0, w, e, (j.n && w <= kForMaxBits) ? 1u : 0u, 0};
+  }
+}
+
+enum AggFormKind : uint32_t { AF_I64 = 0, AF_F64 = 1, AF_IDS = 2 };
+struct AggFormJob {
+  uint64_t src;      // the FK_INDEX page (flat offset)
+  uint64_t dst;      // its agg page (flat offset, may wrap: a buffer of its own)
+  uint64_t voff;     // validity bitmap of the index page, or ~0
+  uint64_t table;    // AF_I64 / AF_F64: the chunk's 8-byte dictionary (flat offset); AF_IDS: device address of gid + lut_base
+  int64_t base;
+  uint32_t rows, sbw, dict_n, w, e, kind;
+};
+// One warp per page; a lane writes whole groups of 32 rows = w words, so no word is shared between lanes.
+__global__ void __launch_bounds__(128) k_agg_form_pack(uint8_t* __restrict__ flat, const AggFormJob* __restrict__ jobs, uint32_t n_jobs) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t ji = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (ji >= n_jobs) return;
+  const AggFormJob j = jobs[ji];
+  const uint32_t* __restrict__ src = reinterpret_cast<const uint32_t*>(flat + j.src);
+  const uint32_t* __restrict__ valid = j.voff != ~0ull ? reinterpret_cast<const uint32_t*>(flat + j.voff) : nullptr;
+  const uint64_t* __restrict__ dict = reinterpret_cast<const uint64_t*>(flat + j.table);
+  const uint32_t* __restrict__ gid = reinterpret_cast<const uint32_t*>(j.table);
+  uint32_t* __restrict__ dst = reinterpret_cast<uint32_t*>(flat + j.dst);
+  const uint32_t smask = j.sbw >= 32 ? 0xffffffffu : ((1u << j.sbw) - 1u), dict_max = j.dict_n ? j.dict_n - 1 : 0u;
+  const DecScale p10 = dec_scale(j.e);
+  for (uint32_t g = lane; g * 32 < j.rows; g += 32) {
+    const uint32_t vw = valid ? valid[g] : 0xffffffffu;
+    uint32_t* out = dst + size_t(g) * j.w;
+    uint64_t acc = 0;
+    uint32_t nacc = 0;
+    for (uint32_t k = 0; k < 32; k++) {
+      const uint32_t r = g * 32 + k;
+      uint32_t x = 0;
+      if (r < j.rows && ((vw >> k) & 1u)) {
+        uint32_t idx = j.sbw ? (bits32_at(src, r * j.sbw) & smask) : 0u;
+        idx = idx < dict_max ? idx : dict_max;   // as col_index: a corrupt index never leaves the dictionary
+        if (j.kind == AF_IDS) x = gid[idx];
+        else {
+          int64_t v = int64_t(dict[idx]);
+          if (j.kind == AF_F64) dec_encode_f64(dict[idx], p10, v);   // succeeds: k_for_classify tried every entry
+          x = uint32_t(for_encode(v, j.base));
+        }
+      }
+      acc |= uint64_t(x) << nacc;
+      nacc += j.w;
+      if (nacc >= 32) { *out++ = uint32_t(acc); acc >>= 32; nacc -= 32; }
+    }
+  }
 }
 
 // ---- DELTA_BINARY_PACKED (Parseable's p_timestamp, streams.rs:587-590) -> aligned 8-byte values ----

@@ -267,6 +267,143 @@ void launch_delta_to_plain8(const uint8_t* arena, const DevPage* pages, const vo
   PQB_CUDA(cudaGetLastError());
 }
 
+// ---- agg pages (flat_store.cuh): built once per table column, kept with the table (callers hold side_mu) ----
+// Packs the jobs into one new buffer (returned; offsets relative to d_flat like every flat page) and records each page's
+// new form in the table's agg page table.  The agg pages are optional: when the device memory for them is not there,
+// nothing is recorded, nullptr comes back and the column keeps reading its index pages.
+static bool try_alloc(void** p, size_t bytes, cudaStream_t stream) {
+  if (cudaMallocAsync(p, bytes, stream) == cudaSuccess) return true;
+  (void)cudaGetLastError();   // an allocation failure is not sticky: clear it, the query goes on without this form
+  *p = nullptr;
+  return false;
+}
+static uint8_t* build_agg_pages(const Table& t, std::vector<AggFormJob>& jobs, const std::vector<uint32_t>& page_of, uint8_t fkind,
+                                uint64_t& bytes, cudaStream_t stream) {
+  if (!t.d_agg_pages) {   // first agg pages of the table: the whole page table, every record FK_NONE (nobody reads it yet)
+    FlatPageRec blank{};
+    blank.voff = ~0ull;
+    t.agg_pages.assign(t.pages.size(), blank);
+    if (!try_alloc((void**)&t.d_agg_pages, t.agg_pages.size() * sizeof(FlatPageRec), stream)) return nullptr;
+    PQB_CUDA(cudaMemcpyAsync(t.d_agg_pages, t.agg_pages.data(), t.agg_pages.size() * sizeof(FlatPageRec), cudaMemcpyHostToDevice, stream));
+  }
+  uint64_t off = 0;
+  for (AggFormJob& j : jobs) {
+    j.dst = off;
+    off += (((uint64_t(j.rows) + 31) / 32) * j.w * 4 + 15) & ~15ull;
+  }
+  uint8_t* buf = nullptr;
+  AggFormJob* dj = nullptr;
+  if (!try_alloc((void**)&buf, off + 64, stream)) return nullptr;   // + the over-read of a slab's last staged word
+  if (!try_alloc((void**)&dj, jobs.size() * sizeof(AggFormJob), stream)) {
+    PQB_CUDA(cudaFreeAsync(buf, stream));
+    return nullptr;
+  }
+  const uint64_t rel = uint64_t(buf) - uint64_t(t.d_flat);      // the subtraction may wrap, d_flat + offset does not
+  for (AggFormJob& j : jobs) j.dst += rel;
+  PQB_CUDA(cudaMemcpyAsync(dj, jobs.data(), jobs.size() * sizeof(AggFormJob), cudaMemcpyHostToDevice, stream));
+  k_agg_form_pack<<<uint32_t((jobs.size() + 3) / 4), 128, 0, stream>>>(t.d_flat, dj, uint32_t(jobs.size()));
+  PQB_CUDA(cudaGetLastError());
+  PQB_CUDA(cudaFreeAsync(dj, stream));
+  for (size_t i = 0; i < jobs.size(); i++) {
+    const AggFormJob& j = jobs[i];
+    FlatPageRec& r = t.agg_pages[page_of[i]];
+    r = t.flat_pages[page_of[i]];
+    r.off = j.dst;
+    r.bw = uint8_t(j.w);
+    r.fkind = fkind;
+    r.dexp = uint16_t(j.e);
+    r.base = uint64_t(j.base);
+  }
+  // only the records of this column's pages go up (runs of consecutive pages): a query running on another stream reads
+  // the table's other records, and those are never written again
+  for (size_t i = 0; i < page_of.size();) {
+    size_t e = i + 1;
+    while (e < page_of.size() && page_of[e] == page_of[e - 1] + 1) e++;
+    PQB_CUDA(cudaMemcpyAsync(t.d_agg_pages + page_of[i], t.agg_pages.data() + page_of[i], (e - i) * sizeof(FlatPageRec),
+                             cudaMemcpyHostToDevice, stream));
+    i = e;
+  }
+  PQB_CUDA(cudaStreamSynchronize(stream));
+  bytes = off;
+  return buf;
+}
+
+bool Table::ensure_for_pages(int tcol, bool f64, cudaStream_t stream) const {
+  std::lock_guard<std::mutex> lk(side_mu);
+  ColSide& cs = sides[tcol];
+  if (cs.for_ready || cs.d_ids) return cs.for_pages != 0;
+  cs.for_ready = true;
+  // one classification per chunk with a numeric dictionary copy
+  std::vector<ForChunkJob> cj;
+  std::vector<int> info_of(row_groups.size(), -1);
+  for (size_t g = 0; g < row_groups.size(); g++) {
+    const TableChunk& tc = row_groups[g].chunks[tcol];
+    if (!tc.present || tc.dict8_off == ~0ull || !tc.dict_n) continue;
+    info_of[g] = int(cj.size());
+    cj.push_back(ForChunkJob{tc.dict8_off, tc.dict_n, f64 ? 1u : 0u});
+  }
+  std::vector<ForChunkInfo> info(cj.size());
+  if (!cj.empty()) {
+    DevBuf<ForChunkJob> dj;
+    dj.upload(cj, stream);
+    DevBuf<ForChunkInfo> di;
+    di.alloc(cj.size(), stream);
+    k_for_classify<<<uint32_t(cj.size()), 256, 0, stream>>>(d_flat, dj.p, di.p);
+    PQB_CUDA(cudaGetLastError());
+    PQB_CUDA(cudaMemcpyAsync(info.data(), di.p, info.size() * sizeof(ForChunkInfo), cudaMemcpyDeviceToHost, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+  }
+  std::vector<AggFormJob> jobs;
+  std::vector<uint32_t> page_of;
+  uint32_t w_max = 0, rest_bw = 0;
+  for (size_t g = 0; g < row_groups.size(); g++) {
+    const TableChunk& tc = row_groups[g].chunks[tcol];
+    if (!tc.present) continue;
+    const ForChunkInfo* fi = info_of[g] >= 0 ? &info[info_of[g]] : nullptr;
+    for (uint32_t k = 0; k < tc.pages.n_pages; k++) {
+      const uint32_t pi = tc.pages.first_page + k;
+      const FlatPageRec& fr = flat_pages[pi];
+      if (fr.fkind != FK_INDEX) continue;
+      if (!fi || !fi->ok) { rest_bw = std::max<uint32_t>(rest_bw, fr.bw); continue; }
+      jobs.push_back(AggFormJob{fr.off, 0, fr.voff, tc.dict8_off, fi->base, fr.rows, fr.bw, tc.dict_n, fi->w, fi->e, f64 ? AF_F64 : AF_I64});
+      page_of.push_back(pi);
+      w_max = std::max(w_max, fi->w);
+    }
+  }
+  if (jobs.empty()) return false;
+  cs.d_for = build_agg_pages(*this, jobs, page_of, FK_FOR, cs.for_bytes, stream);
+  if (!cs.d_for) return false;
+  cs.for_bw = w_max;
+  cs.for_rest_bw = rest_bw;
+  cs.for_pages = uint32_t(jobs.size());
+  return true;
+}
+
+bool Table::ensure_id_pages(int tcol, cudaStream_t stream) const {
+  std::lock_guard<std::mutex> lk(side_mu);
+  ColSide& cs = sides[tcol];
+  if (cs.ids_ready || cs.for_pages) return cs.d_ids != nullptr;
+  cs.ids_ready = true;   // one attempt: without the memory for them, the column keeps its gid LUT
+  const uint32_t w = bit_width_u64(cs.card ? cs.card - 1u : 0u);
+  std::vector<AggFormJob> jobs;
+  std::vector<uint32_t> page_of;
+  for (size_t g = 0; g < row_groups.size(); g++) {
+    const TableChunk& tc = row_groups[g].chunks[tcol];
+    if (!tc.present) continue;
+    for (uint32_t k = 0; k < tc.pages.n_pages; k++) {
+      const uint32_t pi = tc.pages.first_page + k;
+      const FlatPageRec& fr = flat_pages[pi];
+      if (fr.fkind != FK_INDEX) continue;
+      jobs.push_back(AggFormJob{fr.off, 0, fr.voff, uint64_t(cs.d_gid + cs.base_per_rg[g]), 0, fr.rows, fr.bw, tc.dict_n, w, 0, AF_IDS});
+      page_of.push_back(pi);
+    }
+  }
+  if (jobs.empty()) return false;
+  cs.d_ids = build_agg_pages(*this, jobs, page_of, FK_IDS, cs.ids_bytes, stream);
+  cs.ids_bw = w;
+  return cs.d_ids != nullptr;
+}
+
 void launch_entry_offsets(const Table& t, int tcol, uint64_t* d_out, uint32_t* max_len, cudaStream_t stream) {
   std::vector<EntChunk> ch = column_chunks(t, tcol);
   if (ch.empty()) return;
@@ -1456,6 +1593,52 @@ void Query::run(const PqQueryDesc& d) {
       metrics.h2d_bytes += fp.size() * sizeof(FlatPageRec);
     }
   }
+  // ---- agg pages (k_flat_agg): a column slot whose every use in this query only looks its dictionary index up -- as
+  // an aggregate input (value pages) or as a GROUP BY key (id pages) -- reads the table's agg pages instead, and its rows
+  // need no dictionary or gid LUT load.  They are built once per column and kept with the table, so only a resident
+  // table gets them: a file list opens its table for one query, which would pay the build every time ----
+  std::vector<uint32_t> form_bw(ncols, 0);   // marked slots: widest page the slot stages
+  plan.agg_forms = 0;
+  {
+    const char* sw = getenv("PQB_AGG_FORMS");   // A/B switch: 0 = every slot reads its index pages
+    // not with COUNT(DISTINCT): its kernel instantiations carry no agg-page paths (their registers would spill there)
+    if (!(sw && sw[0] == '0') && agg_kernel && n_flat && d.table && !plan.ndist) {
+      for (uint32_t s = 0; s < ncols; s++) {
+        bool as_key = false, as_value = false, other = false;
+        for (uint32_t l = 0; l < nleaves; l++) other |= plan.leaves[l].col == s;
+        int key = -1;
+        for (uint32_t k = 0; k < d.n_group_by; k++)
+          if (plan.keys[k].col == s) {
+            if (plan.keys[k].kind == KK_DICT_LUT) { as_key = true; key = int(k); }
+            else other = true;   // KK_BIN reads the values, KK_BOOL has no dictionary
+          }
+        for (uint32_t a = 0; a < d.n_aggs; a++) {
+          const DevAgg& ag = plan.aggs[a];
+          if (ag.fn == AG_COUNT_STAR || ag.col != s) continue;
+          if (ag.fn == AG_COUNT_DISTINCT) other = true;
+          else if (ag.fn >= AG_SUM && ag.fn <= AG_AVG) as_value = true;   // COUNT(col) reads the validity bits only: any form serves it
+        }
+        if (other || as_key == as_value) continue;
+        const int tc_i = shape_cols[s];
+        const ColSide& cs = table->sides[tc_i];
+        if (as_value) {
+          const uint8_t kind = plan.cols[s].kind;
+          if ((kind != DK_I64 && kind != DK_F64) || !table->ensure_for_pages(tc_i, kind == DK_F64, stream)) continue;
+          form_bw[s] = std::max(cs.for_bw, cs.for_rest_bw);
+        } else {
+          // id pages hold the local numbering: a query in the ranks' agreed numbering keeps the gid LUT
+          if (plan.keys[key].gid != cs.d_gid || !table->ensure_id_pages(tc_i, stream)) continue;
+          form_bw[s] = std::max(cs.ids_bw, key_bw32[s]);
+        }
+        plan.agg_forms |= 1u << s;
+        if (verbose)
+          fprintf(stderr, "[pqb] slot %u (%s): %s pages, %u bits, staged at %u bits (index pages: %u), %.1f MB held by the table\n", s,
+                  table->columns[tc_i].name.c_str(), as_value ? "value" : "id", as_value ? cs.for_bw : cs.ids_bw, form_bw[s],
+                  std::max(shape->flat_max_bw[s], key_bw32[s]),
+                  double(as_value ? cs.for_bytes : cs.ids_bytes) / 1e6);
+      }
+    }
+  }
   mark("side tables ready");
   // ---- shared-memory layout of k_scan (items the flat kernels do not take) ----
   SmemLayout L{};
@@ -1511,7 +1694,8 @@ void Query::run(const PqQueryDesc& d) {
         FL.col_off[s] = off;
         FL.col_voff[s] = off;
         if (!plan.cols[s].staged) continue;
-        const uint32_t cap = std::max<uint32_t>((shape->flat_plain8[s] && !plan.direct8) ? S * 8 : 0, (S * std::max(shape->flat_max_bw[s], key_bw32[s]) + 7) / 8);
+        const uint32_t bw = ((plan.agg_forms >> s) & 1u) ? form_bw[s] : std::max(shape->flat_max_bw[s], key_bw32[s]);
+        const uint32_t cap = std::max<uint32_t>((shape->flat_plain8[s] && !plan.direct8) ? S * 8 : 0, (S * bw + 7) / 8);
         off += align_up(cap + 48, 128);   // + the bit phase of a piece that starts inside a page, + over-read slack
         if (shape->flat_nullable[s]) { FL.col_voff[s] = off; off += align_up(S / 8 + 48, 128); }   // validity bits of pages with NULLs
       }
@@ -1663,6 +1847,7 @@ void Query::run(const PqQueryDesc& d) {
   sa.rg_live = pruned ? d_live.p : nullptr;
   sa.flat = table->d_flat;
   sa.fpages = d_kpages.p ? d_kpages.p : table->d_flat_pages;
+  sa.apages = plan.agg_forms ? table->d_agg_pages : nullptr;
   sa.bitmap = d_bitmap.p;
   sa.item_counts = d_item_counts.p;
   sa.acc = d_acc.p;

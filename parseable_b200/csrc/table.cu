@@ -245,7 +245,10 @@ Table::~Table() {
   if (d_strmat) cudaFreeAsync(d_strmat, cudaStreamPerThread);
   if (d_flat) cudaFreeAsync(d_flat, cudaStreamPerThread);
   if (d_flat_pages) cudaFreeAsync(d_flat_pages, cudaStreamPerThread);
+  if (d_agg_pages) cudaFreeAsync(d_agg_pages, cudaStreamPerThread);
   for (ColSide& cs : sides) {
+    if (cs.d_for) cudaFreeAsync(cs.d_for, cudaStreamPerThread);
+    if (cs.d_ids) cudaFreeAsync(cs.d_ids, cudaStreamPerThread);
     if (cs.d_ent_off) cudaFreeAsync(cs.d_ent_off, cudaStreamPerThread);
     if (cs.d_gid) cudaFreeAsync(cs.d_gid, cudaStreamPerThread);
     if (cs.d_row_ent) cudaFreeAsync(cs.d_row_ent, cudaStreamPerThread);

@@ -91,6 +91,17 @@ int64_t dc_decode_delta(const uint8_t* stream, uint64_t len, uint32_t n, uint32_
   }
   return done;
 }
+// value pages: 1 and k when `bits` has an integer k at decimal exponent e, 0 when it refuses
+int dc_dec_encode_f64(uint64_t bits, uint32_t e, int64_t* k) { return dec_encode_f64(bits, dec_scale(e), *k) ? 1 : 0; }
+uint64_t dc_dec_decode_f64(int64_t k, uint32_t e) { return dec_decode_f64(k, dec_scale(e)); }
+// n values at once (k[i] / 10^e -> out[i]): the tests compare millions of them with IEEE division
+void dc_dec_decode_many(const int64_t* k, uint64_t n, uint32_t e, uint64_t* out) {
+  const DecScale s = dec_scale(e);
+  for (uint64_t i = 0; i < n; i++) out[i] = dec_decode_f64(k[i], s);
+}
+uint64_t dc_for_encode(int64_t v, int64_t base) { return for_encode(v, base); }
+int64_t dc_for_decode(int64_t base, uint32_t bits) { return for_decode(base, bits); }
+uint32_t dc_bit_width(uint64_t x) { return bit_width_u64(x); }
 int64_t dc_f64_key(uint64_t bits) { return f64_order_key(bits); }
 uint64_t dc_f64_from_key(int64_t k) { return f64_from_order_key(k); }
 int dc_like(const uint8_t* s, uint32_t n, const uint8_t* p, uint32_t m, uint32_t kind, int ci) {

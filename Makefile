@@ -38,8 +38,8 @@ oracle/liboracle.so: oracle/oracle.c
 	$(CC) -O2 -std=c11 -fPIC -shared -Wall -o $@ $< -lm
 
 tools: tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so
-tools/liborder_keys_host.so: tools/order_keys_host.cpp $(CSRC)/order_keys.cuh $(CSRC)/decode_core.cuh $(CSRC)/device_structs.hpp
-	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
+tools/liborder_keys_host.so: tools/order_keys_host.cpp $(CSRC)/order_keys.cuh $(CSRC)/percentile_core.cuh $(CSRC)/decode_core.cuh $(CSRC)/device_structs.hpp
+	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 tools/libjson_host.so: tools/json_host.cpp $(CSRC)/json_egress.cuh $(CSRC)/ryu_f64.cuh $(CSRC)/ryu_tables.inc
 	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -Wno-maybe-uninitialized -I$(CSRC) -o $@ $<
 tools/libzstd_host.so: tools/zstd_host.cpp $(CSRC)/zstd_decode.cuh $(CSRC)/inflate_decode.cuh

@@ -149,7 +149,27 @@ typedef enum {
    * distinct as GROUP BY keys are: strings by bytes, integers / timestamps / booleans by value, Float64 by bit
    * pattern (-0.0 and 0.0 differ, as do NaNs with different payloads).  Utf8, Int64, Timestamp(ms), Float64 and
    * Boolean columns; refused (PQ_ERR_UNSUPPORTED) under PQ_QUERY_ALLREDUCE. */
-  PQ_AGG_COUNT_DISTINCT = 6
+  PQ_AGG_COUNT_DISTINCT = 6,
+  /* Exact order statistics (DataFusion's median / percentile_cont, restated from DataFusion 53; its crates are not
+   * vendored here, so the rules are restated, not checked).  Int64 and Float64 inputs (dictionary or PLAIN pages); Utf8,
+   * Boolean and Timestamp inputs return PQ_ERR_UNSUPPORTED.  NULL inputs are ignored and a column missing from a file
+   * reads as NULL; a group with no non-NULL input gets NULL (a global aggregate over zero rows: one row holding NULL).
+   * Values are sorted as ORDER BY sorts them: Int64 signed, Float64 by IEEE totalOrder (-NaN < -inf < ... < -0.0 < +0.0
+   * < ... < +inf < +NaN).
+   *   MEDIAN: output type = input type, named "median(<col>)".  n odd: the middle value.  n even: Int64 (lo + hi) as a
+   *     wrapping i64 add, then / 2 truncating toward zero (add_wrapping(..).div_wrapping(2): the median of two values
+   *     near INT64_MAX wraps); Float64 (lo + hi) / 2.
+   *   PERCENTILE_CONT: p = agg_params[i] (finite, in [0, 1]); output Float64, named "percentile_cont(<col>, <p>)" with p
+   *     in shortest round-trip form (std::to_chars: 0, 0.5, 0.95, 1).  h = p * (n - 1), lo = floor(h), f = h - lo over
+   *     the sorted values as f64: v[lo] when f == 0, else v[lo] + f * (v[lo + 1] - v[lo]).
+   * Float64 arithmetic on NaN follows x86-64 SSE (a NaN operand comes back quieted, the first one when both are NaN;
+   * inf - inf is the default NaN 0xfff8000000000000), so the device and a CPU agree bit for bit.
+   * Several of them over one column share one set of values and one sort.  They combine with every other aggregate but
+   * COUNT(DISTINCT) (together: PQ_ERR_UNSUPPORTED), with every GROUP BY form and with ORDER BY.  PQ_QUERY_ALLREDUCE or
+   * more than 2^32 - 1 values of one column: PQ_ERR_UNSUPPORTED; value and sort buffers above half the free HBM:
+   * PQ_ERR_OOM. */
+  PQ_AGG_MEDIAN = 7,
+  PQ_AGG_PERCENTILE_CONT = 8
 } PqAggFn;
 
 typedef struct {
@@ -262,6 +282,10 @@ typedef struct {
   const PqOrderBy* order_by;
   uint32_t n_order_by;
   uint32_t _pad2;
+
+  /* NULL, or n_aggs entries: a parameter per aggregate.  Only PQ_AGG_PERCENTILE_CONT reads its entry, the fraction p
+   * (finite, in [0, 1]; otherwise, or NULL here, the call returns PQ_ERR_INVALID_ARG) */
+  const double* agg_params;
 } PqQueryDesc;
 
 #define PQ_QUERY_COUNT_ONLY 1u    /* filter scan: only rows_selected is wanted, emit no batches */
@@ -287,6 +311,8 @@ typedef struct {
   uint64_t groups_total;    /* aggregate queries: groups before the ORDER BY ... LIMIT cut (== groups without ORDER BY) */
   double order_ms;          /* CUDA-event time of the ORDER BY kernels, without the one host round trip between them
                                (0 without ORDER BY) */
+  double percentile_ms;     /* CUDA-event time of the MEDIAN / PERCENTILE_CONT kernels (sort and pick), without the host round
+                               trip of each sort (0 without them) */
 } PqMetrics;
 
 /* ---- lifecycle ---- */

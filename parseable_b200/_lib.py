@@ -23,7 +23,8 @@ PQ_T_NULL, PQ_T_BOOL, PQ_T_I64, PQ_T_F64, PQ_T_UTF8, PQ_T_TS_MS = range(6)
 PQ_OP_CMP, PQ_OP_IS_NULL, PQ_OP_IS_NOT_NULL, PQ_OP_LIKE, PQ_OP_AND, PQ_OP_OR, PQ_OP_NOT, PQ_OP_CONST = range(1, 9)
 PQ_EQ, PQ_NE, PQ_LT, PQ_LE, PQ_GT, PQ_GE = range(6)
 PQ_LIKE_NEGATED, PQ_LIKE_CASE_INSENSITIVE = 1, 2
-PQ_AGG_COUNT_STAR, PQ_AGG_COUNT, PQ_AGG_SUM, PQ_AGG_MIN, PQ_AGG_MAX, PQ_AGG_AVG, PQ_AGG_COUNT_DISTINCT = range(7)
+(PQ_AGG_COUNT_STAR, PQ_AGG_COUNT, PQ_AGG_SUM, PQ_AGG_MIN, PQ_AGG_MAX, PQ_AGG_AVG, PQ_AGG_COUNT_DISTINCT, PQ_AGG_MEDIAN,
+ PQ_AGG_PERCENTILE_CONT) = range(9)
 PQ_QUERY_COUNT_ONLY, PQ_QUERY_ALLREDUCE, PQ_QUERY_EMIT_ROW_IDS = 1, 2, 4
 PQ_JSON_LINES = 1
 PQ_COMM_ID_BYTES = 128
@@ -75,6 +76,7 @@ class PqQueryDesc(C.Structure):
         ("shard_index", C.c_uint32), ("shard_count", C.c_uint32), ("flags", C.c_uint32),
         ("group_exprs", C.POINTER(PqKeyExpr)),
         ("order_by", C.POINTER(PqOrderBy)), ("n_order_by", C.c_uint32), ("_pad2", C.c_uint32),
+        ("agg_params", C.POINTER(C.c_double)),
     ]
 
 
@@ -116,7 +118,7 @@ class PqMetrics(C.Structure):
         ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("kernel_launches", C.c_uint64),
         ("device_ms", C.c_double), ("scan_kernel_ms", C.c_double), ("groups", C.c_uint64),
         ("host_ms", C.c_double), ("upload_ms", C.c_double), ("allreduce_ms", C.c_double),
-        ("groups_total", C.c_uint64), ("order_ms", C.c_double),
+        ("groups_total", C.c_uint64), ("order_ms", C.c_double), ("percentile_ms", C.c_double),
     ]
 
     def as_dict(self) -> dict:

@@ -138,7 +138,8 @@ struct DevLeaf {
 enum DevPredKind : uint8_t { PK_LEAF = 1, PK_AND = 2, PK_OR = 3, PK_NOT = 4, PK_CONST = 5 };
 struct DevPredOp { uint8_t kind; uint8_t arg; /* leaf id, or const: 0 F, 1 T, 2 NULL */ };
 
-enum DevAggFn : uint8_t { AG_COUNT_STAR = 0, AG_COUNT = 1, AG_SUM = 2, AG_MIN = 3, AG_MAX = 4, AG_AVG = 5, AG_COUNT_DISTINCT = 6 };
+enum DevAggFn : uint8_t { AG_COUNT_STAR = 0, AG_COUNT = 1, AG_SUM = 2, AG_MIN = 3, AG_MAX = 4, AG_AVG = 5, AG_COUNT_DISTINCT = 6,
+                          AG_MEDIAN = 7, AG_PERCENTILE_CONT = 8 };
 struct DevAgg {
   uint8_t fn;
   uint8_t col;       // column slot
@@ -146,8 +147,20 @@ struct DevAgg {
   uint8_t acc_slot;  // which 8-byte accumulator array (COUNT(DISTINCT): the per-group count of first sightings)
   uint8_t nn_slot;   // which non-null counter array (one per aggregated column)
   uint8_t update_nn; // 1: this aggregate bumps nn[nn_slot] (first aggregate over its column)
-  uint8_t dset;      // COUNT(DISTINCT): which presence structure (DevPlan.dist), one per distinct column
-  uint8_t dset_owner;  // COUNT(DISTINCT): 1 = this aggregate feeds the structure; a second one over the same column shares its cell
+  uint8_t dset;      // COUNT(DISTINCT): which presence structure (DevPlan.dist), one per distinct column;
+                     // MEDIAN / PERCENTILE_CONT: which pair set (DevPlan.pct), one per column
+  uint8_t dset_owner;  // 1 = this aggregate feeds the structure / pair set; the others over the same column share it
+};
+
+// MEDIAN / PERCENTILE_CONT over one column: k_flat_agg appends one (group slot, order key) pair per non-NULL selected
+// row; the pairs are sorted and picked after the scan (percentile_kernels.cuh).  Room for every row of the live row
+// groups, so the cursor never passes the capacity.
+struct DevPairSet {
+  uint32_t* slots;             // group slot (the hash-table cell under a hashed GROUP BY)
+  unsigned long long* keys;    // order_encode(value, OE_I64 | OE_F64, ascending)
+  unsigned int* count;         // append cursor
+  uint32_t enc;                // OrderEnc of the column's values
+  uint32_t _pad;
 };
 
 // COUNT(DISTINCT col): which (group slot, value id) pairs were seen.  Value ids are the GROUP BY ids of the column
@@ -225,6 +238,9 @@ struct DevPlan {
   uint32_t ndist;              // COUNT(DISTINCT) presence structures (distinct columns)
   uint32_t agg_forms;          // k_flat_agg: bit s = column slot s reads a page's agg page (DevScanArgs.apages) where it has one
   DevDistinct dist[kMaxAggs];
+  uint32_t npct;               // MEDIAN / PERCENTILE_CONT pair sets (percentile columns)
+  uint32_t _pad_pct;
+  DevPairSet pct[kMaxAggs];
 };
 
 // Accumulator table layout (device, 8-byte cells, struct of arrays over nslots):

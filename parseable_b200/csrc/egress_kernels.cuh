@@ -94,7 +94,9 @@ __device__ __forceinline__ unsigned long long agg_output_value(const unsigned lo
     case AG_COUNT_STAR: v = rows; break;
     case AG_COUNT: v = nn; break;
     case AG_COUNT_DISTINCT: v = cell; break;   // first sightings of the group's values: 0 when every input was NULL
-    case AG_SUM: valid = nn > 0; v = cell; break;
+    case AG_SUM:
+    case AG_MEDIAN:             // MEDIAN / PERCENTILE_CONT: the output bits k_pct_pick wrote
+    case AG_PERCENTILE_CONT: valid = nn > 0; v = cell; break;
     case AG_AVG:
       valid = nn > 0;
       if (valid) v = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cell) / double(nn));

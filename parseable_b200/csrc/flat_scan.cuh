@@ -38,6 +38,7 @@
 #include "decode_core.cuh"
 #include "device_structs.hpp"
 #include "flat_store.cuh"
+#include "order_keys.cuh"       // order_encode: the value keys of MEDIAN / PERCENTILE_CONT pairs
 #include "ptx_utils.cuh"
 #include "scan_kernel.cuh"   // acc_add / acc_apply / acc_merge
 
@@ -833,8 +834,33 @@ __device__ __forceinline__ void distinct_pass(const DevDistinct& ds, const ColCt
   }
 }
 
-// DIST: the instantiation with the COUNT(DISTINCT) pass (queries without one run code that does not contain it)
-template <int KR, bool HASHED, bool DIST = false>
+// ---- MEDIAN / PERCENTILE_CONT: every non-NULL selected row appends (group slot, order key of its value) ----
+// One atomicAdd per warp on the set's cursor: the lanes' pair counts are scanned across the warp, and each lane writes
+// its pairs at its offset.  Pair order does not matter (the pairs are sorted after the scan).  Called by every lane.
+template <int KR, typename slot_t>
+__device__ __forceinline__ void pct_emit(const DevPairSet& ps, uint32_t vsel, const slot_t* gs, const uint64_t* bits) {
+  const uint32_t lane = threadIdx.x & 31, mine = __popc(vsel);
+  uint32_t incl = mine;
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+    if ((int)lane >= o) incl += t;
+  }
+  const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+  if (total == 0) return;
+  uint32_t base = lane == 31 ? atomicAdd(ps.count, total) : 0u;
+  base = __shfl_sync(0xffffffffu, base, 31) + incl - mine;
+#pragma unroll
+  for (int i = 0; i < KR; i++)
+    if ((vsel >> i) & 1u) {
+      ps.slots[base] = uint32_t(gs[i]);
+      ps.keys[base] = order_encode(bits[i], ps.enc, false);
+      base++;
+    }
+}
+
+// DIST: the instantiation with the COUNT(DISTINCT) pass, PCT: the one with the MEDIAN / PERCENTILE_CONT pair emission
+// (queries without them run code that does not contain them)
+template <int KR, bool HASHED, bool DIST = false, bool PCT = false>
 __global__ void __launch_bounds__(kAggThreads, 1)
 k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLayout L, const __grid_constant__ DevScanArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -970,7 +996,7 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
               if ((sel >> i) & 1u) {
                 const uint32_t r = tc + i * kAggConsumers;
                 if (nullable && !col_valid(c, r)) { slot[i] += nullslot; continue; }
-                slot[i] += row_id_ids<!DIST>(c, key.card, r) * stride;
+                slot[i] += row_id_ids<!DIST && !PCT>(c, key.card, r) * stride;
               }
           } else if (!nullable) {   // the loads of all rows in flight together
             uint32_t g[KR];
@@ -1039,6 +1065,9 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
             }
         }
         if (ag.fn == AG_COUNT) continue;
+        if constexpr (PCT) {
+          if (ag.fn >= AG_MEDIAN && !ag.dset_owner) continue;   // the column's first percentile aggregate emits its pairs
+        }
         const bool plain = c.fkind == FK_PLAIN8;
         const uint64_t* __restrict__ dict = reinterpret_cast<const uint64_t*>(a.flat + st.col[ag.col].dict8);
         const uint64_t* v8 = c.v8;
@@ -1051,12 +1080,12 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
         // the values first (all loads in flight together: a dictionary value is an L2 round trip), then the updates,
         // one straight-line loop per aggregate function
         uint64_t bits[KR];
-        // a value page (FK_FOR): the values are in the stage, no load at all.  Not in the COUNT(DISTINCT) instantiations
-        // (the planner gives those queries no agg pages): there it spilled registers at the 64-register cap
+        // a value page (FK_FOR): the values are in the stage, no load at all.  Not in the COUNT(DISTINCT) or percentile
+        // instantiations (the planner gives those queries no agg pages): there it spilled registers at the 64-register cap
         if (plain) {
 #pragma unroll
           for (int i = 0; i < KR; i++) bits[i] = ((vsel >> i) & 1u) ? __ldg(v8 + tc + i * kAggConsumers) : 0ull;   // in place in the flat store (global)
-        } else if (!DIST && c.fkind == FK_FOR) {
+        } else if (!DIST && !PCT && c.fkind == FK_FOR) {
           const int64_t fbase = int64_t(st.col[ag.col].dict8);
 #pragma unroll
           for (int i = 0; i < KR; i++)
@@ -1069,6 +1098,13 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
         } else {
 #pragma unroll
           for (int i = 0; i < KR; i++) bits[i] = ((vsel >> i) & 1u) ? __ldg(dict + col_index(c, tc + i * kAggConsumers)) : 0ull;
+        }
+        if constexpr (PCT) {
+          if (fn >= AG_MEDIAN) {   // the hash-table cell is the group under a hashed GROUP BY
+            if constexpr (HASHED) pct_emit<KR>(plan.pct[ag.dset], vsel, cell, bits);
+            else pct_emit<KR>(plan.pct[ag.dset], vsel, slot, bits);
+            continue;
+          }
         }
         if (fn == AG_SUM && !f64) {   // wrapping, like DataFusion's SUM(Int64)
 #pragma unroll

@@ -12,6 +12,7 @@
 //   * SQL three-valued logic, NULL group keys, COUNT -> Int64, SUM(Int64) wrapping,
 //     float totalOrder (SURVEY.md §8 rows a11, a12).
 #include <algorithm>
+#include <charconv>
 #include <chrono>
 #include <cmath>
 #include <cstdlib>
@@ -29,6 +30,7 @@
 #include "json_egress.cuh"
 #include "egress_kernels.cuh"
 #include "order_kernels.cuh"
+#include "percentile_kernels.cuh"
 
 namespace pqb {
 
@@ -58,6 +60,11 @@ constexpr uint64_t kKeepDeviceResult = 1ull << 30;   // result blocks up to this
 // the free HBM); above it the column gets a pair set, of at most kDistinctPairsMax 8-byte entries (2 GiB)
 constexpr uint64_t kDistinctDenseBudget = 1ull << 30;
 constexpr uint64_t kDistinctPairsMax = 1ull << 28;
+// MEDIAN / PERCENTILE_CONT: HBM per row of the live row groups.  Every percentile column holds its emitted pairs (4-byte
+// slot + 8-byte key) until its sort; one column at a time is sorted, with at most kPctSortBytes per pair (order_sort's
+// [2][n] values and NULL flags 18, packed words <= 16, two index arrays 8, the kept order 4, the digit tables 2).
+// The query is refused (PQ_ERR_OOM) when rows x (12 x columns + kPctSortBytes) exceeds half the free HBM.
+constexpr uint64_t kPctPairBytes = 12, kPctSortBytes = 48;
 
 struct Timer {
   cudaEvent_t a, b;
@@ -799,6 +806,45 @@ uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, D
   return launches;
 }
 
+// MEDIAN / PERCENTILE_CONT of one column: its n emitted pairs become two ORDER BY terms (slot, key), sorted by order_sort;
+// k_pct_pick then writes every non-empty group's results.  The emitted pairs are freed once staged.  The kernels are
+// timed (without order_sort's one round trip) into pct_ms.  Returns the kernels it launched.
+uint64_t pct_finish(DevBuf<uint32_t>& slots, DevBuf<unsigned long long>& keys, uint32_t n, PctPickArgs pk, const uint32_t* out_slot,
+                    uint32_t n_out, unsigned long long* acc, uint32_t nslots, bool f64, cudaStream_t stream, PqMetrics& m, double& pct_ms) {
+  OrderBufs ob(2, n, stream, m);
+  Timer t_stage, t_sort, t_pick;
+  PQB_CUDA(cudaEventRecord(t_stage.a, stream));
+  k_pct_stage<<<std::min<uint32_t>(2048, (n + 255) / 256), 256, 0, stream>>>(slots.p, keys.p, n, ob.vals.p, ob.nulls.p, ob.ranges.p);
+  PQB_CUDA(cudaEventRecord(t_stage.b, stream));
+  slots.alloc(0, stream);   // stream ordered: the sort below may reuse the memory
+  keys.alloc(0, stream);
+  const uint8_t nulls_first[2] = {0, 0};
+  DevBuf<uint32_t> sorted;
+  bool sort_timed = false;
+  // every pair equal (one group, one value): nothing is sorted and the emission order is the order (sorted stays empty)
+  const uint64_t launches = 2 + order_sort(ob, 2, n, nulls_first, n, nullptr, sorted, stream, m, t_sort, &sort_timed);
+  pk.vals = ob.vals.p;
+  pk.order = sorted.p;
+  pk.out_slot = out_slot;
+  pk.acc = acc;
+  pk.n = n;
+  pk.n_out = n_out;
+  pk.nslots = nslots;
+  pk.f64 = f64 ? 1u : 0u;
+  PQB_CUDA(cudaEventRecord(t_pick.a, stream));
+  k_pct_pick<<<(n_out + 255) / 256, 256, 0, stream>>>(pk);
+  PQB_CUDA(cudaEventRecord(t_pick.b, stream));
+  PQB_CUDA(cudaGetLastError());
+  PQB_CUDA(cudaStreamSynchronize(stream));
+  float ms = 0.0f;
+  cudaEventElapsedTime(&ms, t_stage.a, t_stage.b);
+  pct_ms += ms;
+  if (sort_timed) { cudaEventElapsedTime(&ms, t_sort.a, t_sort.b); pct_ms += ms; }
+  cudaEventElapsedTime(&ms, t_pick.a, t_pick.b);
+  pct_ms += ms;
+  return launches;
+}
+
 }  // namespace
 
 void Query::run(const PqQueryDesc& d) {
@@ -1151,6 +1197,7 @@ void Query::run(const PqQueryDesc& d) {
   const bool agg_kernel = has_aggs && !only_count_star;
   plan.mode = agg_kernel ? SM_AGG : SM_FILTER;
   std::vector<int> agg_out_type(d.n_aggs, PQ_T_I64);
+  std::vector<double> pct_p(kMaxAggs, 0.0);   // PERCENTILE_CONT: the fraction of each aggregate
   if (has_aggs) {
     uint32_t n_acc = 0;
     plan.naggs = d.n_aggs;
@@ -1159,10 +1206,42 @@ void Query::run(const PqQueryDesc& d) {
       ag = DevAgg{};
       ag.fn = uint8_t(d.aggs[a].fn);
       if (ag.fn == AG_COUNT_STAR) { agg_out_type[a] = PQ_T_I64; continue; }
-      if (ag.fn > AG_COUNT_DISTINCT) throw Error(PQ_ERR_INVALID_ARG, "unknown aggregate function");
+      if (ag.fn > AG_PERCENTILE_CONT) throw Error(PQ_ERR_INVALID_ARG, "unknown aggregate function");
       uint32_t qc = uint32_t(d.aggs[a].col);
       ag.col = uint8_t(slot_of[qc]);
       ag.kind = plan.cols[ag.col].kind;
+      if (ag.fn == AG_MEDIAN || ag.fn == AG_PERCENTILE_CONT) {
+        // the output bits go to an accumulator cell of their own (k_pct_pick writes it after the scan); the pairs of one
+        // column are shared by every percentile aggregate over it
+        const char* fname = ag.fn == AG_MEDIAN ? "MEDIAN" : "PERCENTILE_CONT";
+        const int t = out_type_of(qc);
+        if ((t != PQ_T_I64 && t != PQ_T_F64) || (ag.kind != DK_I64 && ag.kind != DK_F64))
+          throw Error(PQ_ERR_UNSUPPORTED, std::string(fname) + " over " + type_name(t) + " is not on the GPU path");
+        if (ag.fn == AG_PERCENTILE_CONT) {
+          if (!d.agg_params) throw Error(PQ_ERR_INVALID_ARG, "PERCENTILE_CONT needs its fraction in agg_params (NULL)");
+          const double p = d.agg_params[a];
+          if (!std::isfinite(p) || p < 0.0 || p > 1.0)
+            throw Error(PQ_ERR_INVALID_ARG, std::string("PERCENTILE_CONT(") + d.columns[qc].name + ", p): p must be finite and in [0, 1]");
+          pct_p[a] = p;
+        }
+        agg_out_type[a] = ag.fn == AG_MEDIAN ? t : PQ_T_F64;
+        ag.acc_slot = uint8_t(n_acc);
+        plan.acc_init[n_acc++] = 0;
+        uint32_t first = a;
+        for (uint32_t b = 0; b < a; b++)
+          if ((plan.aggs[b].fn == AG_MEDIAN || plan.aggs[b].fn == AG_PERCENTILE_CONT) && plan.aggs[b].col == ag.col) { first = b; break; }
+        if (first != a) {
+          ag.dset = plan.aggs[first].dset;
+          ag.dset_owner = 0;
+          continue;
+        }
+        ag.dset = uint8_t(plan.npct);
+        ag.dset_owner = 1;
+        plan.pct[plan.npct] = DevPairSet{};
+        plan.pct[plan.npct].enc = ag.kind == DK_F64 ? OE_F64 : OE_I64;
+        plan.npct++;
+        continue;
+      }
       if (ag.fn == AG_COUNT_DISTINCT) {
         // the count of first sightings is an integer-add cell; COUNT(DISTINCT) twice over one column shares the first
         // one's presence structure and cell
@@ -1203,6 +1282,10 @@ void Query::run(const PqQueryDesc& d) {
       if (plan.aggs[a].fn == AG_COUNT_DISTINCT && (d.flags & PQ_QUERY_ALLREDUCE))
         throw Error(PQ_ERR_UNSUPPORTED, std::string("COUNT(DISTINCT ") + d.columns[d.aggs[a].col].name +
                                             ") under PQ_QUERY_ALLREDUCE: per-rank distinct counts cannot be summed");
+    if (plan.npct && (d.flags & PQ_QUERY_ALLREDUCE))
+      throw Error(PQ_ERR_UNSUPPORTED, "MEDIAN / PERCENTILE_CONT under PQ_QUERY_ALLREDUCE: exact order statistics cannot be all-reduced");
+    if (plan.npct && plan.ndist)
+      throw Error(PQ_ERR_UNSUPPORTED, "MEDIAN / PERCENTILE_CONT together with COUNT(DISTINCT) in one query is not on the GPU path");
   }
 
   mark("plan compiled");
@@ -1375,7 +1458,7 @@ void Query::run(const PqQueryDesc& d) {
         if (plan.leaves[l].col == key.col && (plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE))
           throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[tcol[d.group_by[k]]].name + "' has pages without a dictionary and is also filtered on: not on the GPU path");
       for (uint32_t a = 0; a < d.n_aggs; a++)
-        if (plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG && plan.aggs[a].col == key.col)
+        if (((plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG) || plan.aggs[a].fn >= AG_MEDIAN) && plan.aggs[a].col == key.col)
           throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[tcol[d.group_by[k]]].name + "' has pages without a dictionary and is also aggregated: not on the GPU path");
       row_keys[k] = 1;
     }
@@ -1529,6 +1612,35 @@ void Query::run(const PqQueryDesc& d) {
     }
   }
 
+  // ---- MEDIAN / PERCENTILE_CONT pair sets: room for every row of the live row groups, refused above half the free HBM
+  // (kPctPairBytes / kPctSortBytes) ----
+  std::vector<DevBuf<uint32_t>> d_pct_slots(plan.npct);
+  std::vector<DevBuf<unsigned long long>> d_pct_keys(plan.npct);
+  DevBuf<unsigned int> d_pct_count;
+  uint64_t pct_rows = 0;
+  if (agg_kernel && plan.npct) {
+    for (uint32_t g = 0; g < nrg_table; g++) if (rg_live[g]) pct_rows += table->row_groups[g].num_rows;
+    if (pct_rows > 0xffffffffull)
+      throw Error(PQ_ERR_UNSUPPORTED, "MEDIAN / PERCENTILE_CONT over more than 2^32 - 1 values of one column is not on the GPU path");
+    size_t free_b = 0, total_b = 0;
+    PQB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const uint64_t need = std::max<uint64_t>(pct_rows, 1) * (kPctPairBytes * plan.npct + kPctSortBytes);
+    uint64_t budget = free_b / 2;
+    if (const char* e = getenv("PQB_PCT_BUDGET")) budget = std::min<uint64_t>(budget, strtoull(e, nullptr, 10));   // test switch: a smaller budget in bytes
+    if (need > budget)
+      throw Error(PQ_ERR_OOM, "MEDIAN / PERCENTILE_CONT: the values and their sort need " + std::to_string(need >> 20) +
+                                  " MiB of HBM, more than their budget: half the free HBM (" + std::to_string(budget >> 20) + " MiB)");
+    d_pct_count.alloc(plan.npct, stream);
+    d_pct_count.zero();
+    for (uint32_t i = 0; i < plan.npct; i++) {
+      d_pct_slots[i].alloc(std::max<uint64_t>(pct_rows, 1), stream);
+      d_pct_keys[i].alloc(std::max<uint64_t>(pct_rows, 1), stream);
+      plan.pct[i].slots = d_pct_slots[i].p;
+      plan.pct[i].keys = d_pct_keys[i].p;
+      plan.pct[i].count = d_pct_count.p + i;
+    }
+  }
+
   // ---- which kernels run ----
   (void)has_null_const;   // the flat kernels evaluate SQL three-valued logic, NULL literals included
   const bool flat_ok = !(getenv("PQB_FLAT_SCAN") && getenv("PQB_FLAT_SCAN")[0] == '0');
@@ -1546,6 +1658,8 @@ void Query::run(const PqQueryDesc& d) {
     if (n_general)
       throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + table->columns[shape_cols[plan.dist[i].col]].name +
                                           ") needs a flat-store copy of every page the query reads: " + shape->why_general);
+  if (agg_kernel && plan.npct && n_general)
+    throw Error(PQ_ERR_UNSUPPORTED, "MEDIAN / PERCENTILE_CONT need a flat-store copy of every page the query reads: " + shape->why_general);
   if (row_order && n_general)
     throw Error(PQ_ERR_UNSUPPORTED, "ORDER BY on a scan needs a flat-store copy of every page the query reads: " + shape->why_general);
   // ---- ORDER BY on a scan: a Utf8 term sorts by the bytewise rank of the column's GROUP BY ids (ensure_key, cached with
@@ -1601,8 +1715,9 @@ void Query::run(const PqQueryDesc& d) {
   plan.agg_forms = 0;
   {
     const char* sw = getenv("PQB_AGG_FORMS");   // A/B switch: 0 = every slot reads its index pages
-    // not with COUNT(DISTINCT): its kernel instantiations carry no agg-page paths (their registers would spill there)
-    if (!(sw && sw[0] == '0') && agg_kernel && n_flat && d.table && !plan.ndist) {
+    // not with COUNT(DISTINCT) or MEDIAN / PERCENTILE_CONT: their kernel instantiations carry no agg-page paths (their
+    // registers would spill there)
+    if (!(sw && sw[0] == '0') && agg_kernel && n_flat && d.table && !plan.ndist && !plan.npct) {
       for (uint32_t s = 0; s < ncols; s++) {
         bool as_key = false, as_value = false, other = false;
         for (uint32_t l = 0; l < nleaves; l++) other |= plan.leaves[l].col == s;
@@ -1865,7 +1980,13 @@ void Query::run(const PqQueryDesc& d) {
         PQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(ctx.smem_optin())));
         kern<<<grid, kAggThreads, FL.total, stream>>>(plan, FL, sa);
       };
-      if (plan.ndist) {   // COUNT(DISTINCT): the instantiations with the presence pass
+      if (plan.npct) {   // MEDIAN / PERCENTILE_CONT: the instantiations with the pair emission
+        if (plan.hashed) go(k_flat_agg<4, true, false, true>);
+        else if (plan.flat_krows >= 8) go(k_flat_agg<8, false, false, true>);
+        else if (plan.flat_krows >= 4) go(k_flat_agg<4, false, false, true>);
+        else go(k_flat_agg<2, false, false, true>);
+      }
+      else if (plan.ndist) {   // COUNT(DISTINCT): the instantiations with the presence pass
         if (plan.hashed) go(k_flat_agg<4, true, true>);
         else if (plan.flat_krows >= 8) go(k_flat_agg<8, false, true>);
         else if (plan.flat_krows >= 4) go(k_flat_agg<4, false, true>);
@@ -1965,6 +2086,11 @@ void Query::run(const PqQueryDesc& d) {
     else PQB_CUDA(cudaMemsetAsync(d_totals.p + 1, 0, 8, stream));
     launches += 4;
     unsigned long long totals[2] = {0, 0};
+    std::vector<unsigned int> pct_count(plan.npct, 0u);
+    if (plan.npct) {
+      PQB_CUDA(cudaMemcpyAsync(pct_count.data(), d_pct_count.p, plan.npct * 4, cudaMemcpyDeviceToHost, stream));
+      metrics.d2h_bytes += plan.npct * 4;
+    }
     PQB_CUDA(cudaMemcpyAsync(totals, d_totals.p, 16, cudaMemcpyDeviceToHost, stream));
     PQB_CUDA(cudaMemcpyAsync(h_counters, d_counters.p, sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
     PQB_CUDA(cudaStreamSynchronize(stream));
@@ -1975,12 +2101,38 @@ void Query::run(const PqQueryDesc& d) {
     uint32_t n_out = uint32_t(totals[0]);
     metrics.rows_selected = totals[1];
     if (allreduce) { float ms = 0; cudaEventElapsedTime(&ms, t_ar.a, t_ar.b); metrics.allreduce_ms = ms; }
-    static const char* fn_names[] = {"count(*)", "count", "sum", "min", "max", "avg", "count(distinct"};
+    static const char* fn_names[] = {"count(*)", "count", "sum", "min", "max", "avg", "count(distinct", "median", "percentile_cont"};
     auto agg_name = [&](uint32_t a) {
       const DevAgg& ag = plan.aggs[a];
+      if (ag.fn == AG_PERCENTILE_CONT) {   // p in shortest round-trip form: percentile_cont(latency_ms, 0.99)
+        char buf[32];
+        const auto r = std::to_chars(buf, buf + sizeof(buf), pct_p[a]);
+        return std::string("percentile_cont(") + d.columns[d.aggs[a].col].name + ", " + std::string(buf, r.ptr) + ")";
+      }
       return ag.fn == AG_COUNT_STAR ? std::string("count(*)")
                                     : std::string(fn_names[ag.fn]) + (ag.fn == AG_COUNT_DISTINCT ? " " : "(") + d.columns[d.aggs[a].col].name + ")";
     };
+    // ---- MEDIAN / PERCENTILE_CONT: sort each column's pairs, pick every group's results into the aggregates' cells ----
+    if (plan.npct && n_out) {
+      double pct_ms = 0.0;
+      for (uint32_t i = 0; i < plan.npct; i++) {
+        PctPickArgs pk{};
+        for (uint32_t a = 0; a < d.n_aggs; a++) {
+          const DevAgg& ag = plan.aggs[a];
+          if ((ag.fn != AG_MEDIAN && ag.fn != AG_PERCENTILE_CONT) || ag.dset != i) continue;
+          pk.a[pk.naggs].p = pct_p[a];
+          pk.a[pk.naggs].median = ag.fn == AG_MEDIAN ? 1 : 0;
+          pk.a[pk.naggs].acc_slot = ag.acc_slot;
+          pk.naggs++;
+        }
+        const uint32_t n = pct_count[i];
+        if (verbose) fprintf(stderr, "[pqb] percentile column %u: %u pairs, %u aggregates\n", i, n, pk.naggs);
+        if (n == 0) continue;   // every input NULL: the non-NULL counts make every result NULL
+        launches += pct_finish(d_pct_slots[i], d_pct_keys[i], n, pk, d_out_slot.p, n_out, d_acc.p, plan.nslots,
+                               plan.pct[i].enc == OE_F64, stream, metrics, pct_ms);
+      }
+      metrics.percentile_ms = pct_ms;
+    }
     // ---- ORDER BY [LIMIT]: permute and cut out_slot; after the all-reduce, so every rank orders identical tables ----
     const uint64_t n_total = (d.n_group_by == 0 && n_out == 0) ? 1 : n_out;   // a global aggregate over zero rows is one row
     uint64_t keep = n_total;
@@ -2010,7 +2162,8 @@ void Query::run(const PqQueryDesc& d) {
             const DevAgg& ag = plan.aggs[ob.index];
             ot.agg = ag;
             ot.nn_is_rows = nn_is_rows[ob.index];
-            ot.enc = (ag.fn == AG_AVG || ((ag.fn == AG_SUM || ag.fn == AG_MIN || ag.fn == AG_MAX) && ag.kind == DK_F64)) ? OE_F64 : OE_I64;
+            ot.enc = (ag.fn == AG_AVG || ag.fn == AG_PERCENTILE_CONT ||
+                      ((ag.fn == AG_SUM || ag.fn == AG_MIN || ag.fn == AG_MAX || ag.fn == AG_MEDIAN) && ag.kind == DK_F64)) ? OE_F64 : OE_I64;
             continue;
           }
           const DevKey& key = plan.keys[ob.index];

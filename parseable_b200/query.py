@@ -88,10 +88,36 @@ class Timestamp:
 _FLIP = {L.PQ_LT: L.PQ_GT, L.PQ_GT: L.PQ_LT, L.PQ_LE: L.PQ_GE, L.PQ_GE: L.PQ_LE, L.PQ_EQ: L.PQ_EQ, L.PQ_NE: L.PQ_NE}
 
 
+def shortest_repr(v: float) -> str:
+    """``std::to_chars(double)``: the shortest digits that round-trip, written fixed or scientific, whichever is shorter
+    (fixed on a tie): 0, 0.5, 0.95, 1, 1e-05.  The C side names PERCENTILE_CONT columns with it."""
+    from decimal import Decimal
+    r = repr(float(v))
+    if r in ("inf", "-inf", "nan"):
+        return r
+    sign, dig, exp = Decimal(r).as_tuple()
+    digits = "".join(map(str, dig))
+    stripped = digits.rstrip("0")
+    exp += len(digits) - len(stripped)
+    digits = stripped or "0"
+    if digits == "0":
+        exp = 0
+    if exp >= 0:
+        fixed = digits + "0" * exp
+    elif len(digits) + exp > 0:
+        fixed = digits[:len(digits) + exp] + "." + digits[len(digits) + exp:]
+    else:
+        fixed = "0." + "0" * -(len(digits) + exp) + digits
+    e = exp + len(digits) - 1
+    sci = digits[0] + ("." + digits[1:] if len(digits) > 1 else "") + f"e{'-' if e < 0 else '+'}{abs(e):02d}"
+    return ("-" if sign else "") + (fixed if len(fixed) <= len(sci) else sci)
+
+
 @dataclass
 class Agg:
-    fn: str           # count_star count sum min max avg count_distinct
+    fn: str           # count_star count sum min max avg count_distinct median percentile_cont
     column: str | None = None
+    p: float | None = None   # percentile_cont: the fraction
 
     @property
     def name(self) -> str:
@@ -100,11 +126,14 @@ class Agg:
             return "count(*)"
         if self.fn == "count_distinct":
             return f"count(distinct {self.column})"
+        if self.fn == "percentile_cont":
+            return f"percentile_cont({self.column}, {shortest_repr(self.p)})"
         return f"{self.fn}({self.column})"
 
 
 _AGG_CODE = {"count_star": L.PQ_AGG_COUNT_STAR, "count": L.PQ_AGG_COUNT, "sum": L.PQ_AGG_SUM,
-             "min": L.PQ_AGG_MIN, "max": L.PQ_AGG_MAX, "avg": L.PQ_AGG_AVG, "count_distinct": L.PQ_AGG_COUNT_DISTINCT}
+             "min": L.PQ_AGG_MIN, "max": L.PQ_AGG_MAX, "avg": L.PQ_AGG_AVG, "count_distinct": L.PQ_AGG_COUNT_DISTINCT,
+             "median": L.PQ_AGG_MEDIAN, "percentile_cont": L.PQ_AGG_PERCENTILE_CONT}
 
 
 @dataclass(frozen=True)
@@ -137,6 +166,8 @@ def min_(c): return Agg("min", c)
 def max_(c): return Agg("max", c)
 def avg(c): return Agg("avg", c)
 def count_distinct(c): return Agg("count_distinct", c)
+def median(c): return Agg("median", c)
+def percentile_cont(c, p): return Agg("percentile_cont", c, float(p))
 
 
 # ----------------------------------------------------------------------------- descriptor builder
@@ -487,6 +518,8 @@ class StandardTableProvider:
         ag = []
         for a in aggs:
             ag.append(L.PqAgg(fn=_AGG_CODE[a.fn], col=d.col_index(a.column) if a.column is not None else -1))
+        # agg_params: PERCENTILE_CONT's fraction, one entry per aggregate (the others ignore theirs)
+        params = (C.c_double * len(aggs))(*[a.p if a.p is not None else 0.0 for a in aggs]) if any(a.fn == "percentile_cont" for a in aggs) else None
         proj = [d.col_index(c) for c in projection]
         # PQ_ORDER_COLUMN terms name their column: it joins the referenced columns
         order = [(t, d.col_index(i) if isinstance(i, str) else i, fl) for t, i, fl in order]
@@ -523,6 +556,8 @@ class StandardTableProvider:
             for i, (target, index, fl) in enumerate(order):
                 arr_ob[i].target, arr_ob[i].index, arr_ob[i].flags = target, index, fl
             desc.order_by, desc.n_order_by = arr_ob, len(order)
+        if params is not None:
+            desc.agg_params = params
         desc.limit = -1 if limit is None else int(limit)
         desc.batch_size = batch_size
         desc.shard_index, desc.shard_count = self.shard_index, self.shard_count
@@ -674,6 +709,8 @@ class Query:
             item = ("pos", int(t[1]))                       # 1-based position in the SELECT list
         elif t[0] == "kw" and t[1] in ("COUNT", "SUM", "MIN", "MAX", "AVG"):
             item = ("agg", self._agg_call())
+        elif self._pct_ahead():
+            item = ("agg", self._pct_call())
         else:
             item = ("name", self._next("id")[1])            # a SELECT alias or a GROUP BY column
         direction = "asc"
@@ -696,6 +733,53 @@ class Query:
             item = Agg(t[1].lower(), self._next("id")[1])
         self._expect("op", ")")
         return item
+
+    # MEDIAN / PERCENTILE_CONT (and the refused approximate forms) are an identifier followed by "(": never reserved, so a
+    # column named `median` still parses as a column
+    _PCT_WORDS = ("MEDIAN", "PERCENTILE_CONT", "APPROX_MEDIAN", "APPROX_PERCENTILE_CONT", "APPROX_PERCENTILE_CONT_WITH_WEIGHT")
+
+    def _pct_ahead(self) -> bool:
+        return self._word() in self._PCT_WORDS and self._peek(1) == ("op", "(")
+
+    def _fraction(self) -> float:
+        t = self._next("num")
+        return float(t[1])
+
+    def _pct_call(self) -> Agg:
+        """MEDIAN(col) | PERCENTILE_CONT(col, p) | PERCENTILE_CONT(p) WITHIN GROUP (ORDER BY col [ASC])."""
+        w = self._next("id")[1].upper()
+        if w.startswith("APPROX_"):
+            raise QueryError(L.PQ_ERR_UNSUPPORTED, f"{w.lower()}: approximate percentiles (t-digest) are not on the GPU path; "
+                                                   "the exact MEDIAN / PERCENTILE_CONT would answer differently")
+        self._expect("op", "(")
+        if w == "MEDIAN":
+            item = Agg("median", self._next("id")[1])
+            self._expect("op", ")")
+            return item
+        if self._peek()[0] == "num":                      # PERCENTILE_CONT(p) WITHIN GROUP (ORDER BY col [ASC])
+            p = self._fraction()
+            self._expect("op", ")")
+            if self._word() != "WITHIN":
+                raise QueryError(L.PQ_ERR_INVALID_ARG, "PERCENTILE_CONT(p) needs WITHIN GROUP (ORDER BY col)")
+            self._i += 1
+            self._expect("kw", "GROUP")
+            self._expect("op", "(")
+            if self._word() != "ORDER":
+                raise QueryError(L.PQ_ERR_INVALID_ARG, "WITHIN GROUP needs (ORDER BY col)")
+            self._i += 1
+            self._expect("kw", "BY")
+            c = self._next("id")[1]
+            if self._word() == "DESC":
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, "PERCENTILE_CONT ... WITHIN GROUP (ORDER BY col DESC) is not on the GPU path")
+            if self._word() == "ASC":
+                self._i += 1
+            self._expect("op", ")")
+            return Agg("percentile_cont", c, p)
+        c = self._next("id")[1]
+        self._expect("op", ",")
+        p = self._fraction()
+        self._expect("op", ")")
+        return Agg("percentile_cont", c, p)
 
     def _next(self, kind):
         t = self._peek()
@@ -722,6 +806,10 @@ class Query:
             return ("star",)
         if t[0] == "kw" and t[1] in ("COUNT", "SUM", "MIN", "MAX", "AVG"):
             item = self._agg_call()
+            alias = self._next("id")[1] if self._accept("kw", "AS") else None
+            return ("agg", item, alias)
+        if self._pct_ahead():
+            item = self._pct_call()
             alias = self._next("id")[1] if self._accept("kw", "AS") else None
             return ("agg", item, alias)
         name = self._next("id")[1]

@@ -1,9 +1,11 @@
 // TEST HARNESS ONLY: exposes the pure host/device ORDER BY key functions of order_keys.cuh to tests/test_order_keys.py,
-// run in the same sequence as k_order_encode -> pack plan -> k_order_pack.  Never linked into libparseable_b200.so.
+// run in the same sequence as k_order_encode -> pack plan -> k_order_pack, and the MEDIAN / PERCENTILE_CONT arithmetic of
+// percentile_core.cuh to tests/test_percentile_core.py.  Never linked into libparseable_b200.so.
 #include <cstdint>
 #include <cstring>
 #include <vector>
 #include "order_keys.cuh"
+#include "percentile_core.cuh"
 using namespace pqb;
 
 extern "C" {
@@ -51,4 +53,12 @@ void ok_string_ranks(const uint32_t* offs, const uint8_t* bytes, uint32_t card, 
 }
 
 uint32_t ok_max_words() { return kMaxOrderWords; }
+
+// MEDIAN / PERCENTILE_CONT of one group as k_pct_pick computes it: keys[0, n) are the group's ascending order keys
+// (ok_encode(bits, OE_I64 | OE_F64, 0)); median != 0: MEDIAN, else PERCENTILE_CONT(p).  Returns the result's bits.
+uint64_t pk_pick(const uint64_t* keys, uint64_t n, int median, double p, int f64) {
+  return pct_pick([&](uint64_t i) { return keys[i]; }, n, median != 0, p, f64 != 0);
+}
+uint64_t pk_key_bits(uint64_t key, int f64) { return pct_key_bits(key, f64 != 0); }
+uint64_t pk_f64_op(uint64_t a, uint64_t b, int op) { return pct_f64_op(a, b, op); }
 }

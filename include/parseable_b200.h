@@ -141,6 +141,16 @@ typedef enum {
   PQ_AGG_COUNT_STAR = 0,
   PQ_AGG_COUNT = 1,
   PQ_AGG_SUM = 2,
+  /* MIN / MAX (DataFusion's min / max, restated, not checked): Int64, Timestamp(ms), Float64 (totalOrder), and:
+   *   Utf8: bytewise order, a prefix before any longer string (the order ORDER BY uses); output Utf8 with int32 offsets
+   *     (the shim casts it to Utf8View, as for Utf8 keys), named "min(<col>)" / "max(<col>)".  Dictionary pages,
+   *     PLAIN-fallback pages and DELTA_BYTE_ARRAY / DELTA_LENGTH_BYTE_ARRAY pages.
+   *   Boolean: false < true (MIN is false if any input is false, MAX true if any is true); output Boolean.
+   * NULL inputs are ignored, a group with no non-NULL input gets NULL, a column missing from a file reads as NULL, a global
+   * aggregate over zero rows returns one row holding NULL.  They combine with every other aggregate (COUNT(DISTINCT) and
+   * MEDIAN / PERCENTILE_CONT included), every GROUP BY form, ORDER BY [... LIMIT] and PQ_QUERY_ALLREDUCE.  Over Utf8 /
+   * Boolean, PQ_ERR_UNSUPPORTED: pages without a flat-store copy (the k_scan path), a Utf8 column whose pages lack a
+   * dictionary that the predicate also compares or matches (CMP / LIKE), and more than 2 GiB of result strings. */
   PQ_AGG_MIN = 3,
   PQ_AGG_MAX = 4,
   PQ_AGG_AVG = 5,

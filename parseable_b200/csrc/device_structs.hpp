@@ -143,7 +143,7 @@ enum DevAggFn : uint8_t { AG_COUNT_STAR = 0, AG_COUNT = 1, AG_SUM = 2, AG_MIN = 
 struct DevAgg {
   uint8_t fn;
   uint8_t col;       // column slot
-  uint8_t kind;      // DevKind of the input (I64 / F64 / BOOL)
+  uint8_t kind;      // DevKind of the input (I64 / F64; STR / BOOL: COUNT, COUNT(DISTINCT), MIN / MAX through DevPlan.rank)
   uint8_t acc_slot;  // which 8-byte accumulator array (COUNT(DISTINCT): the per-group count of first sightings)
   uint8_t nn_slot;   // which non-null counter array (one per aggregated column)
   uint8_t update_nn; // 1: this aggregate bumps nn[nn_slot] (first aggregate over its column)
@@ -177,6 +177,17 @@ struct DevDistinct {
   const uint32_t* gid;  // gid LUT of the column (entry = chunk.lut_base + idx)
   unsigned int* bits;   // dense bitmap
   unsigned long long* pairs;   // pair set (~0: empty)
+};
+
+// MIN / MAX over Utf8: a row's value is its bytewise rank among the column's distinct values (ranks of one numbering, local
+// or agreed), so the signed 64-bit MIN / MAX cells order strings; the result maps the winning rank back to its bytes.
+// MIN / MAX over Boolean: ids is {0, 1}, indexed by the row's bit.  64-bit entries: k_flat_agg reads them with the load
+// of its numeric dictionaries.
+struct DevRankLut {
+  const uint64_t* ent;             // rank of every dictionary entry (entry = chunk.lut_base + idx): rank[gid[entry]], composed once per column
+  const uint64_t* ids;             // rank of every group id (id pages, FK_IDS, hold group ids), or the Boolean table
+  uint32_t max_id;                // largest index of ids (card - 1; 0 without values): a corrupt id never leaves the table
+  uint32_t _pad;
 };
 
 enum DevKeyKind : uint8_t { KK_DICT_LUT = 0, KK_BOOL = 1, KK_BIN = 2 };   // KK_BIN: DATE_BIN of an Int64 / Timestamp column
@@ -241,6 +252,7 @@ struct DevPlan {
   uint32_t npct;               // MEDIAN / PERCENTILE_CONT pair sets (percentile columns)
   uint32_t _pad_pct;
   DevPairSet pct[kMaxAggs];
+  DevRankLut rank[kMaxAggs];   // per aggregate: MIN / MAX over Utf8 reads its rows' ranks (unused by every other aggregate)
 };
 
 // Accumulator table layout (device, 8-byte cells, struct of arrays over nslots):

@@ -66,6 +66,15 @@ struct FinishKey {
   uint32_t is_bin;             // DATE_BIN key: value = bin_base + group id * bin_width
   int64_t bin_base, bin_width;
 };
+// MIN / MAX over Utf8: the cell holds the winning rank; inv maps it to its group id in the numbering whose dictionary
+// (kd_offs / kd_bytes) holds the bytes
+struct FinishAggStr {
+  const uint32_t* kd_offs;
+  const uint8_t* kd_bytes;
+  const uint32_t* inv;         // rank -> group id
+  uint64_t len_off;            // u32 length per row (scratch, device only)
+  uint64_t data_off;           // bytes
+};
 struct FinishArgs {
   const unsigned long long* acc;
   const unsigned long long* wide;   // hashed group-by: wide group id per slot (nullptr: the slot is the id)
@@ -76,7 +85,11 @@ struct FinishArgs {
   uint32_t batch_rows, words_per_batch, nbatches;
   DevAgg aggs[kMaxAggs];
   uint8_t nn_is_rows[kMaxAggs];
+  // the output layout of each aggregate: DK_STR (MIN / MAX over Utf8: int32 offsets at val_off, bytes at astr.data_off),
+  // DK_BOOL (MIN / MAX over Boolean: bit-packed values per batch at val_off), anything else 8-byte values
+  uint8_t out_kind[kMaxAggs];
   uint64_t val_off[kMaxAggs], valid_off[kMaxAggs];
+  FinishAggStr astr[kMaxAggs];
   FinishKey keys[kMaxKeys];
 };
 
@@ -124,7 +137,15 @@ __global__ void k_agg_finish(const __grid_constant__ FinishArgs f) {
   for (uint32_t a = 0; a < f.naggs; a++) {
     bool valid;
     const unsigned long long v = agg_output_value(f.acc, f.nslots, f.n_acc, f.aggs[a], f.nn_is_rows[a], slot, rows, valid);
-    reinterpret_cast<unsigned long long*>(f.out + f.val_off[a])[i] = valid ? v : 0ull;
+    if (f.out_kind[a] == DK_STR) {   // the winning rank's length; k_agg_str_gather copies its bytes
+      const FinishAggStr& s = f.astr[a];
+      const uint32_t g = valid ? s.inv[v] : 0u;
+      reinterpret_cast<uint32_t*>(f.out + s.len_off)[i] = valid ? s.kd_offs[g + 1] - s.kd_offs[g] : 0u;
+    } else if (f.out_kind[a] == DK_BOOL) {
+      if (valid && v) atomicOr(reinterpret_cast<uint32_t*>(f.out + f.val_off[a]) + word, bit);
+    } else {
+      reinterpret_cast<unsigned long long*>(f.out + f.val_off[a])[i] = valid ? v : 0ull;
+    }
     if (valid) atomicOr(reinterpret_cast<uint32_t*>(f.out + f.valid_off[a]) + word, bit);
     else atomicAdd(&f.nulls[(f.nkeys + a) * f.nbatches + batch], 1u);
   }
@@ -194,6 +215,20 @@ __global__ void k_key_gather(const __grid_constant__ FinishArgs f, uint32_t k) {
   const uint32_t a = key.kd_offs[gid], n = key.kd_offs[gid + 1] - a;
   uint8_t* dst = f.out + key.data_off + reinterpret_cast<const int32_t*>(f.out + key.val_off)[i];
   for (uint32_t b = lane; b < n; b += 32) dst[b] = key.kd_bytes[a + b];
+}
+
+// bytes of a MIN / MAX over Utf8 (aggregate a): one warp per output row
+__global__ void k_agg_str_gather(const __grid_constant__ FinishArgs f, uint32_t a) {
+  const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (i >= f.n_out) return;
+  const FinishAggStr& s = f.astr[a];
+  const uint32_t n = reinterpret_cast<const uint32_t*>(f.out + s.len_off)[i];
+  if (n == 0) return;   // NULL, or the empty string
+  const unsigned long long rank = f.acc[size_t(1 + f.aggs[a].acc_slot) * f.nslots + f.out_slot[i]];
+  const uint32_t g = s.inv[rank];
+  const uint8_t* src = s.kd_bytes + s.kd_offs[g];
+  uint8_t* dst = f.out + s.data_off + reinterpret_cast<const int32_t*>(f.out + f.val_off[a])[i];
+  for (uint32_t b = lane; b < n; b += 32) dst[b] = src[b];
 }
 
 

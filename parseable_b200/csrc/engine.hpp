@@ -111,6 +111,18 @@ struct TableRowGroup {
 // Query-independent side tables of one table column, built on first use and kept with the table:
 // string dictionary entry offsets, and (GROUP BY) the interned group ids of every dictionary entry.
 struct KeyDict { std::vector<uint32_t> offs; std::vector<uint8_t> bytes; };
+// MIN / MAX over a Utf8 column, one numbering (local or agreed), built from ensure_kd_rank's ranks: the bytewise rank of
+// every dictionary entry (rank[gid[e]], composed once so that the aggregate pass makes one load per row) and of every group
+// id (id pages), as 64-bit values like a numeric dictionary's; and the rank -> group id inverse for the result
+struct RankLuts {
+  uint64_t* ent = nullptr;               // per dictionary entry of the column (ColSide::total_entries)
+  uint64_t* ids = nullptr;               // per group id
+  uint32_t* inv = nullptr;               // per rank: its group id
+  uint32_t card = 0;
+  RankLuts() = default;
+  RankLuts(const RankLuts&) = delete;
+  ~RankLuts();
+};
 struct ColSide {
   std::vector<uint32_t> base_per_rg;   // dictionary entries of this column in the row groups before g
   uint32_t total_entries = 0;
@@ -140,6 +152,7 @@ struct ColSide {
   uint32_t* d_glob_kd_offs = nullptr;
   uint8_t* d_glob_kd_bytes = nullptr;
   std::shared_ptr<const uint32_t> glob_kd_rank;   // the same ranks over the agreed numbering (dropped by every unify_key)
+  std::shared_ptr<const RankLuts> rank_luts, glob_rank_luts;   // MIN / MAX over Utf8 (ensure_rank_luts); the agreed one is dropped by every unify_key
   uint64_t* d_key_hash = nullptr;
   // GROUP BY on a column with pages that have no dictionary (PLAIN fallback, PLAIN / DELTA numerics): every ROW of those
   // pages is an entry behind the dictionary entries; d_gid / d_glob_gid then hold, per such page, one group id per row --
@@ -233,6 +246,9 @@ class Table {
   // bytewise rank per group id of a Utf8 key column, local or agreed numbering (after ensure_key / unify_key)
   // (shared: a query keeps the ranks it sorts with alive even if unify_key replaces them meanwhile)
   std::shared_ptr<const uint32_t> ensure_kd_rank(int tcol, bool agreed, cudaStream_t stream) const;
+  // MIN / MAX over a Utf8 column: its rank tables in the local or agreed numbering (after ensure_key / unify_key), built
+  // once per numbering from ensure_kd_rank's ranks; shared like them
+  std::shared_ptr<const RankLuts> ensure_rank_luts(int tcol, bool agreed, cudaStream_t stream) const;
   void ensure_plain8(int tcol, cudaStream_t stream) const;   // DELTA_BINARY_PACKED pages -> row-addressable 8-byte values
   // agg pages: a second flat page table parallel to pages[] (FK_NONE: the page has no other form), read by k_flat_agg's
   // producer for the column slots a query marks.  ensure_for_pages: value pages of a numeric column; ensure_id_pages: id
@@ -269,6 +285,7 @@ void launch_delta_to_plain8(const uint8_t* arena, const DevPage* pages, const vo
                             cudaStream_t stream);
 void build_key_side(const Table& t, int tcol, ColSide& side, cudaStream_t stream);
 void unify_key_side(const Table& t, int tcol, ColSide& side, cudaStream_t stream);
+void build_rank_luts(const ColSide& side, bool agreed, const uint32_t* rank, RankLuts& luts, cudaStream_t stream);
 
 // page-locked host block that result batches can alias (zero copy); returns to the pool when
 // the last batch that references it is released by the consumer

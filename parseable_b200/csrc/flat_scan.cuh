@@ -1070,6 +1070,14 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
         }
         const bool plain = c.fkind == FK_PLAIN8;
         const uint64_t* __restrict__ dict = reinterpret_cast<const uint64_t*>(a.flat + st.col[ag.col].dict8);
+        if (ag.kind >= DK_STR) {
+          // MIN / MAX over Utf8 / Boolean: the dictionary load below reads the row's rank instead -- through the rank LUT
+          // composed per dictionary entry, or indexed by the row's staged word itself (an id page's group id, a Boolean's bit)
+          const DevRankLut& rl = plan.rank[g];
+          const bool direct = c.fkind != FK_INDEX;
+          dict = direct ? rl.ids : rl.ent + st.col[ag.col].lut_base;
+          if (direct) c.dict_max = rl.max_id;
+        }
         const uint64_t* v8 = c.v8;
         unsigned long long* scell = sacc + size_t(1 + ag.acc_slot) * Hs;
         unsigned long long* gcell = gadj + size_t(1 + ag.acc_slot) * nslots;

@@ -241,6 +241,22 @@ __global__ void k_gid_remap(const uint32_t* __restrict__ gid_in, uint32_t* __res
   }
 }
 
+// MIN / MAX over Utf8, per group id g < card: ids[g] = rank[g] (64-bit), inv[rank[g]] = g (the group id of every rank)
+__global__ void k_rank_ids(const uint32_t* __restrict__ rank, uint32_t card, uint64_t* __restrict__ ids, uint32_t* __restrict__ inv) {
+  for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < card; g += gridDim.x * blockDim.x) {
+    ids[g] = rank[g];
+    inv[rank[g]] = g;
+  }
+}
+// ... and per dictionary entry: ent[e] = rank[gid[e]]
+__global__ void k_rank_compose(const uint32_t* __restrict__ gid, uint32_t n_entries, const uint32_t* __restrict__ rank, uint32_t card,
+                               uint64_t* __restrict__ ent) {
+  for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < n_entries; e += gridDim.x * blockDim.x) {
+    const uint32_t g = gid[e];
+    ent[e] = g < card ? rank[g] : 0u;
+  }
+}
+
 // Occurrences of every group id over a sample of the key column's flat pages: the hot-first
 // numbering of group ids (the flat aggregate kernel keeps slots < hot_slots in shared memory).
 struct KeySamplePage { uint64_t off; uint32_t rows; uint32_t bw; uint32_t base; uint32_t dict_n; };

@@ -204,6 +204,11 @@ const char* type_name(int t) {
 
 uint32_t align_up(uint32_t v, uint32_t a) { return (v + a - 1) & ~(a - 1); }
 
+// MIN / MAX over Utf8: the rows' values are their bytewise ranks (DevPlan.rank), read through the column's GROUP BY ids --
+// like a key column, it reads ids, never the values themselves
+bool rank_min_max(const DevAgg& ag) { return (ag.fn == AG_MIN || ag.fn == AG_MAX) && ag.kind == DK_STR; }
+bool bool_min_max(const DevAgg& ag) { return (ag.fn == AG_MIN || ag.fn == AG_MAX) && ag.kind == DK_BOOL; }
+
 }  // namespace
 
 Query::Query(const PqQueryDesc& d) {
@@ -649,6 +654,7 @@ void unify_key_side(const Table& t, int tcol, ColSide& cs, cudaStream_t stream) 
   renew(cs.d_glob_kd_offs, glob.offs.size() * 4);
   renew(cs.d_glob_kd_bytes, glob.bytes.size());
   cs.glob_kd_rank.reset();   // ranks of the old agreement (a query still sorting with them holds its own reference)
+  cs.glob_rank_luts.reset(); // likewise the MIN / MAX rank tables composed from them
   PQB_CUDA(cudaMemcpyAsync(cs.d_glob_kd_offs, glob.offs.data(), glob.offs.size() * 4, cudaMemcpyHostToDevice, stream));
   if (!glob.bytes.empty()) PQB_CUDA(cudaMemcpyAsync(cs.d_glob_kd_bytes, glob.bytes.data(), glob.bytes.size(), cudaMemcpyHostToDevice, stream));
   cs.glob_max_len = 0;
@@ -664,6 +670,29 @@ void unify_key_side(const Table& t, int tcol, ColSide& cs, cudaStream_t stream) 
   cs.glob_epoch = comm_epoch();
   cs.glob_ready = true;
 }
+
+// MIN / MAX over Utf8 (callers hold side_mu): from the bytewise rank of every group id of the numbering, the rank of
+// every dictionary entry (through the numbering's gid LUT) and of every group id, and the group id of every rank.  Every
+// table has at least one entry, so that a column without values still hands out valid pointers.
+void build_rank_luts(const ColSide& cs, bool agreed, const uint32_t* rank, RankLuts& luts, cudaStream_t stream) {
+  const uint32_t card = agreed ? cs.glob_card : cs.card, n_ent = cs.total_entries;
+  const uint32_t* gid = agreed ? cs.d_glob_gid : cs.d_gid;
+  luts.card = card;
+  auto alloc0 = [&](auto*& p, size_t n) {
+    PQB_CUDA(cudaMallocAsync((void**)&p, std::max<size_t>(n, 1) * sizeof(*p), stream));
+    PQB_CUDA(cudaMemsetAsync(p, 0, std::max<size_t>(n, 1) * sizeof(*p), stream));
+  };
+  alloc0(luts.ent, n_ent);
+  alloc0(luts.ids, card);
+  alloc0(luts.inv, card);
+  if (card && n_ent) k_rank_compose<<<std::min<uint32_t>(1024, (n_ent + 255) / 256), 256, 0, stream>>>(gid, n_ent, rank, card, luts.ent);
+  if (card) k_rank_ids<<<std::min<uint32_t>(1024, (card + 255) / 256), 256, 0, stream>>>(rank, card, luts.ids, luts.inv);
+  PQB_CUDA(cudaGetLastError());
+  PQB_CUDA(cudaStreamSynchronize(stream));
+}
+
+// MIN / MAX over Boolean: the "rank" of a row is its bit (false < true), read through this table like a group id
+__device__ const uint64_t kBoolRank[2] = {0, 1};
 
 namespace {
 
@@ -1266,8 +1295,16 @@ void Query::run(const PqQueryDesc& d) {
         plan.ndist++;
         continue;
       }
+      if ((ag.fn == AG_MIN || ag.fn == AG_MAX) && (ag.kind == DK_STR || ag.kind == DK_BOOL)) {
+        // the signed MIN / MAX cells of the numeric path: a Utf8 row contributes its bytewise rank (plan.rank, set with
+        // the GROUP BY ids below), a Boolean row its bit; the result maps the cell back to the input type
+        ag.acc_slot = uint8_t(n_acc);
+        plan.acc_init[n_acc++] = ag.fn == AG_MIN ? 2 : 3;
+        agg_out_type[a] = out_type_of(qc);
+        continue;
+      }
       if (ag.fn != AG_COUNT && ag.kind != DK_I64 && ag.kind != DK_F64)
-        throw Error(PQ_ERR_UNSUPPORTED, std::string("SUM/MIN/MAX/AVG over ") + type_name(out_type_of(qc)) + " is not on the GPU path");
+        throw Error(PQ_ERR_UNSUPPORTED, std::string("SUM/AVG over ") + type_name(out_type_of(qc)) + " is not on the GPU path");
       if (ag.fn == AG_COUNT) { agg_out_type[a] = PQ_T_I64; continue; }
       ag.acc_slot = uint8_t(n_acc);
       uint8_t how = 0;
@@ -1340,6 +1377,11 @@ void Query::run(const PqQueryDesc& d) {
       if (plan.cols[s].kind == DK_BOOL) continue;
       const ColSide& cs = table->sides[shape_cols[s]];
       if (!cs.glob_ready || cs.glob_epoch != comm_epoch()) f[0] = 1;   // this rank lacks an agreement
+    }
+    for (uint32_t a = 0; a < d.n_aggs; a++) {   // MIN / MAX over Utf8 read their ranks in the agreed numbering too
+      if (!rank_min_max(plan.aggs[a])) continue;
+      const ColSide& cs = table->sides[shape_cols[plan.aggs[a].col]];
+      if (!cs.glob_ready || cs.glob_epoch != comm_epoch()) f[0] = 1;
     }
     for (uint32_t s = 0; s < ncols; s++) f[1 + s] = col_has_nulls[s] ? 1ull : 0ull;
     DevBuf<unsigned long long> df;
@@ -1458,7 +1500,8 @@ void Query::run(const PqQueryDesc& d) {
         if (plan.leaves[l].col == key.col && (plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE))
           throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[tcol[d.group_by[k]]].name + "' has pages without a dictionary and is also filtered on: not on the GPU path");
       for (uint32_t a = 0; a < d.n_aggs; a++)
-        if (((plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG) || plan.aggs[a].fn >= AG_MEDIAN) && plan.aggs[a].col == key.col)
+        if (((plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG) || plan.aggs[a].fn >= AG_MEDIAN) && plan.aggs[a].col == key.col &&
+            !rank_min_max(plan.aggs[a]))
           throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[tcol[d.group_by[k]]].name + "' has pages without a dictionary and is also aggregated: not on the GPU path");
       row_keys[k] = 1;
     }
@@ -1502,7 +1545,7 @@ void Query::run(const PqQueryDesc& d) {
         if (plan.leaves[l].col == ds.col && (plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE))
           throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + cname + "): the column has pages without a dictionary and is also filtered on: not on the GPU path");
       for (uint32_t a = 0; a < d.n_aggs; a++)
-        if (plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG && plan.aggs[a].col == ds.col)
+        if (plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG && plan.aggs[a].col == ds.col && !rank_min_max(plan.aggs[a]))
           throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + cname + "): the column has pages without a dictionary and is also aggregated: not on the GPU path");
       for (uint32_t k = 0; k < d.n_group_by; k++)
         if (plan.keys[k].kind == KK_BIN && plan.keys[k].col == ds.col)
@@ -1513,6 +1556,39 @@ void Query::run(const PqQueryDesc& d) {
     ds.gid = cs.d_gid;
     ds.card = cs.card;
     if (plan.cols[ds.col].has_plain || plan.cols[ds.col].has_delta) ids_gid[ds.col] = ds.gid;
+  }
+  // ---- MIN / MAX over Utf8: ranks through the column's GROUP BY ids, in the numbering the keys use (the ranks' agreed one
+  // under a multi-GPU all-reduce, so that every rank's cells hold ranks of the same values); pages without a dictionary
+  // are read as id pages, as for a key column ----
+  std::vector<std::shared_ptr<const RankLuts>> rank_luts(d.n_aggs);   // held by the query: a unify_key elsewhere may replace the column's
+  {
+    std::set<int> unified;   // key columns agreed on above
+    for (uint32_t k = 0; multi && !keys_agreed && k < d.n_group_by; k++)
+      if (plan.keys[k].kind == KK_DICT_LUT) unified.insert(shape_cols[plan.keys[k].col]);
+    for (uint32_t a = 0; agg_kernel && a < d.n_aggs; a++) {
+      const DevAgg& ag = plan.aggs[a];
+      if (bool_min_max(ag)) {
+        void* bool_rank = nullptr;
+        PQB_CUDA(cudaGetSymbolAddress(&bool_rank, kBoolRank));
+        plan.rank[a] = DevRankLut{nullptr, static_cast<const uint64_t*>(bool_rank), 1u, 0u};
+        continue;
+      }
+      if (!rank_min_max(ag)) continue;
+      const int tc_i = shape_cols[ag.col];
+      if (table->columns[tc_i].kind == 0xfe && !multi) continue;   // in no file: every row NULL, nothing to rank
+      const bool row_ids = plan.cols[ag.col].has_plain || plan.cols[ag.col].has_delta;
+      if (row_ids)
+        for (uint32_t l = 0; l < nleaves; l++)
+          if (plan.leaves[l].col == ag.col && (plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE))
+            throw Error(PQ_ERR_UNSUPPORTED, std::string(ag.fn == AG_MIN ? "MIN(" : "MAX(") + table->columns[tc_i].name +
+                                                "): the column has pages without a dictionary and is also filtered on: not on the GPU path");
+      table->ensure_key(tc_i, stream);
+      if (multi && !keys_agreed && unified.insert(tc_i).second) table->unify_key(tc_i, stream);
+      rank_luts[a] = table->ensure_rank_luts(tc_i, multi, stream);
+      const RankLuts& rl = *rank_luts[a];
+      plan.rank[a] = DevRankLut{rl.ent, rl.ids, rl.card ? rl.card - 1 : 0u, 0u};
+      if (row_ids) ids_gid[ag.col] = multi ? table->sides[tc_i].d_glob_gid : table->sides[tc_i].d_gid;
+    }
   }
   // ---- id pages of key / COUNT(DISTINCT) columns with pages that have no dictionary: this query's copy of the flat
   // page table, with those pages pointing into the column's id array (local or agreed numbering) ----
@@ -1660,6 +1736,10 @@ void Query::run(const PqQueryDesc& d) {
                                           ") needs a flat-store copy of every page the query reads: " + shape->why_general);
   if (agg_kernel && plan.npct && n_general)
     throw Error(PQ_ERR_UNSUPPORTED, "MEDIAN / PERCENTILE_CONT need a flat-store copy of every page the query reads: " + shape->why_general);
+  for (uint32_t a = 0; agg_kernel && n_general && a < d.n_aggs; a++)   // (a column in no file has nothing to read: k_scan takes it)
+    if ((rank_min_max(plan.aggs[a]) || bool_min_max(plan.aggs[a])) && table->columns[shape_cols[plan.aggs[a].col]].kind != 0xfe)
+      throw Error(PQ_ERR_UNSUPPORTED, std::string(plan.aggs[a].fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
+                                          ") over Utf8 / Boolean needs a flat-store copy of every page the query reads: " + shape->why_general);
   if (row_order && n_general)
     throw Error(PQ_ERR_UNSUPPORTED, "ORDER BY on a scan needs a flat-store copy of every page the query reads: " + shape->why_general);
   // ---- ORDER BY on a scan: a Utf8 term sorts by the bytewise rank of the column's GROUP BY ids (ensure_key, cached with
@@ -1731,7 +1811,9 @@ void Query::run(const PqQueryDesc& d) {
           const DevAgg& ag = plan.aggs[a];
           if (ag.fn == AG_COUNT_STAR || ag.col != s) continue;
           if (ag.fn == AG_COUNT_DISTINCT) other = true;
-          else if (ag.fn >= AG_SUM && ag.fn <= AG_AVG) as_value = true;   // COUNT(col) reads the validity bits only: any form serves it
+          else if (bool_min_max(ag)) other = true;   // reads the bits of its pages
+          // MIN / MAX over Utf8 reads group ids: the id pages of a key column serve it (value pages are numeric only)
+          else if (ag.fn >= AG_SUM && ag.fn <= AG_AVG && !rank_min_max(ag)) as_value = true;   // COUNT(col) reads the validity bits only: any form serves it
         }
         if (other || as_key == as_value) continue;
         const int tc_i = shape_cols[s];
@@ -2205,6 +2287,7 @@ void Query::run(const PqQueryDesc& d) {
         oc.values.assign(8, 0);
         const bool is_count = plan.aggs[a].fn == AG_COUNT_STAR || plan.aggs[a].fn == AG_COUNT || plan.aggs[a].fn == AG_COUNT_DISTINCT;
         if (!is_count) { oc.validity.assign(1, 0); oc.null_count = 1; }
+        if (oc.type == PQ_T_UTF8) oc.offsets.assign(2, 0);   // MIN / MAX over Utf8: one NULL row, no bytes
         ob.cols.push_back(std::move(oc));
       }
       metrics.groups = 1;
@@ -2254,7 +2337,25 @@ void Query::run(const PqQueryDesc& d) {
         fa.aggs[a] = plan.aggs[a];
         fa.nn_is_rows[a] = nn_is_rows[a];
         fa.valid_off[a] = take(uint64_t(nbatches) * wpb * 4);
-        fa.val_off[a] = take(uint64_t(n_out) * 8);
+        fa.out_kind[a] = rank_min_max(plan.aggs[a]) ? DK_STR : bool_min_max(plan.aggs[a]) ? DK_BOOL : DK_I64;   // the layouts of the keys
+        if (fa.out_kind[a] == DK_BOOL) fa.val_off[a] = take(uint64_t(nbatches) * wpb * 4);
+        else if (fa.out_kind[a] == DK_STR) fa.val_off[a] = take((uint64_t(n_out) + 1) * 4);
+        else fa.val_off[a] = take(uint64_t(n_out) * 8);
+      }
+      // MIN / MAX over Utf8: the winning values' bytes, bounded by rows x the longest value of the numbering (any group may
+      // hold the longest one)
+      for (uint32_t a = 0; a < d.n_aggs; a++) {
+        if (fa.out_kind[a] != DK_STR) continue;
+        FinishAggStr& s = fa.astr[a];
+        const ColSide& cs = table->sides[shape_cols[plan.aggs[a].col]];
+        s.kd_offs = multi ? cs.d_glob_kd_offs : cs.d_kd_offs;
+        s.kd_bytes = multi ? cs.d_glob_kd_bytes : cs.d_kd_bytes;
+        s.inv = rank_luts[a] ? rank_luts[a]->inv : nullptr;   // nullptr: a column in no file, every group NULL
+        const uint64_t bound = rank_luts[a] ? uint64_t(n_out) * (multi ? cs.glob_max_len : cs.kd_max_len) : 0;
+        if (bound > 0x7fffffffull)
+          throw Error(PQ_ERR_UNSUPPORTED, std::string(plan.aggs[a].fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
+                                              "): the strings of one result may exceed 2 GiB");
+        s.data_off = take(bound);
       }
       // string key bytes: an upper bound (rows x the longest distinct value) keeps the copy to one round trip
       for (uint32_t k = 0; k < d.n_group_by; k++) {
@@ -2274,6 +2375,8 @@ void Query::run(const PqQueryDesc& d) {
       const uint64_t copy_bytes = off;
       for (uint32_t k = 0; k < d.n_group_by; k++)
         if (fa.keys[k].kind == DK_STR) fa.keys[k].len_off = take(uint64_t(n_out) * 4);   // device-only scratch behind the copied part
+      for (uint32_t a = 0; a < d.n_aggs; a++)
+        if (fa.out_kind[a] == DK_STR) fa.astr[a].len_off = take(uint64_t(n_out) * 4);
       DevBuf<uint8_t> d_block;
       d_block.alloc(off, stream);
       PQB_CUDA(cudaMemsetAsync(d_block.p, 0, copy_bytes, stream));
@@ -2297,6 +2400,13 @@ void Query::run(const PqQueryDesc& d) {
         k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.keys[k].len_off), n_out,
                                                reinterpret_cast<int32_t*>(d_block.p + fa.keys[k].val_off));
         k_key_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, k);
+        launches += 2;
+      }
+      for (uint32_t a = 0; a < d.n_aggs; a++) {
+        if (fa.out_kind[a] != DK_STR) continue;
+        k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.astr[a].len_off), n_out,
+                                               reinterpret_cast<int32_t*>(d_block.p + fa.val_off[a]));
+        k_agg_str_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, a);
         launches += 2;
       }
       PQB_CUDA(cudaGetLastError());
@@ -2333,7 +2443,9 @@ void Query::run(const PqQueryDesc& d) {
             oc.name = agg_name(a);
             oc.type = agg_out_type[a];
             oc.ext_validity_off = fa.valid_off[a] + uint64_t(b) * wpb * 4;
-            oc.ext_off = fa.val_off[a] + uint64_t(r0) * 8;
+            if (fa.out_kind[a] == DK_STR) { oc.ext_offsets_off = fa.val_off[a] + uint64_t(r0) * 4; oc.ext_off = fa.astr[a].data_off; }
+            else if (fa.out_kind[a] == DK_BOOL) oc.ext_off = fa.val_off[a] + uint64_t(b) * wpb * 4;
+            else oc.ext_off = fa.val_off[a] + uint64_t(r0) * 8;
           }
           ob.cols.push_back(std::move(oc));
         }

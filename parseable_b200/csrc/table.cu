@@ -1392,9 +1392,7 @@ void Table::unify_key(int tcol, cudaStream_t stream) const {
 
 // Query-independent prep like the hot-first numbering of ensure_key: the host copy of the key dictionary is sorted once
 // per column (and once per agreement of the ranks); keys interned from pages without a dictionary are in it too.
-std::shared_ptr<const uint32_t> Table::ensure_kd_rank(int tcol, bool agreed, cudaStream_t stream) const {
-  std::lock_guard<std::mutex> lk(side_mu);
-  ColSide& cs = sides[tcol];
+static std::shared_ptr<const uint32_t> kd_rank_locked(ColSide& cs, bool agreed, cudaStream_t stream) {
   std::shared_ptr<const uint32_t>& r = agreed ? cs.glob_kd_rank : cs.kd_rank;
   if (r) return r;
   const KeyDict& kd = agreed ? cs.glob_kd : cs.kd;
@@ -1406,6 +1404,29 @@ std::shared_ptr<const uint32_t> Table::ensure_kd_rank(int tcol, bool agreed, cud
   r = std::shared_ptr<const uint32_t>(d, [](const uint32_t* p) { cudaFree(const_cast<uint32_t*>(p)); });
   PQB_CUDA(cudaMemcpyAsync(d, rank.data(), rank.size() * 4, cudaMemcpyHostToDevice, stream));
   PQB_CUDA(cudaStreamSynchronize(stream));
+  return r;
+}
+
+std::shared_ptr<const uint32_t> Table::ensure_kd_rank(int tcol, bool agreed, cudaStream_t stream) const {
+  std::lock_guard<std::mutex> lk(side_mu);
+  return kd_rank_locked(sides[tcol], agreed, stream);
+}
+
+RankLuts::~RankLuts() {
+  if (ent) cudaFree(ent);
+  if (ids) cudaFree(ids);
+  if (inv) cudaFree(inv);
+}
+
+std::shared_ptr<const RankLuts> Table::ensure_rank_luts(int tcol, bool agreed, cudaStream_t stream) const {
+  std::lock_guard<std::mutex> lk(side_mu);
+  ColSide& cs = sides[tcol];
+  std::shared_ptr<const RankLuts>& r = agreed ? cs.glob_rank_luts : cs.rank_luts;
+  if (r) return r;
+  const std::shared_ptr<const uint32_t> rank = kd_rank_locked(cs, agreed, stream);
+  auto luts = std::make_shared<RankLuts>();
+  build_rank_luts(cs, agreed, rank.get(), *luts, stream);
+  r = luts;
   return r;
 }
 

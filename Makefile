@@ -16,9 +16,10 @@ LIB       ?= parseable_b200/libparseable_b200.so
 EXTRA     ?=
 
 CU_SRCS   := $(CSRC)/table.cu $(CSRC)/query.cu
-CPP_SRCS  := $(CSRC)/parquet_meta.cpp $(CSRC)/arrow_export.cpp $(CSRC)/capi.cpp $(CSRC)/comm.cpp $(CSRC)/planning.cpp
+CPP_SRCS  := $(CSRC)/parquet_meta.cpp $(CSRC)/arrow_export.cpp $(CSRC)/capi.cpp $(CSRC)/comm.cpp $(CSRC)/planning.cpp \
+             $(CSRC)/regex_compile.cpp
 OBJS      := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(CU_SRCS)) $(patsubst $(CSRC)/%.cpp,$(OBJDIR)/%.o,$(CPP_SRCS))
-HDRS      := $(wildcard $(CSRC)/*.hpp $(CSRC)/*.cuh include/*.h)
+HDRS      := $(wildcard $(CSRC)/*.hpp $(CSRC)/*.cuh $(CSRC)/*.inc include/*.h)
 
 all: $(LIB) oracle tools
 
@@ -37,7 +38,9 @@ oracle: oracle/liboracle.so
 oracle/liboracle.so: oracle/oracle.c
 	$(CC) -O2 -std=c11 -fPIC -shared -Wall -o $@ $< -lm
 
-tools: tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so
+tools: tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so
+tools/libregex_host.so: tools/regex_host.cpp $(CSRC)/regex_compile.cpp $(CSRC)/regex_compile.hpp $(CSRC)/regex_match.cuh $(CSRC)/regex_unicode.inc
+	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 tools/liborder_keys_host.so: tools/order_keys_host.cpp $(CSRC)/order_keys.cuh $(CSRC)/percentile_core.cuh $(CSRC)/decode_core.cuh $(CSRC)/device_structs.hpp
 	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 tools/libjson_host.so: tools/json_host.cpp $(CSRC)/json_egress.cuh $(CSRC)/ryu_f64.cuh $(CSRC)/ryu_tables.inc
@@ -48,6 +51,6 @@ tools/libdecode_core_host.so: tools/decode_core_host.cpp $(CSRC)/decode_core.cuh
 	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 
 clean:
-	rm -rf $(OBJDIR) $(LIB) oracle/liboracle.so tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so
+	rm -rf $(OBJDIR) $(LIB) oracle/liboracle.so tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so
 
 .PHONY: all oracle tools clean

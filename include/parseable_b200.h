@@ -111,13 +111,38 @@ typedef enum {
   PQ_OP_AND = 5,      /* pop 2, push Kleene AND                                       */
   PQ_OP_OR = 6,       /* pop 2, push Kleene OR                                        */
   PQ_OP_NOT = 7,      /* pop 1, push Kleene NOT                                       */
-  PQ_OP_CONST = 8     /* push literal TRUE/FALSE/NULL (lit.type BOOL or NULL)         */
+  PQ_OP_CONST = 8,    /* push literal TRUE/FALSE/NULL (lit.type BOOL or NULL)         */
+  PQ_OP_REGEX = 9     /* push  col ~ pattern  (flags: NOT, case-insens; see below)    */
 } PqOpKind;
 
 typedef enum { PQ_EQ = 0, PQ_NE = 1, PQ_LT = 2, PQ_LE = 3, PQ_GT = 4, PQ_GE = 5 } PqCmp;
 
 #define PQ_LIKE_NEGATED 1u
 #define PQ_LIKE_CASE_INSENSITIVE 2u
+
+/* PQ_OP_REGEX: `col ~ pattern` (`~*` with PQ_REGEX_CASE_INSENSITIVE, `!~` / `!~*` with PQ_REGEX_NEGATED), lit a PQ_T_UTF8
+ * pattern.  DataFusion's regexp_is_match over the regex crate (1.12, regex-syntax 0.8), restated, not checked: an
+ * unanchored search, TRUE when some substring matches.  `regexp_like(col, p, flags)` is the pattern `(?flags)p`.
+ *   - NULL input -> NULL (so `!~` over NULL is NULL too); a column missing from a file reads as NULL; a column that is not
+ *     Utf8 -> PQ_ERR_INVALID_ARG.  The empty pattern matches every non-NULL value, '' included.
+ *   - `.` is any scalar value but `\n` (any under `s`); `^` / `$` are the text's start / end, and under `m` also after /
+ *     before `\n` (`\r` is not special); `\A` / `\z` are always the text's start / end.
+ *   - Syntax: UTF-8 literals; escapes \t \n \r \f \v \a \xHH \x{..} \uHHHH \u{..} \UHHHHHHHH \U{..}; an escaped ASCII
+ *     punctuation character (or space) is itself, except \< and \>; groups (..) (?:..) (?P<n>..) (?<n>..); flag groups
+ *     (?flags) and (?flags:..) over i m s U with `-`; alternation with empty branches; * + ? {n} {n,} {n,m}, greedy or
+ *     lazy; classes [..] [^..] with ranges, escapes and Perl classes (a negated class matches `\n`); \d \s \w \D \S \W
+ *     with their Unicode meanings (\p{Nd}; \p{White_Space}; Alphabetic + M + Nd + Pc + Join_Control); under `i` Unicode
+ *     simple case folding orbits ((?i)k matches U+212A KELVIN SIGN).  Unicode tables are Unicode 15.0: code points first
+ *     assigned later may classify differently from the regex crate's newer tables.
+ *   - PQ_ERR_INVALID_ARG (the message names the byte position): unbalanced ( ) [ ], a quantifier with nothing to repeat,
+ *     {m,n} with m > n, a reversed range, an unknown escape, backreferences, look-around, unknown or duplicate flags,
+ *     duplicate group names, a pattern that is not UTF-8.
+ *   - PQ_ERR_UNSUPPORTED: word boundaries \b \B \< \>, \p{..} / \P{..} classes, [[:alpha:]], nested classes and class
+ *     set operations (&& -- ~~), the flags x R -u, {,m}, nesting deeper than 250, and patterns past the device DFA's caps
+ *     (pattern 64 KiB, 65 536 NFA states, 4 096 DFA states, 1 MiB of table): "regular expression too large for the device
+ *     DFA". */
+#define PQ_REGEX_NEGATED 1u
+#define PQ_REGEX_CASE_INSENSITIVE 2u
 
 typedef struct {
   int32_t type; /* PqType */

@@ -40,6 +40,7 @@
 #include "flat_store.cuh"
 #include "order_keys.cuh"       // order_encode: the value keys of MEDIAN / PERCENTILE_CONT pairs
 #include "ptx_utils.cuh"
+#include "regex_match.cuh"
 #include "scan_kernel.cuh"   // acc_add / acc_apply / acc_merge
 
 namespace pqb {
@@ -180,7 +181,7 @@ __device__ __noinline__ void flat_producer(const DevPlan& plan, const FlatLayout
       const DevLeaf& lf = plan.leaves[l];
       const uint32_t bw = __shfl_sync(0xffffffffu, mycol.bw, lf.col), fk = __shfl_sync(0xffffffffu, mycol.fkind, lf.col);
       const uint32_t dn = __shfl_sync(0xffffffffu, mycol.dict_n, lf.col), lb = __shfl_sync(0xffffffffu, mycol.lut_base, lf.col);
-      if (!((lf.kind == LK_CMP || lf.kind == LK_LIKE) && fk == FK_INDEX && bw <= 5 && dn <= 32)) continue;
+      if (!(value_leaf(lf.kind) && fk == FK_INDEX && bw <= 5 && dn <= 32)) continue;
       const uint8_t* lut = a.luts + lf.lut_off + lb;
       uint32_t r = __ballot_sync(0xffffffffu, lane < dn && lut[lane] != 0);
       for (uint32_t p = 1u << bw; p < 32; p <<= 1) r |= r << p;
@@ -360,7 +361,35 @@ __device__ __forceinline__ bool plain_cmp(uint64_t bits, const LeafCtx& x) {
   return cmp_i64(v, x.lit, x.cmp);
 }
 
-// the comparison for ONE non-NULL row; x.mode is warp uniform, so the switch costs one predictable branch
+// A regular expression over rows without a dictionary: the DFA walk (a dependent table load per byte) stays out of line,
+// so that the register allocation of the kernels around it does not move.  One row (k_flat_filter) ...
+__device__ __noinline__ bool regex_row(const uint8_t* s, uint32_t len, const uint8_t* dfa, uint32_t flags) {
+  return regex_match(s, len, dfa) != ((flags & 1u) != 0);
+}
+// ... or the rows `sel` of one k_flat_agg<.., RX = true> thread (bit i: row row0 + i * kAggConsumers), one call per leaf
+// and slab.  Returns the TRUE rows in the low word, the NULL rows in the high word.
+__device__ __noinline__ uint64_t regex_rows(const uint8_t* vals, const uint32_t* colw, uint32_t phase, const uint32_t* vw,
+                                            uint32_t vphase, const uint8_t* dfa, uint32_t flags, uint32_t sel, uint32_t row0) {
+  uint32_t t = 0, n = 0;
+  for (; sel; sel &= sel - 1) {
+    const uint32_t i = __ffs(sel) - 1, row = row0 + i * kAggConsumers;
+    if (vw) {
+      const uint32_t b = vphase + row;
+      if (!((vw[b >> 5] >> (b & 31)) & 1u)) { n |= 1u << i; continue; }
+    }
+    const uint8_t* sp = vals + bits32_at(colw, phase + row * 32);
+    if (regex_match(sp, load_u32_unaligned(sp - 4), dfa) != ((flags & 1u) != 0)) t |= 1u << i;
+  }
+  return (uint64_t(n) << 32) | t;
+}
+__device__ __forceinline__ uint64_t regex_rows(const LeafCtx& x, uint32_t sel, uint32_t row0) {
+  return regex_rows(x.lut, x.c.colw, x.c.phase, x.c.vw, x.c.vphase, x.lit_pool + x.lf->str_off, x.lf->flags, sel, row0);
+}
+
+// the comparison for ONE non-NULL row; x.mode is warp uniform, so the switch costs one predictable branch.
+// REGEX = false: no DFA walk here (k_flat_agg answers LK_REGEX leaves on LM_BYTES pages with regex_rows, in its RX
+// instantiations only)
+template <bool REGEX = true>
 __device__ __forceinline__ bool leaf_row(const LeafCtx& x, uint32_t row) {
   switch (x.mode) {
     case LM_FALSE: return false;
@@ -374,6 +403,7 @@ __device__ __forceinline__ bool leaf_row(const LeafCtx& x, uint32_t row) {
       const uint32_t len = load_u32_unaligned(sp - 4);
       const uint8_t* needle = x.lit_pool + x.lf->str_off;
       if (x.lkind == LK_CMP) return cmp_result(cmp_bytes(sp, len, needle, x.lf->str_len), x.cmp);
+      if (REGEX && x.lkind == LK_REGEX) return regex_row(sp, len, needle, x.lf->flags);
       const bool t = like_match(sp, len, needle, x.lf->str_len, x.cmp, (x.lf->flags & 2u) != 0);
       return (x.lf->flags & 1u) ? !t : t;
     }
@@ -384,12 +414,13 @@ __device__ __forceinline__ bool leaf_row(const LeafCtx& x, uint32_t row) {
   }
 }
 // SQL truth of the leaf for one row: 1 TRUE, 0 FALSE, 2 NULL
+template <bool REGEX = true>
 __device__ __forceinline__ uint32_t leaf_row3(const LeafCtx& x, uint32_t row) {
   const bool v = col_valid(x.c, row);
   if (x.lkind == LK_IS_NULL) return v ? 0u : 1u;
   if (x.lkind == LK_IS_NOT_NULL) return v ? 1u : 0u;
   if (!v) return 2u;
-  return leaf_row(x, row) ? 1u : 0u;
+  return leaf_row<REGEX>(x, row) ? 1u : 0u;
 }
 
 // knock the rows of `m` (bit k = row row0 + k, all non-NULL) out that fail the comparison: one trip per surviving row
@@ -858,9 +889,10 @@ __device__ __forceinline__ void pct_emit(const DevPairSet& ps, uint32_t vsel, co
     }
 }
 
-// DIST: the instantiation with the COUNT(DISTINCT) pass, PCT: the one with the MEDIAN / PERCENTILE_CONT pair emission
-// (queries without them run code that does not contain them)
-template <int KR, bool HASHED, bool DIST = false, bool PCT = false>
+// DIST: the instantiation with the COUNT(DISTINCT) pass, PCT: the one with the MEDIAN / PERCENTILE_CONT pair emission,
+// RX: the one with the DFA walk of a regular expression over pages without a dictionary (queries without them run code
+// that does not contain them)
+template <int KR, bool HASHED, bool DIST = false, bool PCT = false, bool RX = false>
 __global__ void __launch_bounds__(kAggThreads, 1)
 k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLayout L, const __grid_constant__ DevScanArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -910,14 +942,16 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
             LeafCtx x;
             leaf_ctx<true>(x, plan, a, st, base, L, l);
             uint32_t m = 0;
-            if (!x.c.absent && !x.c.vw && x.lkind != LK_IS_NULL && x.lkind != LK_IS_NOT_NULL) {   // no NULLs in this slab: plain comparison
+            if (RX && x.mode == LM_BYTES && x.lkind == LK_REGEX) {
+              m = uint32_t(regex_rows(x, sel, tc));
+            } else if (!x.c.absent && !x.c.vw && x.lkind != LK_IS_NULL && x.lkind != LK_IS_NOT_NULL) {   // no NULLs in this slab: plain comparison
 #pragma unroll
               for (int i = 0; i < KR; i++)
-                if ((sel >> i) & 1u) m |= (leaf_row(x, tc + i * kAggConsumers) ? 1u : 0u) << i;
+                if ((sel >> i) & 1u) m |= (leaf_row<false>(x, tc + i * kAggConsumers) ? 1u : 0u) << i;
             } else {
 #pragma unroll
               for (int i = 0; i < KR; i++)
-                if ((sel >> i) & 1u) m |= (leaf_row3(x, tc + i * kAggConsumers) == 1u ? 1u : 0u) << i;
+                if ((sel >> i) & 1u) m |= (leaf_row3<false>(x, tc + i * kAggConsumers) == 1u ? 1u : 0u) << i;
             }
             sel = m;
           }
@@ -931,10 +965,14 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
               LeafCtx x;
               leaf_ctx<true>(x, plan, a, st, base, L, op.arg);
               Tri32 v{0u, 0u};
+              if (RX && x.mode == LM_BYTES && x.lkind == LK_REGEX) {
+                const uint64_t r = regex_rows(x, sel, tc);
+                v = {uint32_t(r), uint32_t(r >> 32)};
+              } else
 #pragma unroll
               for (int j = 0; j < KR; j++)
                 if ((sel >> j) & 1u) {
-                  const uint32_t t3 = leaf_row3(x, tc + j * kAggConsumers);
+                  const uint32_t t3 = leaf_row3<false>(x, tc + j * kAggConsumers);
                   v.t |= (t3 == 1u ? 1u : 0u) << j;
                   v.n |= (t3 == 2u ? 1u : 0u) << j;
                 }

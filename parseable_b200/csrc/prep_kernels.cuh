@@ -11,6 +11,7 @@
 
 #include "decode_core.cuh"
 #include "device_structs.hpp"
+#include "regex_match.cuh"
 
 namespace pqb {
 
@@ -103,7 +104,7 @@ __global__ void k_leaf_luts(DevPrepArgs a, const __grid_constant__ DevPlan plan)
   for (uint32_t e = blockIdx.y * blockDim.x + threadIdx.x; e < ch.dict_n; e += gridDim.y * blockDim.x) {
     for (uint32_t l = 0; l < plan.nleaves; l++) {
       const DevLeaf& lf = plan.leaves[l];
-      if (lf.col != col || (lf.kind != LK_CMP && lf.kind != LK_LIKE)) continue;
+      if (lf.col != col || !value_leaf(lf.kind)) continue;
       bool t;
       if (kind == DK_STR) {
         uint64_t off = a.ent[col][ch.lut_base + e];
@@ -111,6 +112,7 @@ __global__ void k_leaf_luts(DevPrepArgs a, const __grid_constant__ DevPlan plan)
         const uint8_t* s = a.arena + off;
         const uint8_t* lit = a.lit_pool + lf.str_off;
         if (lf.kind == LK_CMP) t = cmp_result(cmp_bytes(s, len, lit, lf.str_len), lf.cmp);
+        else if (lf.kind == LK_REGEX) t = regex_match(s, len, lit) != ((lf.flags & 1u) != 0);   // once per dictionary entry
         else {
           t = like_match(s, len, lit, lf.str_len, lf.cmp, (lf.flags & 2u) != 0);
           if (lf.flags & 1u) t = !t;

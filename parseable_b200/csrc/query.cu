@@ -31,6 +31,7 @@
 #include "egress_kernels.cuh"
 #include "order_kernels.cuh"
 #include "percentile_kernels.cuh"
+#include "regex_compile.hpp"
 
 namespace pqb {
 
@@ -976,7 +977,7 @@ void Query::run(const PqQueryDesc& d) {
     for (uint32_t i = 0; i < d.n_pred; i++) {
       const PqPredOp& op = d.pred[i];
       switch (op.kind) {
-        case PQ_OP_CMP: case PQ_OP_IS_NULL: case PQ_OP_IS_NOT_NULL: case PQ_OP_LIKE: {
+        case PQ_OP_CMP: case PQ_OP_IS_NULL: case PQ_OP_IS_NOT_NULL: case PQ_OP_LIKE: case PQ_OP_REGEX: {
           if (op.col < 0 || uint32_t(op.col) >= d.n_columns) throw Error(PQ_ERR_INVALID_ARG, "predicate column out of range");
           if (leaves.size() >= (size_t)kMaxLeaves) throw Error(PQ_ERR_UNSUPPORTED, "too many leaf predicates");
           HostLeaf lf;
@@ -993,6 +994,17 @@ void Query::run(const PqQueryDesc& d) {
             lf.d.cmp = uint8_t(lp.kind);
             lf.d.flags = op.flags;
             lf.str = lp.needle;
+          } else if (op.kind == PQ_OP_REGEX) {
+            if (kind != DK_STR) throw Error(PQ_ERR_INVALID_ARG, "a regular expression match needs a Utf8 column");
+            if (op.lit.type != PQ_T_UTF8) throw Error(PQ_ERR_INVALID_ARG, "a regular expression match needs a Utf8 pattern");
+            std::vector<uint8_t> blob;
+            std::string err;
+            const int st = regex_compile(op.lit.str, op.lit.str ? op.lit.str_len : 0, (op.flags & PQ_REGEX_CASE_INSENSITIVE) != 0,
+                                         blob, err);
+            if (st != 0) throw Error(st, err);
+            lf.d.kind = LK_REGEX;
+            lf.d.flags = op.flags;
+            lf.str.assign(blob.begin(), blob.end());   // the DFA travels in the literal pool (8-aligned: see below)
           } else {
             lf.d.kind = LK_CMP;
             if (op.cmp < PQ_EQ || op.cmp > PQ_GE) throw Error(PQ_ERR_INVALID_ARG, "bad comparison operator");
@@ -1047,8 +1059,8 @@ void Query::run(const PqQueryDesc& d) {
               default: throw Error(PQ_ERR_UNSUPPORTED, "comparison on this column type");
             }
           }
-          if (kind == DK_STR && (lf.d.kind == LK_CMP || lf.d.kind == LK_LIKE)) {
-            lf.d.str_off = uint32_t(lit_pool.size());
+          if (kind == DK_STR && value_leaf(lf.d.kind)) {
+            lf.d.str_off = uint32_t(lit_pool.size());   // a multiple of 8: the pool starts at 16 and every entry is padded to 8
             lf.d.str_len = uint32_t(lf.str.size());
             lit_pool.insert(lit_pool.end(), lf.str.begin(), lf.str.end());
             lit_pool.resize(align_up(uint32_t(lit_pool.size()) + 8, 8), 0);
@@ -1197,7 +1209,7 @@ void Query::run(const PqQueryDesc& d) {
   for (uint32_t c = 0; c < (uint32_t)kMaxCols; c++) { plan.col_nlut[c] = 0; plan.col_l0[c] = -1; plan.col_l1[c] = -1; }
   for (uint32_t l = 0; l < nleaves; l++) {
     const DevLeaf& lf = plan.leaves[l];
-    if (lf.kind != LK_CMP && lf.kind != LK_LIKE) continue;
+    if (!value_leaf(lf.kind)) continue;
     if (plan.col_nlut[lf.col] == 0) plan.col_l0[lf.col] = int8_t(l);
     else if (plan.col_nlut[lf.col] == 1) plan.col_l1[lf.col] = int8_t(l);
     plan.col_nlut[lf.col]++;
@@ -1209,7 +1221,7 @@ void Query::run(const PqQueryDesc& d) {
   {
     // k_scan: conjunction of 1-4 CMP/LIKE leaves: specialised octet pass over slab-indexed pages
     bool c4 = conj && nleaves >= 1 && nleaves <= 4;
-    for (uint32_t l = 0; l < nleaves; l++) c4 &= plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE;
+    for (uint32_t l = 0; l < nleaves; l++) c4 &= value_leaf(plan.leaves[l].kind);
     const char* fa = getenv("PQB_FAST_AND");
     plan.fast_and = c4 && !(fa && fa[0] == '0');
   }
@@ -1330,7 +1342,7 @@ void Query::run(const PqQueryDesc& d) {
   std::vector<uint8_t> col_needs_ent(ncols, 0);  // entry offsets (string leaf)
   for (uint32_t l = 0; l < nleaves; l++) {
     const DevLeaf& lf = plan.leaves[l];
-    if ((lf.kind == LK_CMP || lf.kind == LK_LIKE) && plan.cols[lf.col].kind == DK_STR) col_needs_ent[lf.col] = 1;
+    if (value_leaf(lf.kind) && plan.cols[lf.col].kind == DK_STR) col_needs_ent[lf.col] = 1;
   }
   uint64_t algo_bytes = 0, scanned_bytes = 0;
   std::vector<uint8_t> col_has_nulls(std::max<uint32_t>(ncols, 1), 0);   // statistics cannot rule NULLs out
@@ -1356,6 +1368,9 @@ void Query::run(const PqQueryDesc& d) {
     if (shape->has_plain[s] && plan.cols[s].kind == DK_STR && shape->n_general)
       throw Error(PQ_ERR_UNSUPPORTED, "column '" + cname + "': PLAIN (dictionary-fallback) string pages without a flat-store copy are not decoded on the GPU");
   }
+  // k_flat_agg walks a regular expression's DFA per row only in its RX instantiations
+  bool rx_bytes = false;
+  for (uint32_t l = 0; l < nleaves; l++) rx_bytes |= plan.leaves[l].kind == LK_REGEX && plan.cols[plan.leaves[l].col].has_plain;
   plan.n_items = uint32_t(items.size());
   metrics.bytes_scanned = scanned_bytes;
   const bool allreduce = (d.flags & PQ_QUERY_ALLREDUCE) != 0;
@@ -1422,7 +1437,7 @@ void Query::run(const PqQueryDesc& d) {
   for (uint32_t l = 0; l < nleaves; l++) {
     DevLeaf& lf = plan.leaves[l];
     lf.lut_off = 0;
-    if (lf.kind != LK_CMP && lf.kind != LK_LIKE) continue;
+    if (!value_leaf(lf.kind)) continue;
     const ColSide& cs = table->sides[shape_cols[lf.col]];
     if (lut_total + cs.total_entries > 0xfffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "leaf LUTs too large");
     lf.lut_off = uint32_t(lut_total);
@@ -1497,7 +1512,7 @@ void Query::run(const PqQueryDesc& d) {
       // their ROWS next to the dictionary entries; the aggregate kernel then stages the pages' ids instead of their values,
       // so nothing else of this query may read the column's values
       for (uint32_t l = 0; l < nleaves; l++)
-        if (plan.leaves[l].col == key.col && (plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE))
+        if (plan.leaves[l].col == key.col && value_leaf(plan.leaves[l].kind))
           throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[tcol[d.group_by[k]]].name + "' has pages without a dictionary and is also filtered on: not on the GPU path");
       for (uint32_t a = 0; a < d.n_aggs; a++)
         if (((plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG) || plan.aggs[a].fn >= AG_MEDIAN) && plan.aggs[a].col == key.col &&
@@ -1542,7 +1557,7 @@ void Query::run(const PqQueryDesc& d) {
     if (plan.cols[ds.col].has_plain || plan.cols[ds.col].has_delta) {
       // the id pages stand in for the values, as for a key column: nothing else of this query may read them
       for (uint32_t l = 0; l < nleaves; l++)
-        if (plan.leaves[l].col == ds.col && (plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE))
+        if (plan.leaves[l].col == ds.col && value_leaf(plan.leaves[l].kind))
           throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + cname + "): the column has pages without a dictionary and is also filtered on: not on the GPU path");
       for (uint32_t a = 0; a < d.n_aggs; a++)
         if (plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG && plan.aggs[a].col == ds.col && !rank_min_max(plan.aggs[a]))
@@ -1579,7 +1594,7 @@ void Query::run(const PqQueryDesc& d) {
       const bool row_ids = plan.cols[ag.col].has_plain || plan.cols[ag.col].has_delta;
       if (row_ids)
         for (uint32_t l = 0; l < nleaves; l++)
-          if (plan.leaves[l].col == ag.col && (plan.leaves[l].kind == LK_CMP || plan.leaves[l].kind == LK_LIKE))
+          if (plan.leaves[l].col == ag.col && value_leaf(plan.leaves[l].kind))
             throw Error(PQ_ERR_UNSUPPORTED, std::string(ag.fn == AG_MIN ? "MIN(" : "MAX(") + table->columns[tc_i].name +
                                                 "): the column has pages without a dictionary and is also filtered on: not on the GPU path");
       table->ensure_key(tc_i, stream);
@@ -1922,6 +1937,7 @@ void Query::run(const PqQueryDesc& d) {
       // one CTA per SM: the hot part of the accumulator table next to the stages
       const uint64_t full = plan.hashed ? 0 : uint64_t(plan.nslots) * cells * 8;   // hashed: no hot table in shared memory
       uint32_t krows = plan.hashed ? 4 : 8;   // the hashed instantiation exists for 4 rows per thread (64-bit slots: registers)
+      if (rx_bytes && !plan.hashed) krows = 2;   // so do the RX ones, and for 2 when not hashed
       if (const char* e = plan.hashed ? nullptr : getenv("PQB_AGG_KROWS")) krows = std::max(1, std::min(8, atoi(e)));   // experiment switch
       while (krows & (krows - 1)) krows &= krows - 1;
       while (krows > 1 && 2 * stage_bytes_for(kAggConsumers * krows) + std::min<uint64_t>(full, 96 * 1024) > avail) krows >>= 1;
@@ -2062,7 +2078,17 @@ void Query::run(const PqQueryDesc& d) {
         PQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(ctx.smem_optin())));
         kern<<<grid, kAggThreads, FL.total, stream>>>(plan, FL, sa);
       };
-      if (plan.npct) {   // MEDIAN / PERCENTILE_CONT: the instantiations with the pair emission
+      if (rx_bytes) {   // a regular expression over pages without a dictionary: the instantiations with the DFA walk
+        if (plan.npct) {
+          if (plan.hashed) go(k_flat_agg<4, true, false, true, true>);
+          else go(k_flat_agg<2, false, false, true, true>);
+        } else if (plan.ndist) {
+          if (plan.hashed) go(k_flat_agg<4, true, true, false, true>);
+          else go(k_flat_agg<2, false, true, false, true>);
+        } else if (plan.hashed) go(k_flat_agg<4, true, false, false, true>);
+        else go(k_flat_agg<2, false, false, false, true>);
+      }
+      else if (plan.npct) {   // MEDIAN / PERCENTILE_CONT: the instantiations with the pair emission
         if (plan.hashed) go(k_flat_agg<4, true, false, true>);
         else if (plan.flat_krows >= 8) go(k_flat_agg<8, false, false, true>);
         else if (plan.flat_krows >= 4) go(k_flat_agg<4, false, false, true>);

@@ -1126,7 +1126,7 @@ __device__ __forceinline__ void row_phase(const DevPlan& plan, ScanCtl& ctl, con
   // ---- 5. leaves the fused pass did not answer: PLAIN pages, NULL-carrying slabs, booleans ----
   for (uint32_t l = 0; l < plan.nleaves; l++) {
     const DevLeaf& lf = plan.leaves[l];
-    if (lf.kind != LK_CMP && lf.kind != LK_LIKE) continue;   // IS [NOT] NULL comes from the validity words
+    if (!value_leaf(lf.kind)) continue;   // IS [NOT] NULL comes from the validity words
     const SlabCol& s = ctl.slab[buf][lf.col];
     if (!s.present) continue;                                 // all NULL: T stays 0
     if (s.enc == DE_DICT && s.all_valid && plan.col_nlut[lf.col] <= 2) continue;  // answered by the fused pass

@@ -38,7 +38,7 @@ class QueryError(RuntimeError):
 # ----------------------------------------------------------------------------- expressions
 @dataclass
 class Expr:
-    kind: str                      # 'col' 'lit' 'cmp' 'and' 'or' 'not' 'is_null' 'is_not_null' 'like'
+    kind: str                      # 'col' 'lit' 'cmp' 'and' 'or' 'not' 'is_null' 'is_not_null' 'like' 'regex'
     args: tuple = ()
     op: int = 0
     flags: int = 0
@@ -65,6 +65,11 @@ class Expr:
 
     def ilike(self, pattern: str, negated=False):
         return self.like(pattern, negated, True)
+
+    def regex(self, pattern: str, negated=False, case_insensitive=False):
+        """``col ~ pattern`` (``~*``, ``!~``, ``!~*``): an unanchored regular-expression search (PQ_OP_REGEX)."""
+        f = (L.PQ_REGEX_NEGATED if negated else 0) | (L.PQ_REGEX_CASE_INSENSITIVE if case_insensitive else 0)
+        return Expr("regex", (self, Expr("lit", (pattern,))), flags=f)
 
 
 def col(name: str) -> Expr:
@@ -220,12 +225,14 @@ class _Desc:
                 raise QueryError(L.PQ_ERR_UNSUPPORTED, "IS NULL on a non-column expression")
             ops.append(L.PqPredOp(kind=L.PQ_OP_IS_NULL if e.kind == "is_null" else L.PQ_OP_IS_NOT_NULL,
                                   col=self.col_index(c.args[0])))
-        elif e.kind == "like":
+        elif e.kind in ("like", "regex"):
             c, p = e.args
             if c.kind != "col":
-                raise QueryError(L.PQ_ERR_UNSUPPORTED, "LIKE on a non-column expression")
-            ops.append(L.PqPredOp(kind=L.PQ_OP_LIKE, col=self.col_index(c.args[0]), flags=e.flags,
-                                  lit=self.literal(p.args[0])))
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, f"{e.kind.upper()} on a non-column expression")
+            if p.kind != "lit" or not isinstance(p.args[0], (str, bytes)):
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, f"{e.kind.upper()} with a pattern that is not a string literal")
+            ops.append(L.PqPredOp(kind=L.PQ_OP_LIKE if e.kind == "like" else L.PQ_OP_REGEX, col=self.col_index(c.args[0]),
+                                  flags=e.flags, lit=self.literal(p.args[0])))
         elif e.kind == "cmp":
             a, b = e.args
             op = e.op
@@ -633,7 +640,7 @@ class Query:
         self._parse(sql)
 
     # --- tokenizer / parser ---
-    _TOK = re.compile(r"\s*(?:(-?\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+)|'((?:[^']|'')*)'|\"([^\"]+)\"|([A-Za-z_][A-Za-z_0-9]*)|(<=|>=|<>|!=|[=<>(),*]))")
+    _TOK = re.compile(r"\s*(?:(-?\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+)|'((?:[^']|'')*)'|\"([^\"]+)\"|([A-Za-z_][A-Za-z_0-9]*)|(<=|>=|<>|!~\*|!~|~\*|!=|~|[=<>(),*]))")
 
     def _parse(self, sql: str):
         toks, pos = [], 0
@@ -812,6 +819,8 @@ class Query:
             item = self._pct_call()
             alias = self._next("id")[1] if self._accept("kw", "AS") else None
             return ("agg", item, alias)
+        if self._peek()[0] == "id" and self._peek(1) == ("op", "(") and self._peek()[1].lower().startswith("regexp_"):
+            raise QueryError(L.PQ_ERR_UNSUPPORTED, f"{self._peek()[1]}(...) as a projected value is not on the GPU path")
         name = self._next("id")[1]
         alias = self._next("id")[1] if self._accept("kw", "AS") else None
         return ("col", name, alias)
@@ -850,13 +859,45 @@ class Query:
             return lit(None)
         raise QueryError(L.PQ_ERR_INVALID_ARG, f"unexpected token {t!r}")
 
+    def _regexp_like(self):
+        """``regexp_like(col, 'pattern' [, 'flags'])``: the pattern with ``(?flags)`` in front, as arrow-string builds it."""
+        self._i += 1
+        self._expect("op", "(")
+        t = self._next("id") if self._peek()[0] == "id" else None
+        if t is None:
+            raise QueryError(L.PQ_ERR_UNSUPPORTED, "regexp_like over an expression that is not a column")
+        self._expect("op", ",")
+        if self._peek()[0] != "str" or self._peek(1) not in (("op", ","), ("op", ")")):
+            raise QueryError(L.PQ_ERR_UNSUPPORTED, "regexp_like with a pattern that is not a string literal")
+        p = self._next("str")[1]
+        if self._accept("op", ","):
+            if self._peek()[0] != "str":
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, "regexp_like with flags that are not a string literal")
+            flags = self._next("str")[1]
+            if "g" in flags:
+                raise QueryError(L.PQ_ERR_INVALID_ARG, "regexp_like() does not support the \"global\" option")
+            if not flags:
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, "regexp_like with an empty flags string")
+            p = f"(?{flags}){p}"
+        self._expect("op", ")")
+        return col(t[1]).regex(p)
+
     def _primary(self):
         if self._accept("op", "("):
             e = self._or()
             self._expect("op", ")")
             return e
+        if self._peek()[0] == "id" and self._peek()[1].lower() == "regexp_like" and self._peek(1) == ("op", "("):
+            return self._regexp_like()
         a = self._value()
         t = self._peek()
+        if t[0] == "op" and t[1] in _REGEX_OPS:
+            self._i += 1
+            b = self._value()
+            if a.kind != "col" or b.kind != "lit" or not isinstance(b.args[0], str):
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, f"{t[1]} needs a column on the left and a string literal pattern")
+            neg, ci = _REGEX_OPS[t[1]]
+            return a.regex(b.args[0], negated=neg, case_insensitive=ci)
         if t[0] == "op" and t[1] in _CMP:
             self._i += 1
             b = self._value()
@@ -890,6 +931,7 @@ class Query:
 _KEYWORDS = {"SELECT", "FROM", "WHERE", "GROUP", "BY", "AND", "OR", "NOT", "LIKE", "ILIKE", "IS", "NULL", "COUNT",
              "SUM", "MIN", "MAX", "AVG", "AS", "LIMIT", "TRUE", "FALSE", "ESCAPE",
              "DISTINCT"}
+_REGEX_OPS = {"~": (False, False), "~*": (False, True), "!~": (True, False), "!~*": (True, True)}   # (negated, case-insens)
 _CMP = {"=": L.PQ_EQ, "!=": L.PQ_NE, "<>": L.PQ_NE, "<": L.PQ_LT, "<=": L.PQ_LE, ">": L.PQ_GT, ">=": L.PQ_GE}
 
 

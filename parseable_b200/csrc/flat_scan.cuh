@@ -1127,7 +1127,8 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
         // one straight-line loop per aggregate function
         uint64_t bits[KR];
         // a value page (FK_FOR): the values are in the stage, no load at all.  Not in the COUNT(DISTINCT) or percentile
-        // instantiations (the planner gives those queries no agg pages): there it spilled registers at the 64-register cap
+        // instantiations (the planner gives those queries no agg pages): there it spilled registers at the 64-register cap.
+        // All KR rows are decoded, selected or not: the planner gives value pages only to slabs of KR x kAggConsumers rows
         if (plain) {
 #pragma unroll
           for (int i = 0; i < KR; i++) bits[i] = ((vsel >> i) & 1u) ? __ldg(v8 + tc + i * kAggConsumers) : 0ull;   // in place in the flat store (global)

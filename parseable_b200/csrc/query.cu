@@ -210,6 +210,14 @@ uint32_t align_up(uint32_t v, uint32_t a) { return (v + a - 1) & ~(a - 1); }
 bool rank_min_max(const DevAgg& ag) { return (ag.fn == AG_MIN || ag.fn == AG_MAX) && ag.kind == DK_STR; }
 bool bool_min_max(const DevAgg& ag) { return (ag.fn == AG_MIN || ag.fn == AG_MAX) && ag.kind == DK_BOOL; }
 
+// KR (rows per thread) of the k_flat_agg instantiation the launch picks for `krows` rows per thread and slab: the
+// hashed ones exist for 4, the RX ones for 2 when not hashed, the others for 8, 4 and 2
+uint32_t agg_kr(const DevPlan& plan, bool rx, uint32_t krows) {
+  if (plan.hashed) return 4;
+  if (rx) return 2;
+  return krows >= 8 ? 8 : krows >= 4 ? 4 : 2;
+}
+
 }  // namespace
 
 Query::Query(const PqQueryDesc& d) {
@@ -1807,6 +1815,7 @@ void Query::run(const PqQueryDesc& d) {
   // need no dictionary or gid LUT load.  They are built once per column and kept with the table, so only a resident
   // table gets them: a file list opens its table for one query, which would pay the build every time ----
   std::vector<uint32_t> form_bw(ncols, 0);   // marked slots: widest page the slot stages
+  uint32_t value_forms = 0;                  // the marked slots that read value pages (FK_FOR)
   plan.agg_forms = 0;
   {
     const char* sw = getenv("PQB_AGG_FORMS");   // A/B switch: 0 = every slot reads its index pages
@@ -1837,6 +1846,7 @@ void Query::run(const PqQueryDesc& d) {
           const uint8_t kind = plan.cols[s].kind;
           if ((kind != DK_I64 && kind != DK_F64) || !table->ensure_for_pages(tc_i, kind == DK_F64, stream)) continue;
           form_bw[s] = std::max(cs.for_bw, cs.for_rest_bw);
+          value_forms |= 1u << s;
         } else {
           // id pages hold the local numbering: a query in the ranks' agreed numbering keeps the gid LUT
           if (plan.keys[key].gid != cs.d_gid || !table->ensure_id_pages(tc_i, stream)) continue;
@@ -1936,11 +1946,27 @@ void Query::run(const PqQueryDesc& d) {
     } else {
       // one CTA per SM: the hot part of the accumulator table next to the stages
       const uint64_t full = plan.hashed ? 0 : uint64_t(plan.nslots) * cells * 8;   // hashed: no hot table in shared memory
-      uint32_t krows = plan.hashed ? 4 : 8;   // the hashed instantiation exists for 4 rows per thread (64-bit slots: registers)
-      if (rx_bytes && !plan.hashed) krows = 2;   // so do the RX ones, and for 2 when not hashed
-      if (const char* e = plan.hashed ? nullptr : getenv("PQB_AGG_KROWS")) krows = std::max(1, std::min(8, atoi(e)));   // experiment switch
-      while (krows & (krows - 1)) krows &= krows - 1;
-      while (krows > 1 && 2 * stage_bytes_for(kAggConsumers * krows) + std::min<uint64_t>(full, 96 * 1024) > avail) krows >>= 1;
+      auto fit_krows = [&]() {
+        uint32_t krows = plan.hashed ? 4 : 8;   // the hashed instantiation exists for 4 rows per thread (64-bit slots: registers)
+        if (rx_bytes && !plan.hashed) krows = 2;   // so do the RX ones, and for 2 when not hashed
+        if (const char* e = plan.hashed ? nullptr : getenv("PQB_AGG_KROWS")) krows = std::max(1, std::min(8, atoi(e)));   // experiment switch
+        while (krows & (krows - 1)) krows &= krows - 1;
+        while (krows > 1 && 2 * stage_bytes_for(kAggConsumers * krows) + std::min<uint64_t>(full, 96 * 1024) > avail) krows >>= 1;
+        return krows;
+      };
+      uint32_t krows = fit_krows();
+      // A thread decodes a value page for all KR rows of its instantiation, selected or not (a row mask there made the
+      // <8> instantiation spill more): over a slab of fewer than KR x kAggConsumers rows its last rows would lie past
+      // the stage -- in the next stage, or past the CTA's shared memory.  The hashed instantiation is <4> and the
+      // narrowest dense one <2>, so a query whose stages leave room for fewer rows per thread reads index pages.
+      if (agg_kr(plan, rx_bytes, krows) > krows && (plan.agg_forms & value_forms)) {
+        if (verbose)
+          fprintf(stderr, "[pqb] value pages off: k_flat_agg<%u> is wider than its %u-row slab\n", agg_kr(plan, rx_bytes, krows),
+                  kAggConsumers * krows);
+        plan.agg_forms &= ~value_forms;
+        value_forms = 0;
+        krows = fit_krows();
+      }
       const uint32_t S = kAggConsumers * krows;
       FL.stage_bytes = stage_bytes_for(S);
       if (2 * FL.stage_bytes + cells * 8 > avail) throw Error(PQ_ERR_UNSUPPORTED, "query needs more shared memory than one SM has");
@@ -2119,10 +2145,16 @@ void Query::run(const PqQueryDesc& d) {
     }
     PQB_CUDA(cudaGetLastError());
     launches++;
-    if (verbose)
-      fprintf(stderr, "[pqb] %s: %u CTAs, %u B smem/CTA, %u stages x %u B, slab %u rows, hot slots %u of %u, %u copies, %u flat items\n",
-              agg_kernel ? "k_flat_agg" : "k_flat_filter", grid, FL.total, FL.nstages, FL.stage_bytes, plan.flat_slab_rows, plan.hot_slots,
-              plan.nslots, plan.replicas, n_flat);
+    if (verbose && agg_kernel)
+      fprintf(stderr, "[pqb] k_flat_agg<%u%s%s%s%s>: %u CTAs, %u B smem/CTA, %u stages x %u B, slab %u rows, hot slots %u of %u, "
+              "lane slots %u, %u copies, smem share %u, f64 global %u, value-page slots %d, id-page slots %d, %u flat items\n",
+              agg_kr(plan, rx_bytes, plan.flat_krows), plan.hashed ? ",hashed" : "", plan.ndist ? ",DIST" : "", plan.npct ? ",PCT" : "",
+              rx_bytes ? ",RX" : "", grid, FL.total, FL.nstages, FL.stage_bytes, plan.flat_slab_rows, plan.hot_slots, plan.nslots,
+              plan.lane_slots, plan.replicas, plan.smem_share, plan.f64_global, __builtin_popcount(plan.agg_forms & value_forms),
+              __builtin_popcount(plan.agg_forms & ~value_forms), n_flat);
+    else if (verbose)
+      fprintf(stderr, "[pqb] k_flat_filter: %u CTAs, %u B smem/CTA, %u stages x %u B, slab %u rows, hot slots %u of %u, %u copies, %u flat items\n",
+              grid, FL.total, FL.nstages, FL.stage_bytes, plan.flat_slab_rows, plan.hot_slots, plan.nslots, plan.replicas, n_flat);
   }
   if (n_general && nrg) {
     if (n_flat) { PQB_CUDA(cudaMemsetAsync(d_counters.p + 2, 0, 8, stream)); }   // the work-queue head

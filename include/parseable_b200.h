@@ -260,6 +260,42 @@ typedef struct {
   int32_t _pad;
 } PqOrderBy;
 
+/* ---- ROW_NUMBER() OVER (PARTITION BY ... ORDER BY ...) cut to a rank range, on the device: the top N rows of every
+ *      partition (BoundedWindowAggExec(ROW_NUMBER / COUNT(*) OVER) + FilterExec(rn range) above the aggregate or scan) ----
+ * The window's ORDER BY is the query's order_by array; partition_by holds the PARTITION BY terms in the same PqOrderBy
+ * form, checked the same way: an aggregate query takes PQ_ORDER_KEY terms (GROUP BY keys, DATE_BIN included), a scan
+ * PQ_ORDER_COLUMN terms (the column need not be projected).  A partition term's flags order the partitions in the
+ * output.  Partition and order terms together are at most 8 (more: PQ_ERR_UNSUPPORTED).
+ * Partitions: two rows share one when every partition term has the same value and NULL flag, GROUP BY equality: NULLs
+ * are one partition, Float64 compares by bit pattern (-0.0 and 0.0 are two partitions, so are NaNs of different
+ * payloads), Utf8 by bytes, a DATE_BIN key by bin.
+ * Ranking: row_number rn counts 1, 2, ... within a partition in the order of the order_by terms; ties keep the order
+ * the query has without a window (as ORDER BY states above: slot order, or file then row order), and with no order_by
+ * terms that order is the ranking.  Under a hashed GROUP BY the order of tied rows may differ from one query to the next.
+ * Output: the rows with offset < rn <= offset + fetch (fetch < 0: no upper bound), ordered by the partition terms and
+ * then the window's order; `limit` (>= 0) then keeps the first `limit` of them (the outer LIMIT), for aggregates too.
+ * PQ_WINDOW_ROW_NUMBER appends an Int64 column "row_number", PQ_WINDOW_PARTITION_ROWS an Int64 column "partition_rows"
+ * (COUNT(*) OVER (PARTITION BY ...): the partition's rows before the cut), in that order: after the keys and aggregates,
+ * or after a scan's projection and __row_id.  Neither is ever NULL.
+ * Scans: a window needs no `limit`; the caps of a scan ORDER BY hold (2^32 - 1 selected rows, 2^31 projected rows, a
+ * flat-store copy of every page read).  Under row-group or file sharding every shard ranks and cuts its own selection;
+ * merging the shards' rows is the caller's.  Aggregates: the window runs after the all-reduce (every rank of a
+ * PQ_QUERY_ALLREDUCE query returns the same rows), and takes every aggregate ORDER BY takes as a term.
+ * rows_selected and groups_total count the rows before any cut; the window's kernels count into order_ms and
+ * kernel_launches.  Errors: offset < 0, unknown flags, a bad term index or target, or a window with PQ_QUERY_COUNT_ONLY
+ * return PQ_ERR_INVALID_ARG (a PQ_ORDER_KEY / PQ_ORDER_AGG partition term on a scan: PQ_ERR_UNSUPPORTED, as for order_by).
+ * Paths: without partition terms the window is ORDER BY ... LIMIT offset + fetch with the first `offset` rows dropped;
+ * with them every row is sorted by (partition terms, order terms), and one host round trip reads the kept count. */
+#define PQ_WINDOW_ROW_NUMBER 1u       /* append Int64 "row_number" (1-based, within the partition) */
+#define PQ_WINDOW_PARTITION_ROWS 2u   /* append Int64 "partition_rows" = COUNT(*) OVER (PARTITION BY ...), before the cut */
+typedef struct {
+  const PqOrderBy* partition_by;  /* PARTITION BY terms, most significant first; same targets as order_by */
+  uint32_t n_partition_by;        /* 0: one partition (ROW_NUMBER() OVER (ORDER BY ...)) */
+  uint32_t flags;                 /* PQ_WINDOW_ROW_NUMBER | PQ_WINDOW_PARTITION_ROWS */
+  int64_t offset;                 /* keep rows whose row number rn satisfies offset < rn <= offset + fetch; >= 0 */
+  int64_t fetch;                  /* < 0: no upper bound */
+} PqWindow;
+
 /* ---- inputs ---- */
 typedef struct {
   const char* path;  /* file to read, or NULL when buf is given */
@@ -321,6 +357,9 @@ typedef struct {
   /* NULL, or n_aggs entries: a parameter per aggregate.  Only PQ_AGG_PERCENTILE_CONT reads its entry, the fraction p
    * (finite, in [0, 1]; otherwise, or NULL here, the call returns PQ_ERR_INVALID_ARG) */
   const double* agg_params;
+
+  /* NULL, or ROW_NUMBER() OVER (PARTITION BY ... ORDER BY order_by) cut to a rank range (see PqWindow) */
+  const PqWindow* window;
 } PqQueryDesc;
 
 #define PQ_QUERY_COUNT_ONLY 1u    /* filter scan: only rows_selected is wanted, emit no batches */

@@ -65,6 +65,14 @@ class PqOrderBy(C.Structure):
     _fields_ = [("target", C.c_int32), ("index", C.c_int32), ("flags", C.c_uint32), ("_pad", C.c_int32)]
 
 
+PQ_WINDOW_ROW_NUMBER, PQ_WINDOW_PARTITION_ROWS = 1, 2
+
+
+class PqWindow(C.Structure):
+    _fields_ = [("partition_by", C.POINTER(PqOrderBy)), ("n_partition_by", C.c_uint32), ("flags", C.c_uint32),
+                ("offset", C.c_int64), ("fetch", C.c_int64)]
+
+
 class PqQueryDesc(C.Structure):
     _fields_ = [
         ("table", C.c_void_p), ("files", C.POINTER(PqFile)), ("n_files", C.c_uint32),
@@ -78,6 +86,7 @@ class PqQueryDesc(C.Structure):
         ("group_exprs", C.POINTER(PqKeyExpr)),
         ("order_by", C.POINTER(PqOrderBy)), ("n_order_by", C.c_uint32), ("_pad2", C.c_uint32),
         ("agg_params", C.POINTER(C.c_double)),
+        ("window", C.POINTER(PqWindow)),
     ]
 
 

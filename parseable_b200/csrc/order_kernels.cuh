@@ -395,4 +395,162 @@ __global__ void k_order_gather(const uint32_t* __restrict__ idx, uint32_t keep, 
   if (r < keep) new_slot[r] = out_slot ? out_slot[idx[r]] : idx[r];
 }
 
+// ---- ROW_NUMBER() OVER (PARTITION BY ...) cut to a rank range, over the n rows order_sort left in (partition terms,
+// order terms) order.  Sorted position p holds row perm[p] (perm == nullptr: row p).  Tiles of kSlotTile positions,
+// 256 threads x 4 consecutive positions, as k_slot_compact:
+//   k_window_heads    a position is a head when its partition terms' (value, NULL flag) differ from its predecessor's;
+//                     heads per tile
+//   k_item_prefix     heads before every tile: a position's partition id is the heads up to it, minus one
+//   k_window_starts   the first position of every partition
+//   k_window_count    rn = p - start + 1, kept when lo < rn <= hi; kept rows per tile
+//   k_item_prefix     kept rows before every tile (and their total: the one host round trip)
+//   k_window_compact  the kept rows in order, with their row_number and partition_rows
+// A partition may straddle tiles and be larger than one: a position before the first head of its tile belongs to the
+// last partition started in an earlier tile (id = heads before the tile - 1), and its start comes from the start table,
+// which k_window_starts completes before k_window_count reads it. ----
+struct WindowArgs {
+  const unsigned long long* vals;        // [nterms][n]: the partition terms are the first nparts
+  const uint8_t* nulls;                  // [nterms][n]
+  const uint32_t* perm;                  // sorted position -> row (nullptr: identity)
+  uint32_t n, nparts;
+  unsigned long long lo, hi;             // kept: lo < rn <= hi
+  uint8_t* heads;                        // [n]
+  uint32_t* start;                       // [n]: partition id -> first sorted position
+  uint32_t* tile_counts;                 // [ntiles]
+  const unsigned long long* part_base;   // [ntiles]: heads before the tile
+  const unsigned long long* n_part;      // partitions in all
+  const unsigned long long* keep_base;   // [ntiles]: kept rows before the tile
+  // k_window_compact: output row j (< cap) is kept row j
+  const uint32_t* rows;                  // nullptr: kept[j] is the row itself, else rows[row]
+  uint32_t* kept;
+  long long* row_number;                 // nullptr: not asked for
+  long long* partition_rows;
+  unsigned long long cap;
+};
+
+// exclusive prefix of c over the 256 threads of the CTA (ws: 8 words of shared memory)
+__device__ __forceinline__ uint32_t window_tile_excl(uint32_t c, uint32_t* ws) {
+  uint32_t incl = c;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+    if ((int)lane >= o) incl += t;
+  }
+  if (lane == 31) ws[warp] = incl;
+  __syncthreads();
+  uint32_t wbase = 0;
+  for (uint32_t w = 0; w < warp; w++) wbase += ws[w];
+  return wbase + incl - c;
+}
+
+// sum of c over the CTA into tile_counts[blockIdx.x]
+__device__ __forceinline__ void window_tile_count(uint32_t c, uint32_t* ws, uint32_t* tile_counts) {
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t t = 0;
+    for (int w = 0; w < 8; w++) t += ws[w];
+    tile_counts[blockIdx.x] = t;
+  }
+}
+
+__global__ void __launch_bounds__(256) k_window_heads(const __grid_constant__ WindowArgs a) {
+  __shared__ uint32_t ws[8];
+  const uint32_t p0 = blockIdx.x * kSlotTile + threadIdx.x * 4;
+  uint32_t c = 0;
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const uint32_t p = p0 + k;
+    if (p >= a.n) break;
+    bool head = p == 0;
+    if (!head) {
+      const uint32_t r = a.perm ? a.perm[p] : p, q = a.perm ? a.perm[p - 1] : p - 1;
+      for (uint32_t t = 0; t < a.nparts && !head; t++) {
+        const uint8_t nr = a.nulls[size_t(t) * a.n + r], nq = a.nulls[size_t(t) * a.n + q];
+        head = nr != nq || (!nr && a.vals[size_t(t) * a.n + r] != a.vals[size_t(t) * a.n + q]);   // a NULL's value is not read
+      }
+    }
+    a.heads[p] = head ? 1 : 0;
+    c += head ? 1u : 0u;
+  }
+  window_tile_count(c, ws, a.tile_counts);
+}
+
+__global__ void __launch_bounds__(256) k_window_starts(const __grid_constant__ WindowArgs a) {
+  __shared__ uint32_t ws[8];
+  const uint32_t p0 = blockIdx.x * kSlotTile + threadIdx.x * 4;
+  uint32_t f[4], c = 0;
+#pragma unroll
+  for (int k = 0; k < 4; k++) { f[k] = p0 + k < a.n ? a.heads[p0 + k] : 0u; c += f[k]; }
+  unsigned long long id = a.part_base[blockIdx.x] + window_tile_excl(c, ws);
+#pragma unroll
+  for (int k = 0; k < 4; k++)
+    if (f[k]) a.start[id++] = p0 + k;
+}
+
+// the rank of this thread's 4 positions (rn[k] = 0 past n) and their partition ids
+__device__ __forceinline__ void window_ranks(const WindowArgs& a, uint32_t* ws, unsigned long long (&rn)[4], uint32_t (&pid)[4]) {
+  const uint32_t p0 = blockIdx.x * kSlotTile + threadIdx.x * 4;
+  uint32_t f[4], c = 0;
+#pragma unroll
+  for (int k = 0; k < 4; k++) { f[k] = p0 + k < a.n ? a.heads[p0 + k] : 0u; c += f[k]; }
+  unsigned long long run = a.part_base[blockIdx.x] + window_tile_excl(c, ws);   // >= 1 past position 0: it is a head
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    run += f[k];
+    pid[k] = uint32_t(run - 1);
+    rn[k] = p0 + k < a.n ? uint64_t(p0 + k) - a.start[pid[k]] + 1 : 0ull;
+  }
+}
+
+__global__ void __launch_bounds__(256) k_window_count(const __grid_constant__ WindowArgs a) {
+  __shared__ uint32_t ws[8];
+  unsigned long long rn[4];
+  uint32_t pid[4], c = 0;
+  window_ranks(a, ws, rn, pid);
+#pragma unroll
+  for (int k = 0; k < 4; k++) c += (rn[k] > a.lo && rn[k] <= a.hi) ? 1u : 0u;
+  __syncthreads();   // ws is reused
+  window_tile_count(c, ws, a.tile_counts);
+}
+
+__global__ void __launch_bounds__(256) k_window_compact(const __grid_constant__ WindowArgs a) {
+  __shared__ uint32_t ws[8];
+  unsigned long long rn[4];
+  uint32_t pid[4], f[4], c = 0;
+  window_ranks(a, ws, rn, pid);
+#pragma unroll
+  for (int k = 0; k < 4; k++) { f[k] = (rn[k] > a.lo && rn[k] <= a.hi) ? 1u : 0u; c += f[k]; }
+  __syncthreads();   // ws is reused
+  unsigned long long j = a.keep_base[blockIdx.x] + window_tile_excl(c, ws);
+  const uint32_t p0 = blockIdx.x * kSlotTile + threadIdx.x * 4;
+  const unsigned long long nparts = *a.n_part;
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    if (!f[k]) continue;
+    if (j < a.cap) {
+      const uint32_t p = p0 + k, r = a.perm ? a.perm[p] : p;
+      a.kept[j] = a.rows ? a.rows[r] : r;
+      if (a.row_number) a.row_number[j] = (long long)rn[k];
+      if (a.partition_rows) {
+        const uint32_t s = a.start[pid[k]], e = pid[k] + 1ull < nparts ? a.start[pid[k] + 1] : a.n;
+        a.partition_rows[j] = (long long)(e - s);
+      }
+    }
+    j++;
+  }
+}
+
+// a window without partition terms: output row j is row offset + j of the ordered rows src (nullptr: the row order),
+// rn = offset + 1 + j, and the one partition holds all n rows
+__global__ void k_window_number(unsigned long long cnt, unsigned long long offset, unsigned long long n, const uint32_t* __restrict__ src,
+                                uint32_t* __restrict__ kept, long long* __restrict__ row_number, long long* __restrict__ partition_rows) {
+  const unsigned long long j = blockIdx.x * uint64_t(blockDim.x) + threadIdx.x;
+  if (j >= cnt) return;
+  kept[j] = src ? src[offset + j] : uint32_t(offset + j);
+  if (row_number) row_number[j] = (long long)(offset + 1 + j);
+  if (partition_rows) partition_rows[j] = (long long)n;
+}
+
 }  // namespace pqb

@@ -17,6 +17,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <limits>
 #include <map>
 #include <set>
@@ -844,6 +845,108 @@ uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, D
   return launches;
 }
 
+// ROW_NUMBER() OVER (PARTITION BY ... ORDER BY ...) cut to a rank range, over n rows whose partition terms and then
+// order terms the caller encoded into `ob`.  count() sorts and counts the kept rows; the caller sizes its result from
+// that count and calls fill(), which writes the kept rows in output order (their entries of `rows`, or their positions
+// with rows == nullptr) and their row_number / partition_rows straight into the caller's result buffers.
+//   no partition terms: order_sort keeps the first offset + fetch rows (the top-K select when that is small), and the
+//                       kept rows are those after the first `offset` (k_window_number)
+//   partition terms:    order_sort orders all n rows, the k_window_* kernels rank and count them; one host round trip
+//                       (beside order_sort's own) reads the kept count
+struct WindowRun {
+  const PqWindow& w;
+  uint32_t n, nparts;
+  DevBuf<uint32_t> sorted;   // order_sort's rows (empty: the row order is the order)
+  WindowArgs a{};
+  uint32_t ntiles = 0;
+  DevBuf<uint8_t> heads;
+  DevBuf<uint32_t> start, tile_counts;
+  DevBuf<unsigned long long> part_base, keep_base, totals;
+  Timer t_sort, t_cut, t_fill;
+  bool sort_timed = false, cut_timed = false, fill_timed = false;
+  uint64_t launches = 0;
+
+  WindowRun(const PqWindow& win, uint32_t rows, uint32_t parts) : w(win), n(rows), nparts(parts) {}
+
+  // the rows in the rank range, before any `limit`
+  unsigned long long count(const OrderBufs& ob, const uint8_t* nulls_first, const uint32_t* rows, cudaStream_t stream, PqMetrics& m) {
+    const unsigned long long lo = uint64_t(w.offset), hi = w.fetch < 0 ? ~0ull : uint64_t(w.offset) + uint64_t(w.fetch);
+    if (nparts == 0) {
+      const uint32_t keep = uint32_t(std::min<unsigned long long>(n, hi));
+      if (keep <= lo) return 0;
+      launches += order_sort(ob, uint32_t(ob.ranges.n), n, nulls_first, keep, rows, sorted, stream, m, t_sort, &sort_timed);
+      return keep - lo;
+    }
+    launches += order_sort(ob, uint32_t(ob.ranges.n), n, nulls_first, n, nullptr, sorted, stream, m, t_sort, &sort_timed);
+    ntiles = uint32_t((uint64_t(n) + kSlotTile - 1) / kSlotTile);
+    heads.alloc(n, stream);
+    start.alloc(n, stream);
+    tile_counts.alloc(ntiles, stream);
+    part_base.alloc(ntiles, stream);
+    keep_base.alloc(ntiles, stream);
+    totals.alloc(2, stream);
+    a.vals = ob.vals.p;
+    a.nulls = ob.nulls.p;
+    a.perm = sorted.p;
+    a.n = n;
+    a.nparts = nparts;
+    a.lo = lo;
+    a.hi = hi;
+    a.heads = heads.p;
+    a.start = start.p;
+    a.tile_counts = tile_counts.p;
+    a.part_base = part_base.p;
+    a.n_part = totals.p;
+    a.keep_base = keep_base.p;
+    PQB_CUDA(cudaEventRecord(t_cut.a, stream));
+    k_window_heads<<<ntiles, 256, 0, stream>>>(a);
+    k_item_prefix<<<1, 1024, 0, stream>>>(tile_counts.p, ntiles, part_base.p, totals.p);
+    k_window_starts<<<ntiles, 256, 0, stream>>>(a);
+    k_window_count<<<ntiles, 256, 0, stream>>>(a);
+    k_item_prefix<<<1, 1024, 0, stream>>>(tile_counts.p, ntiles, keep_base.p, totals.p + 1);
+    PQB_CUDA(cudaEventRecord(t_cut.b, stream));
+    PQB_CUDA(cudaGetLastError());
+    launches += 5;
+    cut_timed = true;
+    unsigned long long kept = 0;
+    PQB_CUDA(cudaMemcpyAsync(&kept, totals.p + 1, 8, cudaMemcpyDeviceToHost, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+    m.d2h_bytes += 8;
+    return kept;
+  }
+
+  // the first `cap` kept rows (cap <= count()) into kept[cap]; row_number / partition_rows: nullptr when not asked for
+  void fill(const uint32_t* rows, unsigned long long cap, uint32_t* kept, long long* row_number, long long* partition_rows,
+            cudaStream_t stream) {
+    PQB_CUDA(cudaEventRecord(t_fill.a, stream));
+    if (nparts == 0) {   // order_sort's rows already went through `rows`
+      k_window_number<<<uint32_t((cap + 255) / 256), 256, 0, stream>>>(cap, uint64_t(w.offset), n, sorted.p ? sorted.p : rows, kept,
+                                                                       row_number, partition_rows);
+    } else {
+      a.rows = rows;
+      a.kept = kept;
+      a.row_number = row_number;
+      a.partition_rows = partition_rows;
+      a.cap = cap;
+      k_window_compact<<<ntiles, 256, 0, stream>>>(a);
+    }
+    PQB_CUDA(cudaEventRecord(t_fill.b, stream));
+    PQB_CUDA(cudaGetLastError());
+    launches++;
+    fill_timed = true;
+  }
+
+  // CUDA-event time of the sort and the window's kernels (after the caller's stream synchronise)
+  double ms() const {
+    double t = 0;
+    float x = 0;
+    if (sort_timed) { cudaEventElapsedTime(&x, t_sort.a, t_sort.b); t += x; }
+    if (cut_timed) { cudaEventElapsedTime(&x, t_cut.a, t_cut.b); t += x; }
+    if (fill_timed) { cudaEventElapsedTime(&x, t_fill.a, t_fill.b); t += x; }
+    return t;
+  }
+};
+
 // MEDIAN / PERCENTILE_CONT of one column: its n emitted pairs become two ORDER BY terms (slot, key), sorted by order_sort;
 // k_pct_pick then writes every non-empty group's results.  The emitted pairs are freed once staged.  The kernels are
 // timed (without order_sort's one round trip) into pct_ms.  Returns the kernels it launched.
@@ -904,14 +1007,24 @@ void Query::run(const PqQueryDesc& d) {
   if (d.n_group_by > (uint32_t)kMaxKeys) throw Error(PQ_ERR_UNSUPPORTED, "too many GROUP BY columns");
   if (d.n_pred > (uint32_t)kMaxPredOps) throw Error(PQ_ERR_UNSUPPORTED, "predicate program too long");
   if (d.n_group_by && !d.n_aggs) throw Error(PQ_ERR_INVALID_ARG, "GROUP BY without aggregates");
-  const bool ordered = d.n_order_by > 0;
+  const PqWindow* win = d.window;   // ROW_NUMBER() OVER (PARTITION BY ... ORDER BY order_by), cut to a rank range
+  const bool ordered = d.n_order_by > 0 || win;
   const bool row_order = ordered && !d.n_aggs;   // ORDER BY ... LIMIT on a filter / projection scan: the terms are columns
+  const uint32_t n_part = win ? win->n_partition_by : 0;
+  if (win) {
+    if (win->offset < 0) throw Error(PQ_ERR_INVALID_ARG, "window: offset < 0");
+    if (win->flags & ~(PQ_WINDOW_ROW_NUMBER | PQ_WINDOW_PARTITION_ROWS)) throw Error(PQ_ERR_INVALID_ARG, "window: unknown flags");
+    if (d.flags & PQ_QUERY_COUNT_ONLY) throw Error(PQ_ERR_INVALID_ARG, "window with PQ_QUERY_COUNT_ONLY: a count has no rows to rank");
+    if (n_part && !win->partition_by) throw Error(PQ_ERR_INVALID_ARG, "n_partition_by > 0 without partition_by");
+    if (uint64_t(n_part) + d.n_order_by > uint64_t(kMaxOrder)) throw Error(PQ_ERR_UNSUPPORTED, "more than 8 PARTITION BY and ORDER BY terms");
+  }
   if (ordered) {
     if (d.n_order_by > uint32_t(kMaxOrder)) throw Error(PQ_ERR_UNSUPPORTED, "more than 8 ORDER BY terms");
-    if (!d.order_by) throw Error(PQ_ERR_INVALID_ARG, "n_order_by > 0 without order_by");
-    for (uint32_t t = 0; t < d.n_order_by; t++) {
-      const PqOrderBy& ob = d.order_by[t];
-      const std::string term = "ORDER BY term " + std::to_string(t) + ": ";
+    if (d.n_order_by && !d.order_by) throw Error(PQ_ERR_INVALID_ARG, "n_order_by > 0 without order_by");
+    for (uint32_t t = 0; t < n_part + d.n_order_by; t++) {   // the partition terms, then the order terms
+      const PqOrderBy& ob = t < n_part ? win->partition_by[t] : d.order_by[t - n_part];
+      const std::string term = t < n_part ? "PARTITION BY term " + std::to_string(t) + ": " : "ORDER BY term " + std::to_string(t - n_part) + ": ";
+      if (t < n_part && !row_order && ob.target == PQ_ORDER_AGG) throw Error(PQ_ERR_INVALID_ARG, term + "a partition is a GROUP BY key or a column, not an aggregate");
       if (ob.target != PQ_ORDER_KEY && ob.target != PQ_ORDER_AGG && ob.target != PQ_ORDER_COLUMN) throw Error(PQ_ERR_INVALID_ARG, term + "unknown target");
       if (row_order && ob.target != PQ_ORDER_COLUMN)
         throw Error(PQ_ERR_UNSUPPORTED, term + "ORDER BY on a filter / projection scan orders by columns (PQ_ORDER_COLUMN), not by a GROUP BY key or an aggregate");
@@ -922,7 +1035,7 @@ void Query::run(const PqQueryDesc& d) {
         throw Error(PQ_ERR_INVALID_ARG, term + (ob.target == PQ_ORDER_KEY ? "GROUP BY" : ob.target == PQ_ORDER_AGG ? "aggregate" : "column") + " index out of range");
     }
     if (row_order && (d.flags & PQ_QUERY_COUNT_ONLY)) throw Error(PQ_ERR_INVALID_ARG, "ORDER BY with PQ_QUERY_COUNT_ONLY: a count has no rows to order");
-    if (row_order && d.limit < 0) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY needs a LIMIT (limit >= 0)");
+    if (row_order && d.limit < 0 && !win) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY needs a LIMIT (limit >= 0)");
   }
 
   cudaStream_t stream;
@@ -1160,6 +1273,7 @@ void Query::run(const PqQueryDesc& d) {
     col_used[d.projection[i]] = true;        // only gathered for the selected rows
   }
   for (uint32_t t = 0; row_order && t < d.n_order_by; t++) col_used[d.order_by[t].index] = true;   // likewise: read for the selected rows
+  for (uint32_t t = 0; row_order && t < n_part; t++) col_used[win->partition_by[t].index] = true;
   // compact to kernel column slots
   std::vector<int> slot_of(d.n_columns, -1);
   std::vector<uint32_t> qcol_of_slot;
@@ -1774,9 +1888,9 @@ void Query::run(const PqQueryDesc& d) {
   DevBuf<FlatPageRec> d_opages;
   if (row_order) {
     std::vector<int> id_cols;   // table columns whose pages without a dictionary are read as id pages
-    roa.nterms = d.n_order_by;
-    for (uint32_t t = 0; t < d.n_order_by; t++) {
-      const PqOrderBy& ob = d.order_by[t];
+    roa.nterms = n_part + d.n_order_by;   // a window sorts by its partition terms first
+    for (uint32_t t = 0; t < roa.nterms; t++) {
+      const PqOrderBy& ob = t < n_part ? win->partition_by[t] : d.order_by[t - n_part];
       RowOrderTerm& ot = roa.t[t];
       ot.slot = uint32_t(slot_of[ob.index]);
       ot.kind = plan.cols[ot.slot].kind;
@@ -2279,9 +2393,11 @@ void Query::run(const PqQueryDesc& d) {
     metrics.groups_total = n_total;
     std::unique_ptr<Timer> t_enc, t_sort;   // only for a query with ORDER BY
     bool sort_timed = false;
+    std::unique_ptr<WindowRun> wrun;       // only for a query with a window over at least one group
+    std::unique_ptr<OrderBufs> wbufs;
     if (ordered) {
       if (d.limit >= 0) keep = std::min<uint64_t>(keep, uint64_t(d.limit));
-      if (keep && n_out > 1) {
+      if (win ? n_out > 0 : keep && n_out > 1) {
         OrderArgs oa{};
         uint8_t nulls_first[kMaxOrder];
         oa.acc = d_acc.p;
@@ -2290,10 +2406,10 @@ void Query::run(const PqQueryDesc& d) {
         oa.n = n_out;
         oa.nslots = plan.nslots;
         oa.n_acc = plan.n_acc;
-        oa.nterms = d.n_order_by;
+        oa.nterms = n_part + d.n_order_by;   // a window sorts by its partition terms first
         std::vector<std::shared_ptr<const uint32_t>> rank_hold;   // a concurrent unify_key may replace the column's ranks
-        for (uint32_t t = 0; t < d.n_order_by; t++) {
-          const PqOrderBy& ob = d.order_by[t];
+        for (uint32_t t = 0; t < oa.nterms; t++) {
+          const PqOrderBy& ob = t < n_part ? win->partition_by[t] : d.order_by[t - n_part];
           OrderTerm& ot = oa.t[t];
           ot.target = uint8_t(ob.target);
           ot.desc = (ob.flags & PQ_ORDER_DESC) ? 1 : 0;
@@ -2326,10 +2442,32 @@ void Query::run(const PqQueryDesc& d) {
         }
         t_enc = std::make_unique<Timer>();
         t_sort = std::make_unique<Timer>();
-        launches += order_groups(oa, nulls_first, uint32_t(keep), d_out_slot, stream, metrics, *t_enc, *t_sort, &sort_timed);
+        if (win) {
+          // the window: encode, then sort and count (WindowRun); the kept groups' slots are written once the result
+          // block is allocated
+          wbufs = std::make_unique<OrderBufs>(oa.nterms, oa.n, stream, metrics);
+          oa.vals = wbufs->vals.p;
+          oa.nulls = wbufs->nulls.p;
+          oa.ranges = wbufs->ranges.p;
+          PQB_CUDA(cudaEventRecord(t_enc->a, stream));
+          k_order_encode<<<(oa.n + 255) / 256, 256, 0, stream>>>(oa);
+          PQB_CUDA(cudaEventRecord(t_enc->b, stream));
+          wrun = std::make_unique<WindowRun>(*win, n_out, n_part);
+          const unsigned long long kept = wrun->count(*wbufs, nulls_first, d_out_slot.p, stream, metrics);
+          launches += 1 + wrun->launches;
+          keep = d.limit >= 0 ? std::min<uint64_t>(kept, uint64_t(d.limit)) : kept;
+        } else {
+          launches += order_groups(oa, nulls_first, uint32_t(keep), d_out_slot, stream, metrics, *t_enc, *t_sort, &sort_timed);
+        }
         n_out = uint32_t(keep);
+      } else if (win) {   // a global aggregate over zero rows: its one row has rn = 1
+        if (!(win->offset == 0 && win->fetch != 0)) keep = 0;
       }
     }
+    // a window's extra columns: Int64, never NULL, after the keys and aggregates
+    std::vector<std::string> win_names;
+    if (win && (win->flags & PQ_WINDOW_ROW_NUMBER)) win_names.push_back("row_number");
+    if (win && (win->flags & PQ_WINDOW_PARTITION_ROWS)) win_names.push_back("partition_rows");
     if (keep == 0) {   // ORDER BY ... LIMIT 0
       metrics.groups = 0;
       PQB_CUDA(cudaEventRecord(t_all.b, stream));
@@ -2348,6 +2486,14 @@ void Query::run(const PqQueryDesc& d) {
         if (oc.type == PQ_T_UTF8) oc.offsets.assign(2, 0);   // MIN / MAX over Utf8: one NULL row, no bytes
         ob.cols.push_back(std::move(oc));
       }
+      for (const std::string& name : win_names) {   // the one row of the one partition: rn = 1, partition_rows = 1
+        OutColumn oc;
+        oc.name = name;
+        oc.type = PQ_T_I64;
+        oc.values.assign(8, 0);
+        oc.values[0] = 1;
+        ob.cols.push_back(std::move(oc));
+      }
       metrics.groups = 1;
       batches_.push_back(std::move(ob));
       PQB_CUDA(cudaEventRecord(t_all.b, stream));
@@ -2361,7 +2507,7 @@ void Query::run(const PqQueryDesc& d) {
       FinishArgs fa{};
       const uint32_t nbatches = (n_out + batch_rows - 1) / batch_rows;
       const uint32_t wpb = (batch_rows + 31) / 32;
-      const uint32_t ncolumns = d.n_group_by + d.n_aggs;
+      const uint32_t ncolumns = d.n_group_by + d.n_aggs + uint32_t(win_names.size());
       uint64_t off = 0;
       auto take = [&](uint64_t bytes) { uint64_t o = off; off = (off + bytes + 63) & ~63ull; return o; };
       const uint64_t nulls_off = take(uint64_t(ncolumns) * nbatches * 4);
@@ -2415,6 +2561,8 @@ void Query::run(const PqQueryDesc& d) {
                                               "): the strings of one result may exceed 2 GiB");
         s.data_off = take(bound);
       }
+      uint64_t win_off[2] = {0, 0};
+      for (size_t w = 0; w < win_names.size(); w++) win_off[w] = take(uint64_t(n_out) * 8);
       // string key bytes: an upper bound (rows x the longest distinct value) keeps the copy to one round trip
       for (uint32_t k = 0; k < d.n_group_by; k++) {
         FinishKey& fk = fa.keys[k];
@@ -2438,6 +2586,19 @@ void Query::run(const PqQueryDesc& d) {
       DevBuf<uint8_t> d_block;
       d_block.alloc(off, stream);
       PQB_CUDA(cudaMemsetAsync(d_block.p, 0, copy_bytes, stream));
+      if (wrun) {   // the kept groups' slots in output order, their row_number / partition_rows into the block
+        DevBuf<uint32_t> slots;
+        slots.alloc(n_out, stream);
+        auto col = [&](uint32_t flag) -> long long* {
+          if (!(win->flags & flag)) return nullptr;
+          const size_t w = (flag == PQ_WINDOW_PARTITION_ROWS && (win->flags & PQ_WINDOW_ROW_NUMBER)) ? 1 : 0;
+          return reinterpret_cast<long long*>(d_block.p + win_off[w]);
+        };
+        wrun->fill(d_out_slot.p, n_out, slots.p, col(PQ_WINDOW_ROW_NUMBER), col(PQ_WINDOW_PARTITION_ROWS), stream);
+        launches++;
+        std::swap(d_out_slot.p, slots.p);   // the old list is freed with `slots`
+        std::swap(d_out_slot.n, slots.n);
+      }
       fa.acc = d_acc.p;
       fa.wide = plan.hashed ? d_hkeys.p : nullptr;
       fa.out_slot = d_out_slot.p;
@@ -2496,6 +2657,11 @@ void Query::run(const PqQueryDesc& d) {
             if (fk.kind == DK_STR) { oc.ext_offsets_off = fk.val_off + uint64_t(r0) * 4; oc.ext_off = fk.data_off; }
             else if (fk.kind == DK_BOOL) oc.ext_off = fk.val_off + uint64_t(b) * wpb * 4;
             else oc.ext_off = fk.val_off + uint64_t(r0) * 8;
+          } else if (c >= d.n_group_by + d.n_aggs) {   // row_number / partition_rows
+            const uint32_t w = c - d.n_group_by - d.n_aggs;
+            oc.name = win_names[w];
+            oc.type = PQ_T_I64;
+            oc.ext_off = win_off[w] + uint64_t(r0) * 8;
           } else {
             const uint32_t a = c - d.n_group_by;
             oc.name = agg_name(a);
@@ -2514,7 +2680,7 @@ void Query::run(const PqQueryDesc& d) {
       float ms = 0, ms2 = 0;
       cudaEventElapsedTime(&ms, t_enc->a, t_enc->b);
       if (sort_timed) cudaEventElapsedTime(&ms2, t_sort->a, t_sort->b);
-      metrics.order_ms = double(ms) + double(ms2);
+      metrics.order_ms = double(ms) + double(ms2) + (wrun ? wrun->ms() : 0.0);
     }
   } else {
     // ---- filter / COUNT(*) ----
@@ -2555,6 +2721,13 @@ void Query::run(const PqQueryDesc& d) {
       const uint32_t wpb = (batch_rows + 31) / 32;
       unsigned long long n_rows = 0;
       DevBuf<uint8_t> d_block;
+      // a window's extra columns (Int64, never NULL, after the projection and __row_id): `win_fill` writes them, and the
+      // kept positions, once gather has allocated the block
+      std::vector<std::string> win_names;
+      if (win && (win->flags & PQ_WINDOW_ROW_NUMBER)) win_names.push_back("row_number");
+      if (win && (win->flags & PQ_WINDOW_PARTITION_ROWS)) win_names.push_back("partition_rows");
+      uint64_t win_off[2] = {0, 0};
+      std::function<void(long long*, long long*)> win_fill;
       // the first `cap` selected rows, or with `handles` the rows at positions kept[0, cap) (ORDER BY ... LIMIT)
       auto gather = [&](unsigned long long cap, const unsigned long long* handles, const uint32_t* kept) {
         nbatches = uint32_t((cap + batch_rows - 1) / batch_rows);
@@ -2580,6 +2753,7 @@ void Query::run(const PqQueryDesc& d) {
           if (bound > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "projected strings of one result exceed 2 GiB: add a LIMIT");
           pc.data_off = take(bound);
         }
+        for (size_t w = 0; w < win_names.size(); w++) win_off[w] = take(cap * 8);
         copy_bytes = off;
         for (uint32_t c = 0; c < npc; c++)
           if (pj.cols[c].kind == DK_STR) { pj.cols[c].src_off = take(cap * 8); pj.cols[c].len_off = take(cap * 4); }
@@ -2602,6 +2776,12 @@ void Query::run(const PqQueryDesc& d) {
         pj.batch_rows = batch_rows;
         pj.words_per_batch = wpb;
         pj.nbatches = nbatches;
+        if (win_fill) {
+          long long* cols[2] = {nullptr, nullptr};
+          for (size_t w = 0; w < win_names.size(); w++) cols[win_names[w] == "row_number" ? 0 : 1] = reinterpret_cast<long long*>(d_block.p + win_off[w]);
+          win_fill(cols[0], cols[1]);
+          launches++;
+        }
         if (handles) {
           k_project_rows<<<uint32_t((cap + 255) / 256), 256, 0, stream>>>(pj, handles, kept);
         } else {
@@ -2629,9 +2809,9 @@ void Query::run(const PqQueryDesc& d) {
         PQB_CUDA(cudaStreamSynchronize(stream));   // the selected-row total sizes the sort
         if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
         if (total > 0xffffffffull) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY over more than 2^32 - 1 selected rows");
-        const unsigned long long keep = std::min(total, lim);
-        if (keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
-        if (keep) {
+        unsigned long long keep = std::min(total, lim);   // a window: the kept rows, known after its sort
+        if (!win && keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
+        if (win ? total > 0 : keep > 0) {
           const uint32_t n = uint32_t(total);
           OrderBufs ob(roa.nterms, n, stream, metrics);
           DevBuf<unsigned long long> handles;
@@ -2659,14 +2839,28 @@ void Query::run(const PqQueryDesc& d) {
           PQB_CUDA(cudaEventRecord(t_enc.a, stream));
           k_order_rows_encode<<<grid, 256, 0, stream>>>(roa);
           PQB_CUDA(cudaEventRecord(t_enc.b, stream));
-          launches += 1 + order_sort(ob, roa.nterms, n, row_nulls_first, uint32_t(keep), nullptr, kept, stream, metrics, t_sort, &sort_timed);
-          gather(keep, handles.p, kept.p);
+          std::unique_ptr<WindowRun> wrun;
+          if (win) {
+            // the window: sort and count, then the kept positions and the extra columns in gather's block
+            wrun = std::make_unique<WindowRun>(*win, n, n_part);
+            keep = std::min(wrun->count(ob, row_nulls_first, nullptr, stream, metrics), lim);
+            launches += 1 + wrun->launches;
+            if (keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
+            if (keep) {
+              kept.alloc(keep, stream);
+              win_fill = [&](long long* rn, long long* prows) { wrun->fill(nullptr, keep, kept.p, rn, prows, stream); };
+              gather(keep, handles.p, kept.p);
+            }
+          } else {
+            launches += 1 + order_sort(ob, roa.nterms, n, row_nulls_first, uint32_t(keep), nullptr, kept, stream, metrics, t_sort, &sort_timed);
+            gather(keep, handles.p, kept.p);
+          }
           PQB_CUDA(cudaStreamSynchronize(stream));
-          metrics.d2h_bytes += copy_bytes;
+          if (keep) metrics.d2h_bytes += copy_bytes;
           float ms = 0, ms2 = 0;
           cudaEventElapsedTime(&ms, t_enc.a, t_enc.b);
           if (sort_timed) cudaEventElapsedTime(&ms2, t_sort.a, t_sort.b);
-          metrics.order_ms = double(ms) + double(ms2);
+          metrics.order_ms = double(ms) + double(ms2) + (wrun ? wrun->ms() : 0.0);
         }
         n_rows = keep;
         shape->last_total.store(total);
@@ -2720,6 +2914,17 @@ void Query::run(const PqQueryDesc& d) {
             else if (pc.kind == DK_BOOL) oc.ext_off = pc.val_off + uint64_t(b) * wpb * 4;
             else oc.ext_off = pc.val_off + r0 * 8;
           } else if (oc.type == PQ_T_UTF8) oc.offsets.assign(1, 0);
+          ob.cols.push_back(std::move(oc));
+        }
+        for (size_t w = 0; w < win_names.size(); w++) {
+          OutColumn oc;
+          oc.name = win_names[w];
+          oc.type = PQ_T_I64;
+          if (nb) {
+            oc.ext = block;
+            oc.ext_all = true;
+            oc.ext_off = win_off[w] + r0 * 8;
+          }
           ob.cols.push_back(std::move(oc));
         }
         batches_.push_back(std::move(ob));
@@ -2786,7 +2991,9 @@ void Query::run(const PqQueryDesc& d) {
         PQB_CUDA(cudaStreamSynchronize(stream));
       }
       metrics.groups_total = 1;
-      if (ordered && d.limit == 0) {   // one row, ordered trivially; LIMIT 0 keeps none
+      // one row, ordered trivially; LIMIT 0 keeps none, and a window keeps it when its rank range holds rn = 1
+      const bool win_drops = win && !(win->offset == 0 && win->fetch != 0);
+      if ((ordered && d.limit == 0) || win_drops) {
         metrics.groups = 0;
       } else {
         OutBatch ob;
@@ -2797,6 +3004,15 @@ void Query::run(const PqQueryDesc& d) {
           oc.type = PQ_T_I64;
           oc.values.resize(8);
           std::memcpy(oc.values.data(), &total, 8);
+          ob.cols.push_back(std::move(oc));
+        }
+        for (uint32_t f : {PQ_WINDOW_ROW_NUMBER, PQ_WINDOW_PARTITION_ROWS}) {   // the one partition of one row
+          if (!win || !(win->flags & f)) continue;
+          OutColumn oc;
+          oc.name = f == PQ_WINDOW_ROW_NUMBER ? "row_number" : "partition_rows";
+          oc.type = PQ_T_I64;
+          oc.values.assign(8, 0);
+          oc.values[0] = 1;
           ob.cols.push_back(std::move(oc));
         }
         metrics.groups = 1;

@@ -274,6 +274,36 @@ def _order_term(group_by: list, aggs: list, term) -> tuple[int, int, int]:
     raise QueryError(L.PQ_ERR_INVALID_ARG, f"ORDER BY {item!r}: neither a GROUP BY key nor an aggregate of the query")
 
 
+@dataclass
+class Window:
+    """``ROW_NUMBER() OVER (PARTITION BY partition_by ORDER BY <the query's order_by>)`` cut to ``offset < rn <= offset +
+    fetch`` (``fetch=None``: no upper bound), ranked on the GPU (PqWindow).  ``partition_by`` items are written like
+    ``order_by`` items, ``item`` or ``(item, "asc" | "desc"[, nulls_first])``: GROUP BY keys (names or DateBin) for
+    ``aggregate``, column names for ``scan``; their direction orders the partitions in the output.  ``row_number`` /
+    ``partition_rows`` append the Int64 columns ``row_number`` and ``partition_rows`` (COUNT(*) OVER the partition)."""
+    partition_by: Sequence = ()
+    offset: int = 0
+    fetch: int | None = None
+    row_number: bool = False
+    partition_rows: bool = False
+
+
+def _window_desc(w: "Window", terms: list):
+    """The PqWindow of ``w`` over its partition terms [(PqOrderTarget, index, flags)] (the caller keeps both alive)."""
+    arr = (L.PqOrderBy * max(1, len(terms)))()
+    for i, (target, index, fl) in enumerate(terms):
+        arr[i].target, arr[i].index, arr[i].flags = target, index, fl
+    pw = L.PqWindow(partition_by=arr if terms else None, n_partition_by=len(terms),
+                    flags=(L.PQ_WINDOW_ROW_NUMBER if w.row_number else 0) | (L.PQ_WINDOW_PARTITION_ROWS if w.partition_rows else 0),
+                    offset=int(w.offset), fetch=-1 if w.fetch is None else int(w.fetch))
+    return pw, arr
+
+
+def _partition_items(w: "Window") -> list:
+    """``partition_by`` items as order terms: a bare item is ascending with the default NULL placement."""
+    return [tuple(p) if isinstance(p, (tuple, list)) else (p, "asc") for p in w.partition_by]
+
+
 _ARROW_TO_PQ = {pa.int64(): L.PQ_T_I64, pa.float64(): L.PQ_T_F64, pa.string(): L.PQ_T_UTF8,
                 pa.large_string(): L.PQ_T_UTF8, pa.bool_(): L.PQ_T_BOOL, pa.timestamp("ms"): L.PQ_T_TS_MS}
 
@@ -368,6 +398,43 @@ def field_stats(provider: "StandardTableProvider", field: str, max_field_statist
         t = res.table()
         top = list(zip(t[field].to_pylist(), t["count(*)"].to_pylist()))
     return res.metrics["rows_selected"], res.metrics["groups_total"], top
+
+
+def dataset_stats(provider: "StandardTableProvider", dataset_name: str, fields: Sequence[str] | None = None, offset: int = 0,
+                  limit: int = 5) -> dict:
+    """The dataset-stats API over a pstats-shaped table (``get_dataset_stats`` / ``build_stats_sql``,
+    src/storage/field_stats.rs:530-757 in the reference) in two GPU queries:
+      * ``GROUP BY field_name, distinct_value`` -> ``SUM(count)`` over the dataset's rows with a non-NULL distinct value
+        (and one of ``fields``), ranked per field by ``SUM DESC, distinct_value ASC`` and cut to ``offset < rn <= offset
+        + limit`` on the device, with each field's distinct count (COUNT(*) OVER (PARTITION BY field_name));
+      * the ``field_totals``: ``GROUP BY field_name`` -> ``SUM(field_stats_count)`` over the dataset's rows.
+    Their join on the field name is the host's.  Returns ``{field: {"field_count", "distinct_count",
+    "distinct_values": {value: count}}}``, the values in rank order."""
+    fname, dval, dcount = "field_stats_field_name", "field_stats_distinct_stats_distinct_value", "field_stats_distinct_stats_count"
+    in_dataset = col("dataset_name") == dataset_name
+    flt = [in_dataset, col(dval).is_not_null()]
+    if fields:
+        any_field = None
+        for f in fields:
+            any_field = (col(fname) == f) if any_field is None else (any_field | (col(fname) == f))
+        flt.append(any_field)
+    total = sum_(dcount)
+    ranked = provider.aggregate([fname, dval], [total], flt, order_by=[(total, "desc"), (dval, "asc")],
+                                window=Window(partition_by=[fname], offset=offset, fetch=limit, partition_rows=True))
+    totals = provider.aggregate([fname], [sum_("field_stats_count")], [in_dataset])
+    field_count = {}
+    if totals.batches:
+        t = totals.table()
+        field_count = dict(zip(t[fname].to_pylist(), t["sum(field_stats_count)"].to_pylist()))
+    out: dict = {}
+    if ranked.batches:
+        t = ranked.table()
+        for f, v, c, dc in zip(t[fname].to_pylist(), t[dval].to_pylist(), t[total.name].to_pylist(), t["partition_rows"].to_pylist()):
+            if f is None or f not in field_count:   # the inner join (NULL joins nothing)
+                continue
+            st = out.setdefault(f, {"field_count": field_count[f], "distinct_count": dc, "distinct_values": {}})
+            st["distinct_values"][v] = c
+    return out
 
 
 class DeviceTable:
@@ -466,14 +533,19 @@ class StandardTableProvider:
     # -- TableProvider::scan -------------------------------------------------
     def scan(self, projection: Sequence[str] | None = None, filters: Iterable[Expr] = (), limit: int | None = None,
              count_only: bool = False, row_ids: bool | None = None, batch_size: int = 0, flags: int = 0,
-             poll: bool = False, json: str | None = None, order_by: Sequence | None = None) -> QueryResult:
+             poll: bool = False, json: str | None = None, order_by: Sequence | None = None,
+             window: Window | None = None) -> QueryResult:
         """``projection``: the columns to return for the selected rows (TableProvider::scan's projection);
         without one the scan returns the selected row ordinals (``__row_id``).  ``row_ids=True`` appends
         ``__row_id`` to a projection.  ``order_by``: ``[(column, "asc" | "desc"[, nulls_first]), ...]``, most
         significant first, with a ``limit``: the first ``limit`` selected rows in that order, selected and sorted on
         the GPU (the SortExec(fetch) / TopK above the scan); the columns need not be projected.  ``nulls_first=None``
-        follows the same default as ``aggregate``."""
-        order = [(L.PQ_ORDER_COLUMN, c, _order_flags(direction, rest[0] if rest else None)) for c, direction, *rest in (order_by or [])]
+        follows the same default as ``aggregate``.  ``window``: the top rows of every partition of columns
+        (Window), ranked by ``order_by``; it needs no ``limit``, which then cuts its output."""
+        def term(c, direction, *rest):
+            return L.PQ_ORDER_COLUMN, c, _order_flags(direction, rest[0] if rest else None)
+        order = [term(*t) for t in (order_by or [])]
+        part = [term(*t) for t in _partition_items(window)] if window is not None else None
         f = 0
         if row_ids is None:
             row_ids = not projection
@@ -481,20 +553,30 @@ class StandardTableProvider:
             f |= L.PQ_QUERY_COUNT_ONLY
         elif row_ids:
             f |= L.PQ_QUERY_EMIT_ROW_IDS
-        return self._run(list(filters), [], [], list(projection or []), limit, batch_size, f | flags, poll=poll, json=json, order=order)
+        win = {} if window is None else {"window": window, "partition": part}
+        return self._run(list(filters), [], [], list(projection or []), limit, batch_size, f | flags, poll=poll, json=json, order=order,
+                         **win)
 
     # -- FilterExec + AggregateExec folded into the same call ----------------
     def aggregate(self, group_by: Sequence[str], aggs: Sequence[Agg], filters: Iterable[Expr] = (),
                   batch_size: int = 0, flags: int = 0, json: str | None = None, order_by: Sequence | None = None,
-                  limit: int | None = None) -> QueryResult:
+                  limit: int | None = None, window: Window | None = None) -> QueryResult:
         """``order_by``: ``[(item, "asc" | "desc"[, nulls_first]), ...]``, most significant first, sorted on the GPU
         (the SortExec / TopK above the AggregateExec).  An item is a GROUP BY key (its name or DateBin), an aggregate
         (an Agg of ``aggs`` or its output name).  ``nulls_first=None`` follows DataFusion's default (restated, not
         checked here): ASC puts NULLs last, DESC first.  With ``order_by``, ``limit`` keeps the first rows of the
-        ordered result; without it the C ABI ignores ``limit`` on an aggregate."""
+        ordered result; without it the C ABI ignores ``limit`` on an aggregate.  ``window``: the top groups of every
+        partition of GROUP BY keys (Window), ranked by ``order_by``; ``limit`` then cuts its output."""
         group_by, aggs = list(group_by), list(aggs)
         order = [_order_term(group_by, aggs, t) for t in (order_by or [])]
-        return self._run(list(filters), group_by, aggs, [], limit, batch_size, flags, json=json, order=order)
+        win = {}
+        if window is not None:
+            part = [_order_term(group_by, aggs, t) for t in _partition_items(window)]
+            for (target, _, _), (item, *_) in zip(part, _partition_items(window)):
+                if target != L.PQ_ORDER_KEY:
+                    raise QueryError(L.PQ_ERR_INVALID_ARG, f"PARTITION BY {item!r}: not a GROUP BY key of the query")
+            win = {"window": window, "partition": part}
+        return self._run(list(filters), group_by, aggs, [], limit, batch_size, flags, json=json, order=order, **win)
 
     def count_distinct(self, group_by: Sequence[str], column: str, filters: Iterable[Expr] = ()) -> pa.Table:
         """``SELECT keys, COUNT(DISTINCT column)`` (Parseable's alerts use it: src/alerts/alert_enums.rs:216-223), one
@@ -506,7 +588,7 @@ class StandardTableProvider:
         return pa.table({**{k: pa.array([], pa.null()) for k in group_by}, name: pa.array([], pa.int64())})
 
     def _run(self, filters, group_by, aggs, projection, limit, batch_size, flags, poll: bool = False, json: str | None = None,
-             order: Sequence[tuple] = ()) -> QueryResult:
+             order: Sequence[tuple] = (), window: Window | None = None, partition: Sequence[tuple] | None = None) -> QueryResult:
         lib = L.load()
         d = _Desc()
         ops: list = []
@@ -530,6 +612,8 @@ class StandardTableProvider:
         proj = [d.col_index(c) for c in projection]
         # PQ_ORDER_COLUMN terms name their column: it joins the referenced columns
         order = [(t, d.col_index(i) if isinstance(i, str) else i, fl) for t, i, fl in order]
+        if window is not None:   # partition terms resolve like order terms
+            partition = [(t, d.col_index(i) if isinstance(i, str) else i, fl) for t, i, fl in (partition or [])]
 
         desc = L.PqQueryDesc()
         hfs = None
@@ -565,6 +649,9 @@ class StandardTableProvider:
             desc.order_by, desc.n_order_by = arr_ob, len(order)
         if params is not None:
             desc.agg_params = params
+        if window is not None:
+            pw, _parr = _window_desc(window, partition)
+            desc.window = C.pointer(pw)
         desc.limit = -1 if limit is None else int(limit)
         desc.batch_size = batch_size
         desc.shard_index, desc.shard_count = self.shard_index, self.shard_count
@@ -630,7 +717,8 @@ class TimeRange:
 
 class Query:
     """``SELECT <cols | aggs> FROM <stream> [WHERE ...] [GROUP BY ...] [ORDER BY ...] [LIMIT n]`` — the subset of SQL the
-    GPU path executes (ORDER BY on a query without aggregates only with a LIMIT).  The reference hands SQL to DataFusion's planner (src/query/mod.rs:261-264);
+    GPU path executes (ORDER BY on a query without aggregates only with a LIMIT).  It parses no subqueries, CTEs or window
+    calls (``ROW_NUMBER() OVER (...)``): windows are reached through ``aggregate`` / ``scan(window=Window(...))``.  The reference hands SQL to DataFusion's planner (src/query/mod.rs:261-264);
     that planner is out of scope (SURVEY §2), so this small recursive-descent parser only exists
     to let tests and the bench state their queries the way Parseable users do."""
 

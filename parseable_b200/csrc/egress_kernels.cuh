@@ -81,6 +81,9 @@ struct FinishArgs {
   const uint32_t* out_slot;
   uint8_t* out;                // the result block
   uint32_t* nulls;             // [(nkeys + naggs) * nbatches] inside the block
+  // n_dev == nullptr: n_out groups.  Otherwise the block was laid out before the group count came back to the host:
+  // n_out is its capacity and the kernels read the count (min(*n_dev, n_out) groups) where k_item_prefix left it
+  const unsigned long long* n_dev;
   uint32_t n_out, nslots, n_acc, naggs, nkeys;
   uint32_t batch_rows, words_per_batch, nbatches;
   DevAgg aggs[kMaxAggs];
@@ -121,6 +124,10 @@ __device__ __forceinline__ unsigned long long agg_output_value(const unsigned lo
   return v;
 }
 
+__device__ __forceinline__ uint32_t finish_rows(const FinishArgs& f) {
+  return f.n_dev ? uint32_t(min(*f.n_dev, (unsigned long long)f.n_out)) : f.n_out;
+}
+
 // the group id of one GROUP BY key of a group slot (hashed GROUP BY: decoded from the slot's wide id); card: NULL
 __device__ __forceinline__ uint32_t key_gid_of_slot(const unsigned long long* __restrict__ wide, uint32_t slot, uint64_t wstride, uint32_t card) {
   return uint32_t(((wide ? wide[slot] : uint64_t(slot)) / wstride) % (card + 1));
@@ -129,7 +136,7 @@ __device__ __forceinline__ uint32_t key_gid_of_slot(const unsigned long long* __
 // one thread per output row: aggregate values + validity, numeric / boolean key values, string key lengths
 __global__ void k_agg_finish(const __grid_constant__ FinishArgs f) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= f.n_out) return;
+  if (i >= finish_rows(f)) return;
   const uint32_t slot = f.out_slot[i];
   const uint32_t batch = i / f.batch_rows, pos = i - batch * f.batch_rows;
   const uint32_t word = batch * f.words_per_batch + (pos >> 5), bit = 1u << (pos & 31);
@@ -171,8 +178,11 @@ __global__ void k_agg_finish(const __grid_constant__ FinishArgs f) {
   }
 }
 
-// exclusive scan of u32 lengths into int32 Arrow offsets (n + 1 entries); one block
-__global__ void k_offsets_scan(const uint32_t* __restrict__ lens, uint32_t n, int32_t* __restrict__ offs) {
+// exclusive scan of u32 lengths into int32 Arrow offsets (n + 1 entries); one block.  n_dev != nullptr: min(*n_dev, n)
+// lengths (a result block laid out for n groups before the count was known)
+__global__ void k_offsets_scan(const uint32_t* __restrict__ lens, uint32_t n, const unsigned long long* __restrict__ n_dev,
+                               int32_t* __restrict__ offs) {
+  if (n_dev) n = uint32_t(min(*n_dev, (unsigned long long)n));
   __shared__ unsigned long long warp_sums[32];
   __shared__ unsigned long long carry;
   if (threadIdx.x == 0) carry = 0;
@@ -208,7 +218,7 @@ __global__ void k_offsets_scan(const uint32_t* __restrict__ lens, uint32_t n, in
 // string key bytes: one warp per output row
 __global__ void k_key_gather(const __grid_constant__ FinishArgs f, uint32_t k) {
   const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (i >= f.n_out) return;
+  if (i >= finish_rows(f)) return;
   const FinishKey& key = f.keys[k];
   const uint32_t gid = uint32_t(((f.wide ? f.wide[f.out_slot[i]] : uint64_t(f.out_slot[i])) / key.wstride) % (key.card + 1));
   if (gid == key.card) return;
@@ -220,7 +230,7 @@ __global__ void k_key_gather(const __grid_constant__ FinishArgs f, uint32_t k) {
 // bytes of a MIN / MAX over Utf8 (aggregate a): one warp per output row
 __global__ void k_agg_str_gather(const __grid_constant__ FinishArgs f, uint32_t a) {
   const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (i >= f.n_out) return;
+  if (i >= finish_rows(f)) return;
   const FinishAggStr& s = f.astr[a];
   const uint32_t n = reinterpret_cast<const uint32_t*>(f.out + s.len_off)[i];
   if (n == 0) return;   // NULL, or the empty string

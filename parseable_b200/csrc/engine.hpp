@@ -13,6 +13,8 @@
 #include <mutex>
 #include <stdexcept>
 #include <string>
+#include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/parseable_b200.h"
@@ -50,6 +52,12 @@ class Context {
   uint8_t* pinned_acquire(size_t bytes);
   void pinned_release(uint8_t* p);
   bool is_pinned(const void* p);
+  // non-blocking streams for queries, kept for reuse: creating and destroying one costs more host time than all the
+  // other launches of a warm resident query.  A released stream may still hold queued frees; whoever takes it next
+  // orders its work after them.  Each stream is kept with its device: stream_acquire hands out only the current
+  // device's (a query that was running while the context moved to another device releases its stream afterwards)
+  cudaStream_t stream_acquire();
+  void stream_release(cudaStream_t s, int device);
 
  private:
   std::mutex mu_;
@@ -61,6 +69,7 @@ class Context {
   size_t l2_bytes_ = 0;
   struct Pinned { uint8_t* p; size_t cap; bool busy; };
   std::vector<Pinned> pinned_;
+  std::vector<std::pair<int, cudaStream_t>> free_streams_;   // (device, stream)
 };
 
 // ---- host view of a Parquet file ----
@@ -193,6 +202,10 @@ struct Shape {
   std::vector<uint8_t> has_dict, has_plain, has_delta, flat_plain8, flat_nullable;   // flat_nullable: some flat page of the slot carries a validity bitmap
   std::string why_general;             // first reason an item could not go to the flat kernels (diagnostics)
   std::atomic<unsigned long long> last_total{~0ull};   // rows the last filter scan of this shape selected (sizes the next result)
+  // groups of the last answer of each aggregate plan over this shape (keyed by plan_hash): a repeat of the query lays its
+  // result block out before the group count is back on the host (at most 64 plans; the map is cleared when full)
+  std::mutex hint_mu;
+  std::unordered_map<uint64_t, uint32_t> groups_hint;
   ~Shape();
 };
 

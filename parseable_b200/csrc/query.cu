@@ -110,6 +110,22 @@ LikePlan classify_like(const std::string& pat) {
   return {LIKE_GENERAL, pat};
 }
 
+// FNV-1a over the bytes of a compiled plan, its literals and the batch size: equal for a repeat of the same query on the
+// same table (DevPlan is zero-initialised, padding included, before the planner fills it)
+uint64_t plan_hash(const DevPlan& plan, const std::vector<uint8_t>& lits, uint32_t batch_rows) {
+  uint64_t h = 1469598103934665603ull;
+  auto mix = [&](const void* p, size_t n) {
+    const uint8_t* b = static_cast<const uint8_t*>(p);
+    size_t i = 0;
+    for (; i + 8 <= n; i += 8) { uint64_t w; std::memcpy(&w, b + i, 8); h = (h ^ w) * 1099511628211ull; }
+    for (; i < n; i++) h = (h ^ b[i]) * 1099511628211ull;
+  };
+  mix(&plan, sizeof(plan));
+  mix(lits.data(), lits.size());
+  mix(&batch_rows, sizeof(batch_rows));
+  return h;
+}
+
 uint64_t f64_bits(double d) { uint64_t b; std::memcpy(&b, &d, 8); return b; }
 double bits_f64(uint64_t b) { double d; std::memcpy(&d, &b, 8); return d; }
 
@@ -1038,9 +1054,8 @@ void Query::run(const PqQueryDesc& d) {
     if (row_order && d.limit < 0 && !win) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY needs a LIMIT (limit >= 0)");
   }
 
-  cudaStream_t stream;
-  PQB_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-  struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamDestroy(s); } } sg{stream};
+  cudaStream_t stream = ctx.stream_acquire();
+  struct StreamGuard { cudaStream_t s; int dev; ~StreamGuard() { Context::get().stream_release(s, dev); } } sg{stream, ctx.device()};
 
   // ---- input: resident table, or upload the referenced columns of a file list ----
   const Table* table = reinterpret_cast<const Table*>(d.table);
@@ -2339,21 +2354,213 @@ void Query::run(const PqQueryDesc& d) {
     if (!items.empty()) k_item_prefix<<<1, 1024, 0, stream>>>(d_item_counts.p, uint32_t(items.size()), d_item_base.p, d_totals.p + 1);
     else PQB_CUDA(cudaMemsetAsync(d_totals.p + 1, 0, 8, stream));
     launches += 4;
+    // a window's extra columns: Int64, never NULL, after the keys and aggregates
+    std::vector<std::string> win_names;
+    if (win && (win->flags & PQ_WINDOW_ROW_NUMBER)) win_names.push_back("row_number");
+    if (win && (win->flags & PQ_WINDOW_PARTITION_ROWS)) win_names.push_back("partition_rows");
+    std::unique_ptr<WindowRun> wrun;       // only for a query with a window over at least one group
+    // ---- the result block: every buffer of every batch for n_out groups, assembled on the device and copied to page-locked
+    // memory (no synchronise).  n_dev != nullptr: n_out is a capacity, the kernels read the group count on the device.
+    // cut: ORDER BY ... LIMIT keeps a subset of the groups ----
+    struct Assembled {
+      uint32_t rows = 0;   // the groups the block has room for (0: none assembled)
+      FinishArgs fa{};
+      uint32_t nbatches = 0, wpb = 0, ncolumns = 0;
+      uint64_t nulls_off = 0, copy_bytes = 0, win_off[2] = {0, 0};
+      std::unique_ptr<DevBuf<uint8_t>> d_block;
+      std::shared_ptr<PinnedBlock> block;
+    };
+    auto assemble = [&](uint32_t n_out, const unsigned long long* n_dev, bool cut) -> Assembled {
+      Assembled r;
+      r.rows = n_out;
+      FinishArgs& fa = r.fa;
+      const uint32_t nbatches = (n_out + batch_rows - 1) / batch_rows;
+      const uint32_t wpb = (batch_rows + 31) / 32;
+      const uint32_t ncolumns = d.n_group_by + d.n_aggs + uint32_t(win_names.size());
+      uint64_t off = 0;
+      auto take = [&](uint64_t bytes) { uint64_t o = off; off = (off + bytes + 63) & ~63ull; return o; };
+      const uint64_t nulls_off = take(uint64_t(ncolumns) * nbatches * 4);
+      for (uint32_t k = 0; k < d.n_group_by; k++) {
+        FinishKey& fk = fa.keys[k];
+        const uint8_t kind = plan.cols[plan.keys[k].col].kind;
+        fk.kind = kind;
+        fk.stride = plan.keys[k].stride;
+        fk.wstride = plan.keys[k].wstride;
+        fk.card = qk[k].card;
+        fk.valid_off = take(uint64_t(nbatches) * wpb * 4);
+        if (kind == DK_BOOL) fk.val_off = take(uint64_t(nbatches) * wpb * 4);
+        else if (kind == DK_STR) fk.val_off = take((uint64_t(n_out) + 1) * 4);
+        else fk.val_off = take(uint64_t(n_out) * 8);
+        if (qk[k].is_bin) {
+          fk.is_bin = 1;
+          fk.bin_base = plan.keys[k].bin_base;
+          fk.bin_width = plan.keys[k].bin_width;
+        } else if (kind != DK_BOOL) {
+          const ColSide& cs = table->sides[shape_cols[plan.keys[k].col]];
+          if (multi) {   // the dictionary every rank agreed on
+            fk.kd_offs = cs.d_glob_kd_offs;
+            fk.kd_bytes = cs.d_glob_kd_bytes;
+          } else {
+            fk.kd_offs = cs.d_kd_offs;
+            fk.kd_bytes = cs.d_kd_bytes;
+          }
+        }
+      }
+      for (uint32_t a = 0; a < d.n_aggs; a++) {
+        fa.aggs[a] = plan.aggs[a];
+        fa.nn_is_rows[a] = nn_is_rows[a];
+        fa.valid_off[a] = take(uint64_t(nbatches) * wpb * 4);
+        fa.out_kind[a] = rank_min_max(plan.aggs[a]) ? DK_STR : bool_min_max(plan.aggs[a]) ? DK_BOOL : DK_I64;   // the layouts of the keys
+        if (fa.out_kind[a] == DK_BOOL) fa.val_off[a] = take(uint64_t(nbatches) * wpb * 4);
+        else if (fa.out_kind[a] == DK_STR) fa.val_off[a] = take((uint64_t(n_out) + 1) * 4);
+        else fa.val_off[a] = take(uint64_t(n_out) * 8);
+      }
+      // MIN / MAX over Utf8: the winning values' bytes, bounded by rows x the longest value of the numbering (any group may
+      // hold the longest one)
+      for (uint32_t a = 0; a < d.n_aggs; a++) {
+        if (fa.out_kind[a] != DK_STR) continue;
+        FinishAggStr& s = fa.astr[a];
+        const ColSide& cs = table->sides[shape_cols[plan.aggs[a].col]];
+        s.kd_offs = multi ? cs.d_glob_kd_offs : cs.d_kd_offs;
+        s.kd_bytes = multi ? cs.d_glob_kd_bytes : cs.d_kd_bytes;
+        s.inv = rank_luts[a] ? rank_luts[a]->inv : nullptr;   // nullptr: a column in no file, every group NULL
+        const uint64_t bound = rank_luts[a] ? uint64_t(n_out) * (multi ? cs.glob_max_len : cs.kd_max_len) : 0;
+        if (bound > 0x7fffffffull)
+          throw Error(PQ_ERR_UNSUPPORTED, std::string(plan.aggs[a].fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
+                                              "): the strings of one result may exceed 2 GiB");
+        s.data_off = take(bound);
+      }
+      uint64_t win_off[2] = {0, 0};
+      for (size_t w = 0; w < win_names.size(); w++) win_off[w] = take(uint64_t(n_out) * 8);
+      // string key bytes: an upper bound (rows x the longest distinct value) keeps the copy to one round trip
+      for (uint32_t k = 0; k < d.n_group_by; k++) {
+        FinishKey& fk = fa.keys[k];
+        if (fk.kind != DK_STR) continue;
+        uint64_t max_len = 0;
+        const KeyDict* kd = qk[k].kd;
+        max_len = multi ? table->sides[shape_cols[plan.keys[k].col]].glob_max_len : table->sides[shape_cols[plan.keys[k].col]].kd_max_len;
+        // the count-based bound is over all the groups; a result cut by ORDER BY ... LIMIT may be any subset of them (the
+        // top 5 rows can all hold the one longest value): rows x the longest value there.  A full ORDER BY holds the same
+        // rows as the unordered result, so the count-based bound still holds for it.
+        const uint64_t bound = cut ? uint64_t(n_out) * max_len
+                                       : std::min<uint64_t>(uint64_t(n_out) * max_len, uint64_t(n_out / std::max<uint32_t>(fk.card, 1) + 1) * kd->bytes.size());
+        if (bound > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "group key strings of one result exceed 2 GiB");
+        fk.data_off = take(bound);
+      }
+      const uint64_t copy_bytes = off;
+      for (uint32_t k = 0; k < d.n_group_by; k++)
+        if (fa.keys[k].kind == DK_STR) fa.keys[k].len_off = take(uint64_t(n_out) * 4);   // device-only scratch behind the copied part
+      for (uint32_t a = 0; a < d.n_aggs; a++)
+        if (fa.out_kind[a] == DK_STR) fa.astr[a].len_off = take(uint64_t(n_out) * 4);
+      r.d_block = std::make_unique<DevBuf<uint8_t>>();
+      DevBuf<uint8_t>& d_block = *r.d_block;
+      d_block.alloc(off, stream);
+      PQB_CUDA(cudaMemsetAsync(d_block.p, 0, copy_bytes, stream));
+      if (wrun) {   // the kept groups' slots in output order, their row_number / partition_rows into the block
+        DevBuf<uint32_t> slots;
+        slots.alloc(n_out, stream);
+        auto col = [&](uint32_t flag) -> long long* {
+          if (!(win->flags & flag)) return nullptr;
+          const size_t w = (flag == PQ_WINDOW_PARTITION_ROWS && (win->flags & PQ_WINDOW_ROW_NUMBER)) ? 1 : 0;
+          return reinterpret_cast<long long*>(d_block.p + win_off[w]);
+        };
+        wrun->fill(d_out_slot.p, n_out, slots.p, col(PQ_WINDOW_ROW_NUMBER), col(PQ_WINDOW_PARTITION_ROWS), stream);
+        launches++;
+        std::swap(d_out_slot.p, slots.p);   // the old list is freed with `slots`
+        std::swap(d_out_slot.n, slots.n);
+      }
+      fa.acc = d_acc.p;
+      fa.wide = plan.hashed ? d_hkeys.p : nullptr;
+      fa.out_slot = d_out_slot.p;
+      fa.out = d_block.p;
+      fa.nulls = reinterpret_cast<uint32_t*>(d_block.p + nulls_off);
+      fa.n_out = n_out;
+      fa.n_dev = n_dev;
+      fa.nslots = plan.nslots;
+      fa.n_acc = plan.n_acc;
+      fa.naggs = d.n_aggs;
+      fa.nkeys = d.n_group_by;
+      fa.batch_rows = batch_rows;
+      fa.words_per_batch = wpb;
+      fa.nbatches = nbatches;
+      k_agg_finish<<<(n_out + 255) / 256, 256, 0, stream>>>(fa);
+      launches++;
+      for (uint32_t k = 0; k < d.n_group_by; k++) {
+        if (fa.keys[k].kind != DK_STR) continue;
+        k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.keys[k].len_off), n_out, n_dev,
+                                               reinterpret_cast<int32_t*>(d_block.p + fa.keys[k].val_off));
+        k_key_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, k);
+        launches += 2;
+      }
+      for (uint32_t a = 0; a < d.n_aggs; a++) {
+        if (fa.out_kind[a] != DK_STR) continue;
+        k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.astr[a].len_off), n_out, n_dev,
+                                               reinterpret_cast<int32_t*>(d_block.p + fa.val_off[a]));
+        k_agg_str_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, a);
+        launches += 2;
+      }
+      PQB_CUDA(cudaGetLastError());
+      r.block = std::make_shared<PinnedBlock>();
+      r.block->p = ctx.pinned_acquire(copy_bytes);
+      r.block->bytes = copy_bytes;
+      PQB_CUDA(cudaMemcpyAsync(r.block->p, d_block.p, copy_bytes, cudaMemcpyDeviceToHost, stream));
+      PQB_CUDA(cudaEventRecord(t_all.b, stream));
+      metrics.d2h_bytes += copy_bytes;
+      r.nbatches = nbatches;
+      r.wpb = wpb;
+      r.ncolumns = ncolumns;
+      r.nulls_off = nulls_off;
+      r.copy_bytes = copy_bytes;
+      r.win_off[0] = win_off[0];
+      r.win_off[1] = win_off[1];
+      return r;
+    };
+    // ---- one round trip: an unordered GROUP BY whose plan this shape has answered before lays its result block out for
+    // that many groups now, and the block comes back with the group count.  Should the count have grown (other ranks'
+    // tables under PQ_QUERY_ALLREDUCE), the block is laid out again after the round trip.  ORDER BY / windows (the count
+    // sizes their sort), MEDIAN / PERCENTILE_CONT (their pick runs on the groups) and global aggregates keep two ----
+    Assembled pre;
+    const bool tail_hint = d.n_group_by && !ordered && !plan.npct;
+    uint64_t tail_key = 0;
+    if (tail_hint) {
+      tail_key = plan_hash(plan, lit_pool, batch_rows);
+      uint32_t cap = 0;
+      {
+        std::lock_guard<std::mutex> lk(shape->hint_mu);
+        auto it = shape->groups_hint.find(tail_key);
+        if (it != shape->groups_hint.end()) cap = it->second;
+      }
+      if (const char* e = getenv("PQB_TAIL_CAP")) cap = uint32_t(atoi(e));   // test switch: the block's room in groups
+      cap = uint32_t(std::min<uint64_t>(cap, out_cap));
+      if (verbose) fprintf(stderr, "[pqb] result tail: %s\n", cap ? ("one round trip, block for " + std::to_string(cap) + " groups").c_str()
+                                                                     : "no earlier answer of this plan: two round trips");
+      if (cap) pre = assemble(cap, d_totals.p, false);
+    }
     unsigned long long totals[2] = {0, 0};
     std::vector<unsigned int> pct_count(plan.npct, 0u);
-    if (plan.npct) {
-      PQB_CUDA(cudaMemcpyAsync(pct_count.data(), d_pct_count.p, plan.npct * 4, cudaMemcpyDeviceToHost, stream));
-      metrics.d2h_bytes += plan.npct * 4;
+    {   // into page-locked memory: a copy to pageable memory holds the host until it is done, and the next copy waits for
+        // that.  pinned_acquire hands out any free block of the context's pool that is large enough (1 MB at least)
+      PinnedBlock small;
+      small.p = ctx.pinned_acquire(16 + sizeof(h_counters) + plan.npct * 4);
+      PQB_CUDA(cudaMemcpyAsync(small.p, d_totals.p, 16, cudaMemcpyDeviceToHost, stream));
+      PQB_CUDA(cudaMemcpyAsync(small.p + 16, d_counters.p, sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
+      if (plan.npct) PQB_CUDA(cudaMemcpyAsync(small.p + 16 + sizeof(h_counters), d_pct_count.p, plan.npct * 4, cudaMemcpyDeviceToHost, stream));
+      PQB_CUDA(cudaStreamSynchronize(stream));
+      std::memcpy(totals, small.p, 16);
+      std::memcpy(h_counters, small.p + 16, sizeof(h_counters));
+      if (plan.npct) std::memcpy(pct_count.data(), small.p + 16 + sizeof(h_counters), plan.npct * 4);
     }
-    PQB_CUDA(cudaMemcpyAsync(totals, d_totals.p, 16, cudaMemcpyDeviceToHost, stream));
-    PQB_CUDA(cudaMemcpyAsync(h_counters, d_counters.p, sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
-    PQB_CUDA(cudaStreamSynchronize(stream));
-    metrics.d2h_bytes += 16 + sizeof(h_counters);
+    metrics.d2h_bytes += 16 + sizeof(h_counters) + plan.npct * 4;
     if (plan.hashed && h_counters[1] == 100) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: more distinct groups than the hashed accumulator table holds (2^26)");
     if (plan.ndist && h_counters[1] == kDistinctFull) throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT): more distinct (group, value) pairs than the pair set holds (2^27)");
     if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
     uint32_t n_out = uint32_t(totals[0]);
     metrics.rows_selected = totals[1];
+    if (tail_hint && n_out) {
+      std::lock_guard<std::mutex> lk(shape->hint_mu);
+      if (shape->groups_hint.size() >= 64 && !shape->groups_hint.count(tail_key)) shape->groups_hint.clear();   // a bound, not an LRU
+      shape->groups_hint[tail_key] = n_out;
+    }
     if (allreduce) { float ms = 0; cudaEventElapsedTime(&ms, t_ar.a, t_ar.b); metrics.allreduce_ms = ms; }
     static const char* fn_names[] = {"count(*)", "count", "sum", "min", "max", "avg", "count(distinct", "median", "percentile_cont"};
     auto agg_name = [&](uint32_t a) {
@@ -2393,7 +2600,6 @@ void Query::run(const PqQueryDesc& d) {
     metrics.groups_total = n_total;
     std::unique_ptr<Timer> t_enc, t_sort;   // only for a query with ORDER BY
     bool sort_timed = false;
-    std::unique_ptr<WindowRun> wrun;       // only for a query with a window over at least one group
     std::unique_ptr<OrderBufs> wbufs;
     if (ordered) {
       if (d.limit >= 0) keep = std::min<uint64_t>(keep, uint64_t(d.limit));
@@ -2464,10 +2670,6 @@ void Query::run(const PqQueryDesc& d) {
         if (!(win->offset == 0 && win->fetch != 0)) keep = 0;
       }
     }
-    // a window's extra columns: Int64, never NULL, after the keys and aggregates
-    std::vector<std::string> win_names;
-    if (win && (win->flags & PQ_WINDOW_ROW_NUMBER)) win_names.push_back("row_number");
-    if (win && (win->flags & PQ_WINDOW_PARTITION_ROWS)) win_names.push_back("partition_rows");
     if (keep == 0) {   // ORDER BY ... LIMIT 0
       metrics.groups = 0;
       PQB_CUDA(cudaEventRecord(t_all.b, stream));
@@ -2503,142 +2705,20 @@ void Query::run(const PqQueryDesc& d) {
       PQB_CUDA(cudaEventRecord(t_all.b, stream));
       PQB_CUDA(cudaStreamSynchronize(stream));
     } else {
-      // ---- the result block: every buffer of every batch, assembled on the device ----
-      FinishArgs fa{};
-      const uint32_t nbatches = (n_out + batch_rows - 1) / batch_rows;
-      const uint32_t wpb = (batch_rows + 31) / 32;
-      const uint32_t ncolumns = d.n_group_by + d.n_aggs + uint32_t(win_names.size());
-      uint64_t off = 0;
-      auto take = [&](uint64_t bytes) { uint64_t o = off; off = (off + bytes + 63) & ~63ull; return o; };
-      const uint64_t nulls_off = take(uint64_t(ncolumns) * nbatches * 4);
-      for (uint32_t k = 0; k < d.n_group_by; k++) {
-        FinishKey& fk = fa.keys[k];
-        const uint8_t kind = plan.cols[plan.keys[k].col].kind;
-        fk.kind = kind;
-        fk.stride = plan.keys[k].stride;
-        fk.wstride = plan.keys[k].wstride;
-        fk.card = qk[k].card;
-        fk.valid_off = take(uint64_t(nbatches) * wpb * 4);
-        if (kind == DK_BOOL) fk.val_off = take(uint64_t(nbatches) * wpb * 4);
-        else if (kind == DK_STR) fk.val_off = take((uint64_t(n_out) + 1) * 4);
-        else fk.val_off = take(uint64_t(n_out) * 8);
-        if (qk[k].is_bin) {
-          fk.is_bin = 1;
-          fk.bin_base = plan.keys[k].bin_base;
-          fk.bin_width = plan.keys[k].bin_width;
-        } else if (kind != DK_BOOL) {
-          const ColSide& cs = table->sides[shape_cols[plan.keys[k].col]];
-          if (multi) {   // the dictionary every rank agreed on
-            fk.kd_offs = cs.d_glob_kd_offs;
-            fk.kd_bytes = cs.d_glob_kd_bytes;
-          } else {
-            fk.kd_offs = cs.d_kd_offs;
-            fk.kd_bytes = cs.d_kd_bytes;
-          }
-        }
+      if (pre.rows < n_out) {   // no block yet, or one too small for the groups: lay it out for n_out
+        if (pre.rows && verbose) fprintf(stderr, "[pqb] result tail: %u groups, the block had room for %u: second copy\n", n_out, pre.rows);
+        pre = assemble(n_out, nullptr, keep < n_total);
+        PQB_CUDA(cudaStreamSynchronize(stream));
       }
-      for (uint32_t a = 0; a < d.n_aggs; a++) {
-        fa.aggs[a] = plan.aggs[a];
-        fa.nn_is_rows[a] = nn_is_rows[a];
-        fa.valid_off[a] = take(uint64_t(nbatches) * wpb * 4);
-        fa.out_kind[a] = rank_min_max(plan.aggs[a]) ? DK_STR : bool_min_max(plan.aggs[a]) ? DK_BOOL : DK_I64;   // the layouts of the keys
-        if (fa.out_kind[a] == DK_BOOL) fa.val_off[a] = take(uint64_t(nbatches) * wpb * 4);
-        else if (fa.out_kind[a] == DK_STR) fa.val_off[a] = take((uint64_t(n_out) + 1) * 4);
-        else fa.val_off[a] = take(uint64_t(n_out) * 8);
-      }
-      // MIN / MAX over Utf8: the winning values' bytes, bounded by rows x the longest value of the numbering (any group may
-      // hold the longest one)
-      for (uint32_t a = 0; a < d.n_aggs; a++) {
-        if (fa.out_kind[a] != DK_STR) continue;
-        FinishAggStr& s = fa.astr[a];
-        const ColSide& cs = table->sides[shape_cols[plan.aggs[a].col]];
-        s.kd_offs = multi ? cs.d_glob_kd_offs : cs.d_kd_offs;
-        s.kd_bytes = multi ? cs.d_glob_kd_bytes : cs.d_kd_bytes;
-        s.inv = rank_luts[a] ? rank_luts[a]->inv : nullptr;   // nullptr: a column in no file, every group NULL
-        const uint64_t bound = rank_luts[a] ? uint64_t(n_out) * (multi ? cs.glob_max_len : cs.kd_max_len) : 0;
-        if (bound > 0x7fffffffull)
-          throw Error(PQ_ERR_UNSUPPORTED, std::string(plan.aggs[a].fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
-                                              "): the strings of one result may exceed 2 GiB");
-        s.data_off = take(bound);
-      }
-      uint64_t win_off[2] = {0, 0};
-      for (size_t w = 0; w < win_names.size(); w++) win_off[w] = take(uint64_t(n_out) * 8);
-      // string key bytes: an upper bound (rows x the longest distinct value) keeps the copy to one round trip
-      for (uint32_t k = 0; k < d.n_group_by; k++) {
-        FinishKey& fk = fa.keys[k];
-        if (fk.kind != DK_STR) continue;
-        uint64_t max_len = 0;
-        const KeyDict* kd = qk[k].kd;
-        max_len = multi ? table->sides[shape_cols[plan.keys[k].col]].glob_max_len : table->sides[shape_cols[plan.keys[k].col]].kd_max_len;
-        // the count-based bound is over all the groups; a result cut by ORDER BY ... LIMIT may be any subset of them (the
-        // top 5 rows can all hold the one longest value): rows x the longest value there.  A full ORDER BY holds the same
-        // rows as the unordered result, so the count-based bound still holds for it.
-        const uint64_t bound = keep < n_total ? uint64_t(n_out) * max_len
-                                       : std::min<uint64_t>(uint64_t(n_out) * max_len, uint64_t(n_out / std::max<uint32_t>(fk.card, 1) + 1) * kd->bytes.size());
-        if (bound > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "group key strings of one result exceed 2 GiB");
-        fk.data_off = take(bound);
-      }
-      const uint64_t copy_bytes = off;
-      for (uint32_t k = 0; k < d.n_group_by; k++)
-        if (fa.keys[k].kind == DK_STR) fa.keys[k].len_off = take(uint64_t(n_out) * 4);   // device-only scratch behind the copied part
-      for (uint32_t a = 0; a < d.n_aggs; a++)
-        if (fa.out_kind[a] == DK_STR) fa.astr[a].len_off = take(uint64_t(n_out) * 4);
-      DevBuf<uint8_t> d_block;
-      d_block.alloc(off, stream);
-      PQB_CUDA(cudaMemsetAsync(d_block.p, 0, copy_bytes, stream));
-      if (wrun) {   // the kept groups' slots in output order, their row_number / partition_rows into the block
-        DevBuf<uint32_t> slots;
-        slots.alloc(n_out, stream);
-        auto col = [&](uint32_t flag) -> long long* {
-          if (!(win->flags & flag)) return nullptr;
-          const size_t w = (flag == PQ_WINDOW_PARTITION_ROWS && (win->flags & PQ_WINDOW_ROW_NUMBER)) ? 1 : 0;
-          return reinterpret_cast<long long*>(d_block.p + win_off[w]);
-        };
-        wrun->fill(d_out_slot.p, n_out, slots.p, col(PQ_WINDOW_ROW_NUMBER), col(PQ_WINDOW_PARTITION_ROWS), stream);
-        launches++;
-        std::swap(d_out_slot.p, slots.p);   // the old list is freed with `slots`
-        std::swap(d_out_slot.n, slots.n);
-      }
-      fa.acc = d_acc.p;
-      fa.wide = plan.hashed ? d_hkeys.p : nullptr;
-      fa.out_slot = d_out_slot.p;
-      fa.out = d_block.p;
-      fa.nulls = reinterpret_cast<uint32_t*>(d_block.p + nulls_off);
-      fa.n_out = n_out;
-      fa.nslots = plan.nslots;
-      fa.n_acc = plan.n_acc;
-      fa.naggs = d.n_aggs;
-      fa.nkeys = d.n_group_by;
-      fa.batch_rows = batch_rows;
-      fa.words_per_batch = wpb;
-      fa.nbatches = nbatches;
-      k_agg_finish<<<(n_out + 255) / 256, 256, 0, stream>>>(fa);
-      launches++;
-      for (uint32_t k = 0; k < d.n_group_by; k++) {
-        if (fa.keys[k].kind != DK_STR) continue;
-        k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.keys[k].len_off), n_out,
-                                               reinterpret_cast<int32_t*>(d_block.p + fa.keys[k].val_off));
-        k_key_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, k);
-        launches += 2;
-      }
-      for (uint32_t a = 0; a < d.n_aggs; a++) {
-        if (fa.out_kind[a] != DK_STR) continue;
-        k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.astr[a].len_off), n_out,
-                                               reinterpret_cast<int32_t*>(d_block.p + fa.val_off[a]));
-        k_agg_str_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, a);
-        launches += 2;
-      }
-      PQB_CUDA(cudaGetLastError());
-      auto block = std::make_shared<PinnedBlock>();
-      block->p = ctx.pinned_acquire(copy_bytes);
-      block->bytes = copy_bytes;
-      PQB_CUDA(cudaMemcpyAsync(block->p, d_block.p, copy_bytes, cudaMemcpyDeviceToHost, stream));
-      PQB_CUDA(cudaEventRecord(t_all.b, stream));
-      PQB_CUDA(cudaStreamSynchronize(stream));
-      if (copy_bytes <= kKeepDeviceResult) { block->dev = d_block.p; d_block.p = nullptr; dev_blocks_.push_back(block); }   // JSON egress formats it where it is
-      metrics.d2h_bytes += copy_bytes;
+      Assembled& r = pre;
+      if (r.copy_bytes <= kKeepDeviceResult) { r.block->dev = r.d_block->p; r.d_block->p = nullptr; dev_blocks_.push_back(r.block); }   // JSON egress formats it where it is
       metrics.groups = n_out;
-      const uint32_t* nulls = reinterpret_cast<const uint32_t*>(block->p + nulls_off);
+      const FinishArgs& fa = r.fa;
+      const std::shared_ptr<PinnedBlock>& block = r.block;
+      const uint32_t wpb = r.wpb, ncolumns = r.ncolumns;
+      const uint64_t* win_off = r.win_off;
+      const uint32_t nbatches = (n_out + batch_rows - 1) / batch_rows;   // r.nbatches: the batches the block has room for
+      const uint32_t* nulls = reinterpret_cast<const uint32_t*>(block->p + r.nulls_off);
       for (uint32_t b = 0; b < nbatches; b++) {
         const uint32_t r0 = b * batch_rows, nb = std::min(batch_rows, n_out - r0);
         OutBatch ob;
@@ -2647,7 +2727,7 @@ void Query::run(const PqQueryDesc& d) {
           OutColumn oc;
           oc.ext = block;
           oc.ext_all = true;
-          oc.null_count = nulls[c * nbatches + b];
+          oc.null_count = nulls[c * r.nbatches + b];
           if (c < d.n_group_by) {
             const FinishKey& fk = fa.keys[c];
             const uint32_t qc = uint32_t(d.group_by[c]);
@@ -2792,7 +2872,7 @@ void Query::run(const PqQueryDesc& d) {
         for (uint32_t c = 0; c < npc; c++) {
           if (pj.cols[c].kind != DK_STR) continue;
           // rows beyond the selected total have length 0: the scan over `cap` rows is exact
-          k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + pj.cols[c].len_off), uint32_t(cap),
+          k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + pj.cols[c].len_off), uint32_t(cap), nullptr,
                                                  reinterpret_cast<int32_t*>(d_block.p + pj.cols[c].val_off));
           k_project_bytes<<<uint32_t((cap * 32 + 255) / 256), 256, 0, stream>>>(pj, c, cap);
           launches += 2;

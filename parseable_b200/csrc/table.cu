@@ -90,7 +90,29 @@ void Context::shutdown() {
   std::lock_guard<std::mutex> lk(mu_);
   for (auto& p : pinned_) cudaFreeHost(p.p);
   pinned_.clear();
+  for (auto& [dev, s] : free_streams_) cudaStreamDestroy(s);
+  free_streams_.clear();
   inited_ = false;
+}
+
+cudaStream_t Context::stream_acquire() {
+  {
+    std::lock_guard<std::mutex> lk(mu_);
+    for (size_t i = free_streams_.size(); i-- > 0;) {
+      if (free_streams_[i].first != device_) continue;
+      cudaStream_t s = free_streams_[i].second;
+      free_streams_.erase(free_streams_.begin() + i);
+      return s;
+    }
+  }
+  cudaStream_t s;
+  PQB_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  return s;
+}
+
+void Context::stream_release(cudaStream_t s, int device) {
+  std::lock_guard<std::mutex> lk(mu_);
+  free_streams_.emplace_back(device, s);
 }
 
 uint8_t* Context::pinned_acquire(size_t bytes) {

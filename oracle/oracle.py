@@ -151,6 +151,9 @@ class Oracle:
             v = b.args[0]
             if isinstance(v, Timestamp):
                 v = v.ms
+            if v is None:   # a comparison with NULL is NULL on every row
+                N[:] = 1
+                return T, N
             if c.kind == "str":
                 s = v.encode() if isinstance(v, str) else v
                 L.or_cmp_str(_ptr(c.offsets), _ptr(c.data), _ptr(c.valid), C.c_int64(n), op, s, len(s), _ptr(T), _ptr(N))

@@ -197,6 +197,7 @@ struct Shape {
   DevChunk* d_chunks = nullptr;        // [table row group * ncols + slot]
   DevItem* d_items = nullptr;
   uint32_t n_flat = 0, n_general = 0, n_slab_fast = 0;
+  uint32_t n_uncopied = 0;             // items with a page that has no flat-store copy
   uint32_t bitmap_words = 0;
   std::vector<uint32_t> max_bw, flat_max_bw;          // per slot
   std::vector<uint8_t> has_dict, has_plain, has_delta, flat_plain8, flat_nullable;   // flat_nullable: some flat page of the slot carries a validity bitmap
@@ -252,7 +253,9 @@ class Table {
   mutable std::mutex side_mu;
   mutable std::vector<ColSide> sides;
   mutable std::map<std::vector<int>, std::shared_ptr<Shape>> shapes;
-  std::shared_ptr<Shape> shape_for(const std::vector<int>& tcols, cudaStream_t stream) const;
+  // pieces = false: no item is cut at the page starts of other columns or handed to the flat kernels (k_scan enters
+  // every page of an item at its first row, so it reads only whole-page items)
+  std::shared_ptr<Shape> shape_for(const std::vector<int>& tcols, cudaStream_t stream, bool pieces = true) const;
   void ensure_ent_off(int tcol, cudaStream_t stream) const;
   void ensure_key(int tcol, cudaStream_t stream) const;
   void unify_key(int tcol, cudaStream_t stream) const;        // collective over the pq_comm communicator

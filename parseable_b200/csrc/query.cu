@@ -170,13 +170,9 @@ Tri leaf_from_stats(const HostLeaf& lf, uint8_t kind, const TableChunk& ch, uint
     if (mn == 0.0 || mx == 0.0 || lit == 0.0) return TRI_MAYBE;
     lo_c = mn < lit ? -1 : (mn > lit ? 1 : 0);
     hi_c = mx < lit ? -1 : (mx > lit ? 1 : 0);
-    // a chunk may still hold NaN (greater than everything in totalOrder) outside [min,max]
-    // -> never claim TRI_TRUE/FALSE on the upper side
-    switch (lf.d.cmp) {
-      case PQ_LT: case PQ_LE: return (lf.d.cmp == PQ_LT ? lo_c >= 0 : lo_c > 0) ? TRI_FALSE : TRI_MAYBE;
-      case PQ_EQ: return (lo_c > 0) ? TRI_FALSE : TRI_MAYBE;
-      default: return TRI_MAYBE;
-    }
+    // a chunk may still hold NaN outside [min,max], on either side: totalOrder puts a NaN with the sign bit below -inf
+    // and one without it above +inf.  Only `=` against a non-NaN literal is FALSE on every NaN row.
+    return (lf.d.cmp == PQ_EQ && (lo_c > 0 || hi_c < 0)) ? TRI_FALSE : TRI_MAYBE;
   } else if (kind == DK_STR) {
     auto cmpb = [&](const std::string& a) {
       int c = cmp_bytes((const uint8_t*)a.data(), uint32_t(a.size()), (const uint8_t*)lf.str.data(), uint32_t(lf.str.size()));
@@ -1115,6 +1111,12 @@ void Query::run(const PqQueryDesc& d) {
       switch (op.kind) {
         case PQ_OP_CMP: case PQ_OP_IS_NULL: case PQ_OP_IS_NOT_NULL: case PQ_OP_LIKE: case PQ_OP_REGEX: {
           if (op.col < 0 || uint32_t(op.col) >= d.n_columns) throw Error(PQ_ERR_INVALID_ARG, "predicate column out of range");
+          if (op.kind == PQ_OP_CMP && op.lit.type == PQ_T_NULL) {   // `col <op> NULL` is NULL on every row (SQL)
+            prog.push_back({PK_CONST, 2});
+            has_null_const = true;
+            depth++;
+            break;
+          }
           if (leaves.size() >= (size_t)kMaxLeaves) throw Error(PQ_ERR_UNSUPPORTED, "too many leaf predicates");
           HostLeaf lf;
           lf.qcol = op.col;
@@ -1155,14 +1157,26 @@ void Query::run(const PqQueryDesc& d) {
                   // DataFusion coerces the COLUMN to Float64 and compares there.  Against a literal that is no int64 this
                   // has an exact integer restatement (a non-integer double is < 2^52 in magnitude, where the cast of
                   // any int64 at or beyond it cannot cross it):  v > 100.5  <=>  v > 100,  v < 100.5  <=>  v < 101,
-                  // v = 100.5 never, v != 100.5 always (for non-NULL v).  NaN is the greatest value (totalOrder).
+                  // v = 100.5 never, v != 100.5 always (for non-NULL v).  A NaN sits by its sign bit (totalOrder): above
+                  // every value without it, below every value (-inf included) with it.
                   const double L = op.lit.f64;
                   const int64_t kMin = std::numeric_limits<int64_t>::min();
                   auto never = [&] { lf.d.cmp = PQ_LT; lf.d.lit_i64 = kMin; };    // v < INT64_MIN
                   auto always = [&] { lf.d.cmp = PQ_GE; lf.d.lit_i64 = kMin; };   // v >= INT64_MIN
-                  const bool above = std::isnan(L) || L >= 9223372036854775808.0;   // greater than every int64
-                  const bool below = L < -9223372036854775808.0;                     // less than every int64
-                  if (above || below) {
+                  const bool nan = std::isnan(L);
+                  const bool above = (nan && !std::signbit(L)) || L >= 9223372036854775808.0;   // greater than every int64
+                  const bool below = (nan && std::signbit(L)) || L < -9223372036854775808.0;     // less than every int64
+                  if (L == 9223372036854775808.0) {
+                    // 2^63: the int64 values from 2^63 - 512 up round to it when cast (to nearest, ties to even), the
+                    // others cast below it
+                    const int64_t kTop = std::numeric_limits<int64_t>::max() - 511;
+                    switch (op.cmp) {
+                      case PQ_EQ: case PQ_GE: lf.d.cmp = PQ_GE; lf.d.lit_i64 = kTop; break;
+                      case PQ_NE: case PQ_LT: lf.d.cmp = PQ_LT; lf.d.lit_i64 = kTop; break;
+                      case PQ_LE: always(); break;
+                      default: never(); break;   // PQ_GT
+                    }
+                  } else if (above || below) {
                     const bool lt = op.cmp == PQ_LT || op.cmp == PQ_LE, gt = op.cmp == PQ_GT || op.cmp == PQ_GE;
                     if (op.cmp == PQ_EQ) never();
                     else if (op.cmp == PQ_NE) always();
@@ -1309,7 +1323,8 @@ void Query::run(const PqQueryDesc& d) {
     // p_timestamp): its pages get row-addressable 8-byte copies, once per table
     if (table->sides[shape_cols[s]].has_delta) table->ensure_plain8(shape_cols[s], stream);
   }
-  std::shared_ptr<Shape> shape = table->shape_for(shape_cols, stream);
+  const bool flat_ok = !(getenv("PQB_FLAT_SCAN") && getenv("PQB_FLAT_SCAN")[0] == '0');   // A/B switch: every item on k_scan
+  std::shared_ptr<Shape> shape = table->shape_for(shape_cols, stream, flat_ok);
   const std::vector<DevItem>& items = shape->items;
 
   // is the predicate a pure conjunction of leaves (folded TRUE constants are neutral)?
@@ -1342,6 +1357,44 @@ void Query::run(const PqQueryDesc& d) {
   }
   plan.nleaves = nleaves;
   plan.conj = conj ? 1 : 0;
+  if (verbose) {
+    // PQB_VERBOSE: per live leaf, the flat page kinds under it and the leaf mode each flat piece selects (leaf_ctx in
+    // flat_scan.cuh: a register LUT for a dictionary of <= 32 entries at an index width <= 5), with the index widths
+    // seen per mode; "off-grid" counts the index pieces whose first bit is off the 128-bit grid of the staged copy
+    static const char* const kLeafKind[] = {"?", "CMP", "IS_NULL", "IS_NOT_NULL", "LIKE", "REGEX"};
+    for (size_t l = 0; l < leaves.size(); l++) {
+      if (leaf_slot[l] < 0) continue;
+      const uint32_t s = uint32_t(slot_of[leaves[l].qcol]);
+      uint32_t kinds = 0, widest = 0, offgrid = 0, absent = 0;
+      uint64_t bws[4] = {0, 0, 0, 0};   // REGLUT, MEMLUT, CONST (width 0 under a larger dictionary), other: bit w = width w
+      for (const DevItem& it : items) {
+        if (!(it.fast & kItemFlat)) continue;
+        if ((it.absent >> s) & 1u) { absent++; continue; }
+        const FlatPageRec& fr = table->flat_pages[it.page[s]];
+        kinds |= 1u << fr.fkind;
+        if (fr.fkind != FK_INDEX) continue;
+        widest = std::max<uint32_t>(widest, fr.bw);
+        if (fr.bw && (uint64_t(it.poff[s]) * fr.bw) % 128u) offgrid++;
+        const uint32_t dn = table->row_groups[it.rg].chunks[shape_cols[s]].dict_n;
+        const int m = !value_leaf(leaves[l].d.kind) ? 3 : (fr.bw <= 5 && dn <= 32) ? 0 : fr.bw == 0 ? 2 : 1;
+        bws[m] |= 1ull << std::min<uint32_t>(fr.bw, 63);
+      }
+      std::string pk, modes;
+      static const char* const kFlat[] = {"NONE", "INDEX", "PLAIN8", "BITS", "BYTES"};
+      for (uint32_t k = 0; k < 5; k++) if ((kinds >> k) & 1u) pk += (pk.empty() ? "" : "+") + std::string(kFlat[k]);
+      static const char* const kMode[] = {"REGLUT", "MEMLUT", "CONST"};
+      for (int m = 0; m < 3; m++) {
+        if (!bws[m]) continue;
+        modes += std::string(" ") + kMode[m] + "{";
+        for (uint32_t w = 0, first = 1; w < 64; w++) if ((bws[m] >> w) & 1ull) { modes += (first ? "" : ",") + std::to_string(w); first = 0; }
+        modes += "}";
+      }
+      fprintf(stderr, "[pqb] leaf %d: column '%s', %s, flat pages %s, widest index %u, register LUT %s, off-grid %u, absent %u,%s\n",
+              leaf_slot[l], table->columns[shape_cols[s]].name.c_str(), kLeafKind[leaves[l].d.kind < 6 ? leaves[l].d.kind : 0],
+              pk.empty() ? "-" : pk.c_str(), widest, bws[0] ? (bws[1] || bws[2] ? "some" : "all") : "none", offgrid, absent,
+              modes.empty() ? " -" : modes.c_str());
+    }
+  }
   // per column: the leaves a dictionary LUT answers (k_scan fuses up to two into the unpack)
   for (uint32_t c = 0; c < (uint32_t)kMaxCols; c++) { plan.col_nlut[c] = 0; plan.col_l0[c] = -1; plan.col_l1[c] = -1; }
   for (uint32_t l = 0; l < nleaves; l++) {
@@ -1502,7 +1555,7 @@ void Query::run(const PqQueryDesc& d) {
     plan.cols[s].max_bw = shape->max_bw[s];
     if (shape->has_delta[s] && plan.cols[s].kind != DK_I64)
       throw Error(PQ_ERR_UNSUPPORTED, "column '" + cname + "': DELTA_BINARY_PACKED is decoded for INT64 columns only");
-    if (shape->has_plain[s] && plan.cols[s].kind == DK_STR && shape->n_general)
+    if (shape->has_plain[s] && plan.cols[s].kind == DK_STR && shape->n_uncopied)
       throw Error(PQ_ERR_UNSUPPORTED, "column '" + cname + "': PLAIN (dictionary-fallback) string pages without a flat-store copy are not decoded on the GPU");
   }
   // k_flat_agg walks a regular expression's DFA per row only in its RX instantiations
@@ -1871,7 +1924,6 @@ void Query::run(const PqQueryDesc& d) {
 
   // ---- which kernels run ----
   (void)has_null_const;   // the flat kernels evaluate SQL three-valued logic, NULL literals included
-  const bool flat_ok = !(getenv("PQB_FLAT_SCAN") && getenv("PQB_FLAT_SCAN")[0] == '0');
   plan.no_flat = flat_ok ? 0 : 1;
   const uint32_t n_flat = flat_ok ? shape->n_flat : 0;
   const uint32_t n_general = flat_ok ? shape->n_general : uint32_t(items.size());
@@ -2282,7 +2334,8 @@ void Query::run(const PqQueryDesc& d) {
               plan.lane_slots, plan.replicas, plan.smem_share, plan.f64_global, __builtin_popcount(plan.agg_forms & value_forms),
               __builtin_popcount(plan.agg_forms & ~value_forms), n_flat);
     else if (verbose)
-      fprintf(stderr, "[pqb] k_flat_filter: %u CTAs, %u B smem/CTA, %u stages x %u B, slab %u rows, hot slots %u of %u, %u copies, %u flat items\n",
+      fprintf(stderr, "[pqb] k_flat_filter<%s>: %u live leaves, %u CTAs, %u B smem/CTA, %u stages x %u B, slab %u rows, hot slots %u of %u, "
+              "%u copies, %u flat items\n", (plan.conj || !plan.npred) ? "CONJ" : "KLEENE", plan.nleaves,
               grid, FL.total, FL.nstages, FL.stage_bytes, plan.flat_slab_rows, plan.hot_slots, plan.nslots, plan.replicas, n_flat);
   }
   if (n_general && nrg) {

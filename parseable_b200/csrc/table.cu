@@ -1191,9 +1191,11 @@ void Table::build_flat_store(cudaStream_t stream) {
 }
 
 // ---- per column-set shape: chunk table + work items (built once, reused by every query) ----------
-std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStream_t stream) const {
+std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStream_t stream, bool pieces) const {
   std::lock_guard<std::mutex> lk(side_mu);
-  auto it = shapes.find(tcols);
+  std::vector<int> key = tcols;
+  if (!pieces) key.push_back(-1);   // a shape of its own
+  auto it = shapes.find(key);
   if (it != shapes.end()) return it->second;
   auto sh = std::make_shared<Shape>();
   sh->tcols = tcols;
@@ -1287,7 +1289,7 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
       it.nrows = (i + 1 < common.size() ? common[i + 1] : rg.num_rows) - common[i];
       it.global_row0 = rg.global_row0 + common[i];
       const uint32_t row_end = it.row0 + it.nrows;
-      bool fast = use_slab_index, flat = use_flat && it.nrows != 0;
+      bool fast = use_slab_index, copied = use_flat && it.nrows != 0;
       cuts.clear();
       for (uint32_t s = 0; s < ncols; s++) {
         const TableChunk& tc = rg.chunks[tcols[s]];
@@ -1299,7 +1301,7 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
         // every page of this column under the item needs a flat copy; their starts cut the item into pieces
         for (uint32_t pi = it.page[s]; pi < tc.pages.first_page + tc.pages.n_pages && pages[pi].first_row < row_end; pi++) {
           if (flat_pages.empty() || flat_pages[pi].fkind == FK_NONE) {
-            flat = false;
+            copied = false;
             if (sh->why_general.empty())
               sh->why_general = "column '" + columns[tcols[s]].name + "', row group " + std::to_string(g) + ", page " + std::to_string(pi - tc.pages.first_page) +
                                 " (encoding " + std::to_string(pages[pi].enc) + ", " + std::to_string(pages[pi].num_rows) + " rows) has no flat-store copy";
@@ -1308,7 +1310,8 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
         }
       }
       if (!it.nrows) fast = false;
-      if (!flat) { push_item(it, false, fast); continue; }
+      sh->n_uncopied += copied ? 0 : 1;
+      if (!copied || !pieces) { push_item(it, false, fast); continue; }
       // flat: one piece per stretch between page starts of ANY column (a piece lies in one page of every column)
       std::sort(cuts.begin(), cuts.end());
       cuts.erase(std::unique(cuts.begin(), cuts.end()), cuts.end());
@@ -1337,7 +1340,7 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
   if (!sh->items.empty())
     PQB_CUDA(cudaMemcpyAsync(sh->d_items, sh->items.data(), sh->items.size() * sizeof(DevItem), cudaMemcpyHostToDevice, stream));
   PQB_CUDA(cudaStreamSynchronize(stream));
-  shapes.emplace(tcols, sh);
+  shapes.emplace(key, sh);
   return sh;
 }
 

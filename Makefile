@@ -38,7 +38,16 @@ oracle: oracle/liboracle.so
 oracle/liboracle.so: oracle/oracle.c
 	$(CC) -O2 -std=c11 -fPIC -shared -Wall -o $@ $< -lm
 
-tools: tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so
+tools: tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so \
+       tools/liblz_host.so tools/liblz_host_desc.so tools/libdecomp_dev.so
+# the LZ4_RAW / SNAPPY decoders on the host, lanes in ascending and in descending order
+tools/liblz_host.so: tools/lz_host.cpp $(CSRC)/lz_decode.cuh $(CSRC)/zstd_decode.cuh
+	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
+tools/liblz_host_desc.so: tools/lz_host.cpp $(CSRC)/lz_decode.cuh $(CSRC)/zstd_decode.cuh
+	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -DLZ_LANES_DESCENDING=1 -I$(CSRC) -o $@ $<
+# the page decoder kernels, launched as table.cu launches them (GPU tests only)
+tools/libdecomp_dev.so: tools/decomp_dev.cu $(HDRS)
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -shared -o $@ $< -lcudart
 tools/libregex_host.so: tools/regex_host.cpp $(CSRC)/regex_compile.cpp $(CSRC)/regex_compile.hpp $(CSRC)/regex_match.cuh $(CSRC)/regex_unicode.inc
 	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 tools/liborder_keys_host.so: tools/order_keys_host.cpp $(CSRC)/order_keys.cuh $(CSRC)/percentile_core.cuh $(CSRC)/decode_core.cuh $(CSRC)/device_structs.hpp
@@ -51,6 +60,7 @@ tools/libdecode_core_host.so: tools/decode_core_host.cpp $(CSRC)/decode_core.cuh
 	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 
 clean:
-	rm -rf $(OBJDIR) $(LIB) oracle/liboracle.so tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so
+	rm -rf $(OBJDIR) $(LIB) oracle/liboracle.so tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so \
+	      tools/liblz_host.so tools/liblz_host_desc.so tools/libdecomp_dev.so
 
 .PHONY: all oracle tools clean

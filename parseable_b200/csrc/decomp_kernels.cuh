@@ -2,18 +2,21 @@
 // /root/reference/src/cli.rs:441-448), SNAPPY (what the reference's CI pins,
 // docker-compose-test.yaml:45), ZSTD and GZIP (zstd_decode.cuh, inflate_decode.cuh; k_decompress_zstd below).  The reference gets these from the lz4_flex 0.13 /
 // snap 1.1 crates through parquet 58.1.0 (SURVEY.md §8 row a10); here one warp
-// decodes one page: every lane parses the (tiny) sequence headers redundantly — the
-// loads broadcast — and the 32 lanes share the literal / match copies.
+// decodes one page (the formats: lz_decode.cuh).  table.cu and the test library
+// tools/decomp_dev.cu both go through launch_decompress below.
 //
 // Output goes into the same HBM arena the scan kernel reads, so a compressed file
 // costs one extra HBM write + read of the decoded pages and nothing else changes.
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
+#include <vector>
 
 #include "device_structs.hpp"
 #include "inflate_decode.cuh"
+#include "lz_decode.cuh"
 #include "zstd_decode.cuh"
 
 namespace pqb {
@@ -23,164 +26,26 @@ struct DecompJob {
   uint64_t dst_off;   // decoded page payload inside the arena
   uint32_t src_len;
   uint32_t dst_len;   // uncompressed_page_size from the page header
-  uint32_t codec;     // parquet CompressionCodec: 7 LZ4_RAW, 1 SNAPPY, 0 plain copy
+  uint32_t codec;     // parquet CompressionCodec: 7 LZ4_RAW, 1 SNAPPY, 6 ZSTD, 2 GZIP, 0 plain copy (src_len must equal dst_len)
   uint32_t _pad;
 };
 
-// literal run: `len` bytes that do not overlap, any alignment of source and destination.  A page of incompressible
-// bit-packed indices or PLAIN doubles is ONE literal run of 40-160 KB handled by one warp, so the copy must keep many
-// bytes in flight: the destination is walked in aligned 16-byte chunks, every lane builds its chunk from five aligned
-// source words with a funnel shift (the source sits at an arbitrary byte phase), four chunks per lane and trip.
-__device__ __forceinline__ void warp_literal_copy(uint8_t* __restrict__ d, const uint8_t* __restrict__ s, uint32_t len, uint32_t lane) {
-  uint32_t head = uint32_t(-reinterpret_cast<uintptr_t>(d)) & 15u;   // bytes until d is 16-byte aligned
-  if (head > len) head = len;
-  if (lane < head) d[lane] = s[lane];
-  d += head; s += head; len -= head;
-  const uint32_t n16 = len >> 4;
-  if (n16) {
-    const uint32_t sh = (uint32_t(reinterpret_cast<uintptr_t>(s)) & 3u) * 8u;
-    const uint32_t* sw = reinterpret_cast<const uint32_t*>(reinterpret_cast<uintptr_t>(s) & ~uintptr_t(3));
-    uint4* dw = reinterpret_cast<uint4*>(d);
-    uint32_t c = lane;
-    for (; c + 3 * 32 < n16; c += 4 * 32) {
-      uint32_t w[4][5];
-#pragma unroll
-      for (int k = 0; k < 4; k++)
-#pragma unroll
-        for (int j = 0; j < 5; j++) w[k][j] = (j < 4 || sh) ? sw[(c + k * 32) * 4 + j] : 0u;   // the fifth word only when the phase needs it (it may lie past the source)
-#pragma unroll
-      for (int k = 0; k < 4; k++)
-        dw[c + k * 32] = make_uint4(__funnelshift_r(w[k][0], w[k][1], sh), __funnelshift_r(w[k][1], w[k][2], sh),
-                                    __funnelshift_r(w[k][2], w[k][3], sh), __funnelshift_r(w[k][3], w[k][4], sh));
-    }
-    for (; c < n16; c += 32) {
-      uint32_t w[5];
-#pragma unroll
-      for (int j = 0; j < 5; j++) w[j] = (j < 4 || sh) ? sw[c * 4 + j] : 0u;
-      dw[c] = make_uint4(__funnelshift_r(w[0], w[1], sh), __funnelshift_r(w[1], w[2], sh), __funnelshift_r(w[2], w[3], sh), __funnelshift_r(w[3], w[4], sh));
-    }
-  }
-  const uint32_t done = n16 << 4;
-  if (done + lane < len) d[done + lane] = s[done + lane];   // < 16 bytes left
-}
-
-// match copy with LZ77 overlap semantics: the source pattern [dp-off, dp) already exists, bytes
-// beyond it repeat with period `off`
-__device__ __forceinline__ void warp_match_copy(uint8_t* d, uint32_t dp, uint32_t off, uint32_t len, uint32_t lane) {
-  if (off >= len) {
-    for (uint32_t i = lane; i < len; i += 32) d[dp + i] = d[dp - off + i];
-  } else {
-    for (uint32_t i = lane; i < len; i += 32) d[dp + i] = d[dp - off + (i % off)];
-  }
-}
-
 __global__ void k_decompress_pages(const DecompJob* __restrict__ jobs, uint32_t njobs, const uint8_t* __restrict__ src_base,
                                    uint8_t* __restrict__ arena, unsigned long long* __restrict__ counters) {
-  const uint32_t lane = threadIdx.x & 31;
   const uint32_t j = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (j >= njobs) return;
   const DecompJob job = jobs[j];
   const uint8_t* s = src_base + job.src_off;
   uint8_t* d = arena + job.dst_off;
-  const uint32_t sn = job.src_len, dn = job.dst_len;
-  uint32_t sp = 0, dp = 0;
-  bool bad = false;
-  if (job.codec == 0) {
-    warp_literal_copy(d, s, sn < dn ? sn : dn, lane);
-    return;
-  }
-  if (job.codec == 7) {
-    // ---- LZ4 block format: token | literal length ext | literals | offset(2) | match length ext ----
-    while (sp < sn) {
-      const uint32_t token = s[sp++];
-      uint32_t lit = token >> 4;
-      if (lit == 15) {
-        uint32_t b;
-        do { if (sp >= sn) { bad = true; break; } b = s[sp++]; lit += b; } while (b == 255);
-      }
-      if (bad || sp + lit > sn || dp + lit > dn) { bad = true; break; }
-      warp_literal_copy(d + dp, s + sp, lit, lane);
-      sp += lit;
-      dp += lit;
-      if (sp >= sn) break;  // the last sequence carries literals only
-      if (sp + 2 > sn) { bad = true; break; }
-      const uint32_t off = uint32_t(s[sp]) | (uint32_t(s[sp + 1]) << 8);
-      sp += 2;
-      uint32_t ml = token & 15;
-      if (ml == 15) {
-        uint32_t b;
-        do { if (sp >= sn) { bad = true; break; } b = s[sp++]; ml += b; } while (b == 255);
-      }
-      ml += 4;
-      if (bad || off == 0 || off > dp || dp + ml > dn) { bad = true; break; }
-      __syncwarp();  // the literals just written may be the match source
-      warp_match_copy(d, dp, off, ml, lane);
-      dp += ml;
-      __syncwarp();
-    }
-  } else {
-    // ---- Snappy: varint uncompressed length, then tagged elements ----
-    uint32_t ulen = 0, shift = 0;
-    while (sp < sn) {
-      uint32_t b = s[sp++];
-      ulen |= (b & 0x7f) << shift;
-      shift += 7;
-      if (!(b & 0x80) || shift > 28) break;
-    }
-    if (ulen != dn) bad = true;
-    while (!bad && sp < sn) {
-      const uint32_t tag = s[sp++];
-      const uint32_t kind = tag & 3;
-      if (kind == 0) {
-        uint32_t len = (tag >> 2) + 1;
-        if (len > 60) {
-          const uint32_t nb = len - 60;
-          if (sp + nb > sn) { bad = true; break; }
-          len = 0;
-          for (uint32_t k = 0; k < nb; k++) len |= uint32_t(s[sp + k]) << (8 * k);
-          len += 1;
-          sp += nb;
-        }
-        if (sp + len > sn || dp + len > dn) { bad = true; break; }
-        warp_literal_copy(d + dp, s + sp, len, lane);
-        sp += len;
-        dp += len;
-        __syncwarp();
-      } else {
-        uint32_t len, off;
-        if (kind == 1) {
-          if (sp + 1 > sn) { bad = true; break; }
-          len = 4 + ((tag >> 2) & 7);
-          off = ((tag >> 5) << 8) | s[sp];
-          sp += 1;
-        } else if (kind == 2) {
-          if (sp + 2 > sn) { bad = true; break; }
-          len = (tag >> 2) + 1;
-          off = uint32_t(s[sp]) | (uint32_t(s[sp + 1]) << 8);
-          sp += 2;
-        } else {
-          if (sp + 4 > sn) { bad = true; break; }
-          len = (tag >> 2) + 1;
-          off = uint32_t(s[sp]) | (uint32_t(s[sp + 1]) << 8) | (uint32_t(s[sp + 2]) << 16) | (uint32_t(s[sp + 3]) << 24);
-          sp += 4;
-        }
-        if (off == 0 || off > dp || dp + len > dn) { bad = true; break; }
-        __syncwarp();
-        warp_match_copy(d, dp, off, len, lane);
-        dp += len;
-        __syncwarp();
-      }
-    }
-  }
-  if ((bad || dp != dn) && lane == 0) atomicExch(&counters[0], 1ull);
+  bool ok = false;
+  if (job.codec == 7) ok = lz4_raw_decode(s, job.src_len, d, job.dst_len);
+  else if (job.codec == 1) ok = snappy_decode(s, job.src_len, d, job.dst_len);
+  else if (job.codec == 0) ok = stored_decode(s, job.src_len, d, job.dst_len);
+  if (!ok && (threadIdx.x & 31) == 0) atomicExch(&counters[0], 1ull);
 }
 
 // ZSTD (codec 6) and GZIP (codec 2) pages: persistent warps draw pages from a counter; every warp owns one workspace
 // (tables + the literals of one zstd block) in global memory.  zstd_decode.cuh / inflate_decode.cuh hold the formats.
-union HeavyWs {
-  ZstdWs z;
-  InflateWs g;
-};
 __global__ void __launch_bounds__(128) k_decompress_zstd(const DecompJob* __restrict__ jobs, uint32_t njobs, const uint8_t* __restrict__ src_base,
                                                          uint8_t* __restrict__ arena, unsigned long long* __restrict__ counters,
                                                          HeavyWs* __restrict__ ws, unsigned int* __restrict__ next) {
@@ -192,11 +57,37 @@ __global__ void __launch_bounds__(128) k_decompress_zstd(const DecompJob* __rest
     j = __shfl_sync(0xffffffffu, j, 0);
     if (j >= njobs) break;
     const DecompJob job = jobs[j];
-    const bool ok = job.codec == 2u ? gzip_decode(w.g, src_base + job.src_off, job.src_len, arena + job.dst_off, job.dst_len)
-                                    : zstd_decode(w.z, src_base + job.src_off, job.src_len, arena + job.dst_off, job.dst_len);
+    const bool ok = heavy_page_decode(w, job.codec, src_base + job.src_off, job.src_len, arena + job.dst_off, job.dst_len);
     if (!ok && lane == 0) atomicExch(&counters[0], 1ull);
     __syncwarp();
   }
+}
+
+// Queues the decoding of `djobs` on `stream`: src_base holds the compressed payloads (with 256 bytes of slack behind
+// the last: the literal copy reads up to 3 bytes past a literal), arena receives the pages, *flag (zeroed by the
+// caller) becomes nonzero when a page does not decode to its declared size.  djobs is reordered: ZSTD / GZIP pages
+// go behind the others, their decoders are a kernel of their own (persistent warps, one workspace each).  The job
+// list, the workspaces and the ticket counter are allocated here on `stream` and handed back for the caller to free
+// once the stream is done; whatever this allocated is in them even when it returns an error.
+inline cudaError_t launch_decompress(std::vector<DecompJob>& djobs, const uint8_t* src_base, uint8_t* arena, unsigned long long* flag,
+                                     int sm_count, cudaStream_t stream, DecompJob** d_djobs, HeavyWs** d_ws, unsigned int** d_next) {
+  if (djobs.empty()) return cudaSuccess;
+  cudaError_t e = cudaMallocAsync((void**)d_djobs, djobs.size() * sizeof(DecompJob), stream);
+  if (e != cudaSuccess) return e;
+  const uint32_t n_other = uint32_t(std::stable_partition(djobs.begin(), djobs.end(), [](const DecompJob& j) { return j.codec != 6u && j.codec != 2u; }) - djobs.begin());
+  const uint32_t n_heavy = uint32_t(djobs.size()) - n_other;
+  if ((e = cudaMemcpyAsync(*d_djobs, djobs.data(), djobs.size() * sizeof(DecompJob), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
+  if (n_other) k_decompress_pages<<<(n_other + 3) / 4, 128, 0, stream>>>(*d_djobs, n_other, src_base, arena, flag);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  if (n_heavy) {
+    const uint32_t blocks = std::min<uint32_t>((n_heavy + 3) / 4, uint32_t(sm_count) * 2u);
+    if ((e = cudaMallocAsync((void**)d_ws, size_t(blocks) * 4 * sizeof(HeavyWs), stream)) != cudaSuccess) return e;
+    if ((e = cudaMallocAsync((void**)d_next, 4, stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(*d_next, 0, 4, stream)) != cudaSuccess) return e;
+    k_decompress_zstd<<<blocks, 128, 0, stream>>>(*d_djobs + n_other, n_heavy, src_base, arena, flag, *d_ws, *d_next);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 // After decompression the host still does not know two bytes it normally reads from the file:

@@ -238,4 +238,14 @@ ZS_FN_NOINLINE bool gzip_decode(InflateWs& w, const uint8_t* src, uint32_t sn, u
   return dp == dn;
 }
 
+// The workspace of one k_decompress_zstd warp (decomp_kernels.cuh): it decodes page after page, ZSTD and GZIP mixed,
+// in the same memory.  Parquet codec 2 is GZIP, anything else reaching here is ZSTD (codec 6).
+union HeavyWs {
+  ZstdWs z;
+  InflateWs g;
+};
+ZS_FN bool heavy_page_decode(HeavyWs& w, uint32_t codec, const uint8_t* src, uint32_t sn, uint8_t* dst, uint32_t dn) {
+  return codec == 2u ? gzip_decode(w.g, src, sn, dst, dn) : zstd_decode(w.z, src, sn, dst, dn);
+}
+
 }  // namespace pqb

@@ -764,23 +764,9 @@ void Table::open(const PqFile* in_files, uint32_t n_files, const std::vector<std
   unwind.own(d_zws);
   unwind.own(d_znext);
   if (!djobs.empty()) {
-    PQB_CUDA(cudaMallocAsync((void**)&d_djobs, djobs.size() * sizeof(DecompJob), stream));
     PQB_CUDA(cudaMallocAsync((void**)&d_dflag, 8, stream));
     PQB_CUDA(cudaMemsetAsync(d_dflag, 0, 8, stream));
-    // ZSTD / GZIP pages are sorted behind the others: their decoders are a kernel of their own (persistent warps, one workspace each)
-    const uint32_t n_other = uint32_t(std::stable_partition(djobs.begin(), djobs.end(), [](const DecompJob& j) { return j.codec != uint32_t(CODEC_ZSTD) && j.codec != uint32_t(CODEC_GZIP); }) - djobs.begin());
-    const uint32_t n_zstd = uint32_t(djobs.size()) - n_other;
-    PQB_CUDA(cudaMemcpyAsync(d_djobs, djobs.data(), djobs.size() * sizeof(DecompJob), cudaMemcpyHostToDevice, stream));
-    if (n_other) k_decompress_pages<<<(n_other + 3) / 4, 128, 0, stream>>>(d_djobs, n_other, d_comp, d_arena, d_dflag);
-    PQB_CUDA(cudaGetLastError());
-    if (n_zstd) {
-      const uint32_t blocks = std::min<uint32_t>((n_zstd + 3) / 4, uint32_t(ctx.sm_count()) * 2u);
-      PQB_CUDA(cudaMallocAsync((void**)&d_zws, size_t(blocks) * 4 * sizeof(HeavyWs), stream));
-      PQB_CUDA(cudaMallocAsync((void**)&d_znext, 4, stream));
-      PQB_CUDA(cudaMemsetAsync(d_znext, 0, 4, stream));
-      k_decompress_zstd<<<blocks, 128, 0, stream>>>(d_djobs + n_other, n_zstd, d_comp, d_arena, d_dflag, d_zws, d_znext);
-      PQB_CUDA(cudaGetLastError());
-    }
+    PQB_CUDA(launch_decompress(djobs, d_comp, d_arena, d_dflag, ctx.sm_count(), stream, &d_djobs, &d_zws, &d_znext));
   }
   // ---- page walks, in parallel, while the copies above are in flight ----
   {

@@ -9,7 +9,8 @@
 // broadcast, like the LZ4 decoder in decomp_kernels.cuh); the parallel parts are shared: the four
 // Huffman streams of a literals section go to four lanes, literal and match copies to all 32.
 // The same source compiles for the host (one "lane"): tools/zstd_host.cpp exposes it to
-// tests/test_zstd.py, which checks it against pyarrow's zstd on the CPU.
+// tests/test_zstd.py, which checks it against pyarrow's zstd on the CPU, and tools/decomp_dev.cu runs the kernel
+// itself over the same inputs on the GPU.
 #pragma once
 #include <cstdint>
 

@@ -161,3 +161,38 @@ def test_gzip_garbled_input_is_refused_without_faults(zs):
             g[int(rng.integers(0, len(g)))] ^= 1 << int(rng.integers(0, 8))
         refused += 0 if zs(bytes(g), len(data), gz=True)[0] else 1     # CRC-32 is not verified: a flip inside literals may pass
     assert refused > 50
+
+
+# ---- the same inputs through the GPU kernels (k_decompress_zstd: 32 lanes, four Huffman streams on lanes 0-3,
+# persistent warps taking pages by ticket) -- one launch per test, every page at its own source phase ----
+@pytest.mark.gpu
+def test_gpu_zstd_levels():
+    from test_page_codecs import ZSTD, DevImages
+    im = DevImages()
+    for li, level in enumerate([None, -5, 1, 3, 9, 19, 22]):
+        codec = pa.Codec("zstd") if level is None else pa.Codec("zstd", compression_level=level)
+        for k, (name, data) in enumerate(_inputs()):
+            im.add(ZSTD, codec.compress(data, asbytes=True), data, sphase=(li + k) % 16, odd=k % 2 == 1)
+    dst, flag = im.run()
+    assert flag == 0
+    im.check(dst)
+
+
+@pytest.mark.gpu
+def test_gpu_gzip_variants():
+    import gzip
+    import zlib
+    from test_page_codecs import GZIP, DevImages
+    im = DevImages()
+    for li, level in enumerate([1, 6, 9]):
+        for k, (name, data) in enumerate(_inputs()):
+            h = len(data) // 2
+            co = zlib.compressobj(level, zlib.DEFLATED, 31, 9, zlib.Z_FIXED)
+            for v, comp in enumerate((pa.Codec("gzip", compression_level=level).compress(data, asbytes=True),
+                                      gzip.compress(data, compresslevel=level),
+                                      co.compress(data) + co.flush(),
+                                      gzip.compress(data[:h], compresslevel=0) + gzip.compress(data[h:], compresslevel=level))):
+                im.add(GZIP, comp, data, sphase=(li + k + v) % 16, odd=(k + v) % 2 == 1)
+    dst, flag = im.run()
+    assert flag == 0
+    im.check(dst)

@@ -312,53 +312,6 @@ PQ_HD uint32_t bp_get(const uint32_t* words, uint32_t bitoff, uint32_t bw, uint3
   return bw >= 32 ? v : (v & ((1u << bw) - 1u));
 }
 
-// ---- hybrid stream -> flat bit-packed stream ----------------------------------------------------
-// Skewed low-cardinality columns (a `status` that is 200 four times out of five) alternate short
-// RLE runs and single bit-packed groups: hundreds of run headers per 2048 rows, far more than a
-// run directory should hold.  For such pages the slab index keeps a flat copy instead: every value
-// at bw bits, LSB first, no headers — exactly what a single bit-packed run would hold — so a slab is
-// one directory entry and an octet is always bw consecutive bytes.
-struct BitWriter {
-  uint32_t* out;
-  uint64_t acc;
-  uint32_t nbits;
-};
-PQ_HD void bitwriter_put(BitWriter& b, uint32_t v, uint32_t bw) {
-  b.acc |= uint64_t(v) << b.nbits;
-  b.nbits += bw;
-  if (b.nbits >= 32) {
-    *b.out++ = uint32_t(b.acc);
-    b.acc >>= 32;
-    b.nbits -= 32;
-  }
-}
-PQ_HD void bitwriter_flush(BitWriter& b) {
-  if (b.nbits) { *b.out++ = uint32_t(b.acc); b.acc = 0; b.nbits = 0; }
-}
-// Append the next `n` values of the stream to the writer; returns the values written (< n: corrupt).
-PQ_HD uint32_t transcode_values(StreamState& s, const uint8_t* arena, uint32_t n, BitWriter& b) {
-  const uint32_t bw = s.bw;
-  uint32_t done = 0;
-  while (done < n) {
-    const uint64_t base = stream_window_start(s) & ~15ull;
-    const uint64_t span = s.end > base ? s.end - base : 0;
-    const Window w{arena + base, base, span > 0x1000000ull ? 0x1000000u : uint32_t(span)};
-    DirEntry tmp[8];
-    uint32_t m = 0;
-    const uint32_t got = walk_stream(s, w, n - done, tmp, m, 8);
-    if (got == 0) break;
-    const uint32_t* words = reinterpret_cast<const uint32_t*>(arena + base);
-    for (uint32_t e = 0; e < m; e++) {
-      const DirEntry d = tmp[e];
-      if (bw == 0) continue;
-      if (d.kind) for (uint32_t j = 0; j < d.count; j++) bitwriter_put(b, bp_get(words, d.payload, bw, j), bw);
-      else for (uint32_t j = 0; j < d.count; j++) bitwriter_put(b, d.payload, bw);
-    }
-    done += got;
-  }
-  return done;
-}
-
 // Unaligned little-endian 8-byte load built from two aligned 8-byte loads.  The
 // arena keeps 16 bytes of slack after every chunk, so the second load is in bounds.
 PQ_HD uint64_t load_u64_unaligned(const uint8_t* p) {

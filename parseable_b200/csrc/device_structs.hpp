@@ -18,8 +18,8 @@ constexpr int kDirEntryMaxValues = 512;
 constexpr int kMaxDeltaEntries = 80;  // DELTA_BINARY_PACKED miniblock directory entries per slab
 constexpr int kDeltaWindowBytes = 8192 + 64;
 constexpr int kPredStack = 8;
-constexpr int kFastDirEntries = 16;   // slab index: run-directory entry budget per slab (a page's slabs share the page's budget)
-constexpr int kRecBatch = 16;         // slab records a CTA keeps in shared memory at a time
+// k_scan: staged window bytes for one slab of a dictionary-index stream of the given bit width
+inline uint32_t valwin_cap_for_bw(uint32_t max_bw) { return ((kSlabRows * max_bw / 8 + kSlabRows / 8 + 64) + 15u) & ~15u; }
 
 // page value encodings as the kernels see them
 enum DevEnc : uint8_t { DE_DICT = 0, DE_PLAIN = 1, DE_DELTA = 2, DE_RLE_BOOL = 3,
@@ -42,8 +42,6 @@ struct DevPage {               // one data page
   uint8_t bit_width;           // DE_DICT: index bit width
   uint16_t chunk_slot;         // table column of this page
   uint32_t chunk;              // index into chunks[]
-  uint32_t slab0;              // first record of this page in the table's slab index
-  uint32_t flags;              // host copy only: bit 0 = every slab of the page is in the slab index
 };
 
 // DELTA_BYTE_ARRAY / DELTA_LENGTH_BYTE_ARRAY pages are rewritten as PLAIN BYTE_ARRAY pages at table open (flat_store.cuh)
@@ -92,25 +90,11 @@ struct DevItem {               // unit of CTA work: rows between two page bounda
   uint64_t global_row0;        // ordinal of row0 in the scanned table (row-id output)
   uint32_t page[kMaxCols];     // page index (into pages[]) holding row0, per column slot
   uint32_t poff[kMaxCols];     // flat items: row0 minus the page's first row (a piece may start inside a page)
-  uint32_t fast;               // bit 0: every referenced column has exactly one, slab-indexed page over this item (k_scan);
-                               // bit 1: ... exactly one page with a flat-store copy (k_flat_*)
+  uint32_t fast;               // kItemFlat: every referenced column has exactly one page with a flat-store copy over this
+                               // item (k_flat_*); 0: k_scan reads it
   uint32_t absent;             // flat items: bit s = column slot s is missing from this file (reads as all NULL)
 };
-constexpr uint32_t kItemSlabIndexed = 1u, kItemFlat = 2u;
-
-// One slab (kSlabRows rows from the page start) of one page in the table's slab index
-// (k_slab_index, built when the table is opened): what the per-slab control of k_scan would derive
-// by walking the run headers, computed for every page at once.
-struct DevSlabRec {
-  uint64_t win_off;            // arena offset the value window is staged from (16-byte aligned)
-  uint64_t val_base;           // arena offset of the page's values section
-  uint32_t vals_done;          // values of the page consumed before this slab
-  uint16_t nent;               // run-directory entries (two sentinels follow)
-  uint8_t enc;                 // DevEnc
-  uint8_t bw;                  // index bit width
-  uint32_t ent0;               // first run-directory entry of this slab in the index (entries are 16 bytes)
-  uint32_t _pad;
-};
+constexpr uint32_t kItemFlat = 2u;
 
 struct DevColumn {
   uint8_t kind;                // DevKind
@@ -281,16 +265,10 @@ struct DevScanArgs {
   unsigned long long* acc;     // accumulator table (global)
   unsigned long long* hkeys;   // hashed group-by: wide group id per accumulator slot (~0: empty)
   unsigned long long* counters;  // [0] rows selected, [1] error flag, [2] work-queue head
-  // the table's slab index (fast items)
-  const DevSlabRec* slab_recs;       // [page.slab0 + k]
-  const struct DirEntry* slab_dirs;  // [rec.ent0 + e]
 };
 
-// one page the second pass of the slab index re-packs flat (k_flatten_pages)
-struct FlatJob { uint32_t page; uint32_t _pad; uint64_t side_off; };
-
 // run-directory entry produced by the stream walker
-struct DirEntry {     // 16 bytes: bulk-copyable (TMA) from the prebuilt slab directory
+struct DirEntry {     // 16 bytes
   uint32_t start;    // first value (slab relative)
   uint16_t count;
   uint8_t kind;      // 0 RLE, 1 bit-packed

@@ -196,7 +196,7 @@ struct Shape {
   std::vector<DevItem> items;
   DevChunk* d_chunks = nullptr;        // [table row group * ncols + slot]
   DevItem* d_items = nullptr;
-  uint32_t n_flat = 0, n_general = 0, n_slab_fast = 0;
+  uint32_t n_flat = 0, n_general = 0;
   uint32_t n_uncopied = 0;             // items with a page that has no flat-store copy
   uint32_t bitmap_words = 0;
   std::vector<uint32_t> max_bw, flat_max_bw;          // per slot
@@ -226,15 +226,7 @@ class Table {
   uint8_t* d_arena = nullptr;
   uint64_t arena_bytes = 0;
   DevPage* d_pages = nullptr;
-  // slab index (k_slab_index): per page, per kSlabRows rows, the run directory and window start the
-  // scan kernel would otherwise derive by walking the run headers; see DESIGN.md
-  DevSlabRec* d_slab_recs = nullptr;
-  DirEntry* d_slab_dirs = nullptr;
   uint8_t* d_strmat = nullptr;            // DELTA_BYTE_ARRAY pages rewritten as PLAIN BYTE_ARRAY pages (outside the arena: DevPage.off wraps)
-  uint8_t* d_slab_flat = nullptr;         // flat bit-packed copies of run-heavy pages (k_flatten_pages)
-  uint64_t slab_flat_bytes = 0;
-  uint64_t total_slabs = 0;
-  std::vector<uint32_t> col_valwin_cap;   // per table column: staged window bytes the index was built for
   uint64_t total_rows = 0;
   uint64_t h2d_bytes = 0;
   uint64_t chunk_bytes = 0;
@@ -247,7 +239,6 @@ class Table {
   mutable std::vector<FlatPageRec> flat_pages;   // host copy, parallel to pages (ensure_plain8 adds entries later)
   mutable FlatPageRec* d_flat_pages = nullptr;
   uint64_t flat_page_count = 0;
-  bool nulls_classified = false;         // build_flat_store looked at every page's definition levels (voff == ~0 then means: no NULLs)
 
   // lazily built, query independent (the table is immutable once opened); guarded by side_mu
   mutable std::mutex side_mu;
@@ -280,13 +271,6 @@ class Table {
   void build_flat_store(cudaStream_t stream);
 };
 
-// staged window bytes for one slab of a dictionary-index stream of the given bit width
-inline uint32_t valwin_cap_for_bw(uint32_t max_bw) { return ((kSlabRows * max_bw / 8 + kSlabRows / 8 + 64) + 15u) & ~15u; }
-// launches k_slab_index (defined next to k_scan, query.cu)
-void launch_slab_index(const uint8_t* arena, const DevPage* pages, uint32_t n_pages, const uint32_t* col_caps, DevSlabRec* recs,
-                       DirEntry* dirs, uint8_t* page_fast, cudaStream_t stream);
-void launch_flatten_pages(const uint8_t* arena, const DevPage* pages, const void* jobs, uint32_t n_jobs, uint8_t* side,
-                          DevSlabRec* recs, DirEntry* dirs, uint8_t* page_fast, cudaStream_t stream);
 // launches k_flat_store (flat_store.cuh); jobs are FlatStoreJob records on the device
 void launch_flat_store(const uint8_t* arena, const DevPage* pages, const void* jobs, uint32_t n_jobs, uint8_t* flat, uint8_t* ok,
                        uint32_t* maxlen, cudaStream_t stream);

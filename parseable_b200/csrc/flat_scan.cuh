@@ -4,8 +4,7 @@
 // (/root/reference/src/query/mod.rs:287; SURVEY.md §8 rows a10-a12), for the common case: every
 // referenced column of a work item has pages with a flat copy (pages with NULLs carry a validity
 // bitmap and one slot per ROW; a column missing from a file reads as all NULL).  A file whose value
-// streams the flattener refuses is refused as corrupt at table open (PQB_FLAT_LENIENT keeps such
-// pages on k_scan for debugging).
+// streams the flattener refuses is refused as corrupt at table open.
 //
 // Shape (both kernels): persistent CTAs, one PRODUCER warp and N consumer warps.  The producer's
 // elected lane pulls work items from the queue, and for every slab of an item stages the slab's

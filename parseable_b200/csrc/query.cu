@@ -241,20 +241,6 @@ Query::~Query() {
     if (b && b->dev) { cudaFree(b->dev); b->dev = nullptr; }
 }
 
-void launch_slab_index(const uint8_t* arena, const DevPage* pages, uint32_t n_pages, const uint32_t* col_caps, DevSlabRec* recs,
-                       DirEntry* dirs, uint8_t* page_fast, cudaStream_t stream) {
-  if (!n_pages) return;
-  k_slab_index<<<(n_pages + 63) / 64, 64, 0, stream>>>(arena, pages, n_pages, col_caps, recs, dirs, page_fast);
-  PQB_CUDA(cudaGetLastError());
-}
-
-void launch_flatten_pages(const uint8_t* arena, const DevPage* pages, const void* jobs, uint32_t n_jobs, uint8_t* side,
-                          DevSlabRec* recs, DirEntry* dirs, uint8_t* page_fast, cudaStream_t stream) {
-  if (!n_jobs) return;
-  k_flatten_pages<<<(n_jobs + 31) / 32, 32, 0, stream>>>(arena, pages, static_cast<const FlatJob*>(jobs), n_jobs, side, recs, dirs, page_fast);
-  PQB_CUDA(cudaGetLastError());
-}
-
 void launch_flat_store(const uint8_t* arena, const DevPage* pages, const void* jobs, uint32_t n_jobs, uint8_t* flat, uint8_t* ok,
                        uint32_t* maxlen, cudaStream_t stream) {
   if (!n_jobs) return;
@@ -1409,7 +1395,7 @@ void Query::run(const PqQueryDesc& d) {
     plan.row_major = rm && rm[0] == '1';
   }
   {
-    // k_scan: conjunction of 1-4 CMP/LIKE leaves: specialised octet pass over slab-indexed pages
+    // k_scan: conjunction of 1-4 CMP/LIKE leaves: specialised octet pass over no-NULL dictionary slabs
     bool c4 = conj && nleaves >= 1 && nleaves <= 4;
     for (uint32_t l = 0; l < nleaves; l++) c4 &= value_leaf(plan.leaves[l].kind);
     const char* fa = getenv("PQB_FAST_AND");
@@ -1927,7 +1913,6 @@ void Query::run(const PqQueryDesc& d) {
   plan.no_flat = flat_ok ? 0 : 1;
   const uint32_t n_flat = flat_ok ? shape->n_flat : 0;
   const uint32_t n_general = flat_ok ? shape->n_general : uint32_t(items.size());
-  const uint32_t n_fast_items = shape->n_slab_fast;
 
   for (uint32_t k = 0; agg_kernel && k < d.n_group_by; k++)
     if (plan.keys[k].kind == KK_BIN && n_general)
@@ -2053,8 +2038,6 @@ void Query::run(const PqQueryDesc& d) {
       // anything denser makes the kernel shrink the slab (always correct, only slower)
       L.defwin_cap[s] = plan.cols[s].max_def ? align_up(kSlabRows / 8 + kSlabRows / 16 + 64, 16) : 0;
       L.valwin_cap[s] = plan.cols[s].has_dict ? valwin_cap_for_bw(plan.cols[s].max_bw) : 0;
-      // the slab index holds window-relative bit offsets: stage at least the window it was built for
-      if (n_fast_items && plan.cols[s].has_dict) L.valwin_cap[s] = std::max(L.valwin_cap[s], table->col_valwin_cap[shape_cols[s]]);
       if (plan.cols[s].has_delta) L.valwin_cap[s] = std::max<uint32_t>(L.valwin_cap[s], align_up(kDeltaWindowBytes, 16));
       for (int b = 0; b < 2; b++) { L.defwin[s][b] = off; off += align_up(L.defwin_cap[s] + 16, 128); }
       for (int b = 0; b < 2; b++) { L.valwin[s][b] = off; off += align_up(L.valwin_cap[s] + 16, 128); }
@@ -2064,14 +2047,13 @@ void Query::run(const PqQueryDesc& d) {
       L.idx[s] = (plan.cols[s].has_dict || plan.cols[s].has_delta) ? off : 0;
       off += plan.cols[s].has_delta ? kSlabRows * 8 : (plan.cols[s].has_dict ? kSlabRows * 4 : 0);
       L.defdir[s] = off; off += kMaxDirEntries * sizeof(DirEntry);
-      for (int b = 0; b < 2; b++) {   // bulk-copy destination for prebuilt directories: 16-byte aligned
+      for (int b = 0; b < 2; b++) {   // DirEntry / DeltaEntry records (DeltaEntry holds an int64): 16-byte aligned
         off = align_up(off, 16);
         L.valdir[s][b] = off;
         off += std::max<uint32_t>(kMaxDirEntries * sizeof(DirEntry), plan.cols[s].has_delta ? kMaxDeltaEntries * sizeof(DeltaEntry) : 0);
       }
     }
     off = align_up(off, 16);
-    L.recs = off; off += uint32_t(kRecBatch * std::max<uint32_t>(ncols, 1) * sizeof(DevSlabRec));
     L.leafT = off; off += std::max<uint32_t>(nleaves, 1) * kLeafWords * 4;
     L.sel = off; off += kSlabWords * 4;
     L.lutc = off; if (plan.fast_and) off += nleaves * kLutCacheBytes;
@@ -2273,8 +2255,6 @@ void Query::run(const PqQueryDesc& d) {
   sa.acc = d_acc.p;
   sa.hkeys = d_hkeys.p;
   sa.counters = d_counters.p;
-  sa.slab_recs = table->d_slab_recs;
-  sa.slab_dirs = table->d_slab_dirs;
   PQB_CUDA(cudaEventRecord(t_scan.a, stream));
   if (n_flat && nrg) {
     uint32_t grid;
@@ -2347,8 +2327,8 @@ void Query::run(const PqQueryDesc& d) {
     uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * occ));
     if (const char* g = getenv("PQB_GRID")) grid = std::max(1, atoi(g));   // debugging aid: forces several items per CTA
     if (verbose)
-      fprintf(stderr, "[pqb] k_scan: %u CTAs x %d threads, %zu B smem/CTA, %d CTAs/SM, %u of %zu items (%u slab-indexed)\n", grid,
-              kScanThreads, size_t(smem_total), occ, n_general, items.size(), n_fast_items);
+      fprintf(stderr, "[pqb] k_scan: %u CTAs x %d threads, %zu B smem/CTA, %d CTAs/SM, %u of %zu items\n", grid,
+              kScanThreads, size_t(smem_total), occ, n_general, items.size());
     k_scan<<<grid, kScanThreads, smem_total, stream>>>(plan, L, sa);
     PQB_CUDA(cudaGetLastError());
     launches++;

@@ -55,7 +55,6 @@ struct SmemLayout {
   uint32_t leafT;             // uint32[nleaves][kSlabWords + 2]
   uint32_t sel;               // uint32[kSlabWords]
   uint32_t acc;               // shared accumulator table
-  uint32_t recs;              // DevSlabRec[kRecBatch][ncols]: slab records of the current fast item
   uint32_t lutc;              // uint8[nleaves][kLutCacheBytes]: leaf LUTs of the current row group (fast AND path)
   uint32_t total;
 };
@@ -114,8 +113,7 @@ struct ScanCtl {
   uint32_t stk[kScanWarps][2 * kPredStack]; // fast row pass: per warp Kleene stack (t, n) words
   uint32_t lut_smem[kMaxLeaves];            // fast AND path: leaf LUT of this item's row group is cached in smem
   ColCursor cur[kMaxCols];
-  SlabCol slab[2][kMaxCols];                // per staging buffer: warps of a barrier-free item may be one slab apart
-  uint64_t empty[2];                        // rows -> producer: every warp is done with the buffer
+  SlabCol slab[2][kMaxCols];                // per staging buffer
   int64_t dl_last[kMaxCols];                // DELTA pages: value of the last row decoded so far in the page (carried across slabs)
 };
 
@@ -914,165 +912,6 @@ __device__ __forceinline__ void fill_lut_cache(const DevPlan& plan, ScanCtl& ctl
   }
 }
 
-// one thread: publish the per-slab view of batch slab k in buffer `buf` (rows_left = rows of the
-// item from this slab on)
-__device__ __forceinline__ void fast_view(ScanCtl& ctl, const DevSlabRec* recs, uint32_t k, uint32_t ncols, uint32_t buf,
-                                          uint32_t rows_left) {
-  const uint32_t R = rows_left < (uint32_t)kSlabRows ? rows_left : (uint32_t)kSlabRows;
-  for (uint32_t c = 0; c < ncols; c++) {
-    const DevSlabRec& rc = recs[k * ncols + c];
-    SlabCol& s = ctl.slab[buf][c];
-    s.val_base = rc.val_base;
-    s.vals_done = rc.vals_done;
-    s.enc = rc.enc;
-    s.bw = rc.bw;
-    s.nval = rc.nent;
-    s.nv = s.present ? R : 0;
-  }
-}
-
-// thread 0: stage slab k0 + k of a fast item (its records sit in shared memory) into buffer `buf`:
-// the value windows and the indexed run directories, one mbarrier transaction
-__device__ __forceinline__ void fast_issue(ScanCtl& ctl, const SmemLayout& L, uint8_t* smem, const DevScanArgs& a,
-                                           const DevSlabRec* recs, uint32_t k0, uint32_t k, uint32_t ncols, uint32_t buf) {
-  uint32_t bytes = 0;
-  for (uint32_t c = 0; c < ncols; c++) {
-    const DevSlabRec& rc = recs[k * ncols + c];
-    if (PQB_ENC_HAS_STREAM(rc.enc) && rc.nent) bytes += L.valwin_cap[c] + (uint32_t(rc.nent) + 2u) * uint32_t(sizeof(DirEntry));
-  }
-  mbar_arrive_expect_tx(&ctl.mbar[buf], bytes);
-  for (uint32_t c = 0; c < ncols; c++) {
-    const DevSlabRec& rc = recs[k * ncols + c];
-    if (!(PQB_ENC_HAS_STREAM(rc.enc) && rc.nent)) continue;
-    tma_load_1d(smem + L.valwin[c][buf], a.arena + rc.win_off, L.valwin_cap[c], &ctl.mbar[buf]);
-    tma_load_1d(smem + L.valdir[c][buf], a.slab_dirs + rc.ent0,
-                (uint32_t(rc.nent) + 2u) * uint32_t(sizeof(DirEntry)), &ctl.mbar[buf]);
-  }
-}
-
-// ---- slab index ----------------------------------------------------------------------------------
-// The run headers of an RLE / bit-packed hybrid stream can only be walked sequentially, and inside
-// k_scan that walk sat on the critical path of every slab (one lane busy, 255 waiting: 40 % of all
-// stall samples in profiles/k_scan_r1c).  But every page's stream is independent of every other, so
-// this kernel — run once, when the table is opened — walks them all at the same time, one thread
-// per page, reading the few header bytes straight from HBM/L2, and leaves for every slab of
-// kSlabRows rows exactly what the in-kernel control would have built: the window start, the run
-// directory (window-relative bit offsets) and the page cursor.  Pages it cannot cover (NULLs in the
-// definition levels, DELTA pages, more runs per slab than kFastDirEntries, a window that does not
-// hold a whole slab) stay on the in-kernel path (page_fast = 0).
-__global__ void k_slab_index(const uint8_t* __restrict__ arena, const DevPage* __restrict__ pages, uint32_t n_pages,
-                             const uint32_t* __restrict__ col_caps, DevSlabRec* __restrict__ slab_recs,
-                             DirEntry* __restrict__ slab_dirs, uint8_t* __restrict__ page_fast) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_pages) return;
-  ColCursor cur;
-  page_enter(cur, pages, i);
-  const DevPage& pg = pages[i];
-  const uint32_t cap = col_caps[pg.chunk_slot];
-  page_fast[i] = 2;   // 1: indexed; otherwise why not (2 DELTA page, 3 NULLs / bit-packed definition levels, 4 runs or window overflow)
-  if (cur.enc == DE_DELTA) return;
-  uint32_t rows_left = pg.num_rows;
-  const uint32_t nslabs = (pg.num_rows + kSlabRows - 1) / kSlabRows;
-  DevSlabRec rec{};
-  // the page's slabs share one entry budget: a slab with many short runs borrows from its neighbours
-  const uint32_t ent_base = pg.slab0 * kFastDirEntries, budget = nslabs * kFastDirEntries;
-  uint32_t used = 0;
-  bool flat = false;
-  for (uint32_t k = 0; k < nslabs; k++) {
-    const uint32_t R = rows_left < (uint32_t)kSlabRows ? rows_left : (uint32_t)kSlabRows;
-    if (cur.has_def) {  // every definition level of the slab must be 1 (RLE runs of 1s)
-      const uint64_t base = stream_window_start(cur.def) & ~15ull;
-      const Window w{arena + base, base, uint32_t(cur.def.end - base)};
-      uint32_t covered = 0;
-      bool ok = true;
-      while (covered < R && ok) {
-        DirEntry tmp[4];
-        uint32_t n = 0;
-        const uint32_t got = walk_stream(cur.def, w, R - covered, tmp, n, 4);
-        for (uint32_t e = 0; e < n; e++) ok = ok && tmp[e].kind == 0 && (tmp[e].payload & 1);
-        ok = ok && got != 0;
-        covered += got;
-      }
-      if (!ok) { page_fast[i] = 3; return; }
-    }
-    rec.win_off = 0;
-    rec.nent = 0;
-    rec.bw = 0;
-    if (PQB_ENC_HAS_STREAM(cur.enc) && !flat) {
-      const uint64_t base = stream_window_start(cur.val) & ~15ull;
-      const Window w{arena + base, base, cap};
-      uint32_t n = 0, got = 0;
-      if (used + 3 <= budget) {
-        DirEntry* out = slab_dirs + ent_base + used;
-        const uint32_t room = budget - used - 2;
-        got = walk_stream(cur.val, w, R, out, n, room < uint32_t(kMaxDirEntries - 2) ? room : uint32_t(kMaxDirEntries - 2));
-        if (got == R && n) dir_sentinels(out, n);
-      }
-      if (got < R || n == 0) {
-        // too many runs for the page's entry budget (or for one staged window): the page gets a
-        // flat bit-packed copy instead (k_flatten_pages); keep checking the definition levels only
-        flat = true;
-      } else {
-        rec.ent0 = ent_base + used;
-        used += n + 2;
-        rec.win_off = base;
-        rec.nent = uint16_t(n);
-        rec.bw = cur.val.bw;
-      }
-    }
-    rec.val_base = cur.val_base;
-    rec.vals_done = cur.vals_done;
-    rec.enc = uint8_t(cur.enc);
-    slab_recs[pg.slab0 + k] = rec;
-    cur.vals_done += R;
-    rows_left -= R;
-  }
-  page_fast[i] = flat ? 5 : 1;
-}
-
-// Second pass of the slab index: pages whose run structure does not fit a directory get a flat
-// bit-packed copy of their index stream (decode_core.cuh transcode_values) in a side buffer; every
-// slab of such a page is then a single bit-packed directory entry at a 256 * bw byte stride.
-__global__ void k_flatten_pages(const uint8_t* __restrict__ arena, const DevPage* __restrict__ pages, const FlatJob* __restrict__ jobs,
-                                uint32_t n_jobs, uint8_t* __restrict__ side, DevSlabRec* __restrict__ slab_recs,
-                                DirEntry* __restrict__ slab_dirs, uint8_t* __restrict__ page_fast) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_jobs) return;
-  const uint32_t pi = jobs[i].page;
-  ColCursor cur;
-  page_enter(cur, pages, pi);
-  const DevPage& pg = pages[pi];
-  const uint32_t bw = cur.val.bw;
-  uint8_t* dst = side + jobs[i].side_off;
-  BitWriter b{reinterpret_cast<uint32_t*>(dst), 0, 0};
-  uint32_t rows_left = pg.num_rows;
-  const uint32_t nslabs = (pg.num_rows + kSlabRows - 1) / kSlabRows;
-  DevSlabRec rec{};
-  for (uint32_t k = 0; k < nslabs; k++) {
-    const uint32_t R = rows_left < (uint32_t)kSlabRows ? rows_left : (uint32_t)kSlabRows;
-    if (transcode_values(cur.val, arena, R, b) < R) { page_fast[pi] = 4; return; }
-    DirEntry* out = slab_dirs + size_t(pg.slab0) * kFastDirEntries + 3 * k;
-    out[0].start = 0;
-    out[0].count = uint16_t(R);
-    out[0].kind = bw ? 1 : 0;   // a one-entry dictionary has no bits at all: one RLE run of index 0
-    out[0].chunk0 = 0;
-    out[0].payload = 0;
-    out[0]._pad = 0;
-    dir_sentinels(out, 1);
-    rec.win_off = uint64_t(dst + size_t(k) * (kSlabRows / 8) * bw) - uint64_t(arena);   // relative to the arena, may wrap
-    rec.val_base = cur.val_base;
-    rec.vals_done = k * kSlabRows;
-    rec.nent = 1;
-    rec.enc = uint8_t(cur.enc);
-    rec.bw = uint8_t(bw);
-    rec.ent0 = pg.slab0 * kFastDirEntries + 3 * k;
-    slab_recs[pg.slab0 + k] = rec;
-    rows_left -= R;
-  }
-  bitwriter_flush(b);
-  page_fast[pi] = 1;
-}
-
 // ---- the row phase of one slab: DELTA decode, then the row pass the slab qualifies for; adds the
 // selected rows to ctl.sel_count.  All threads of the CTA call it. ----
 __device__ __forceinline__ void row_phase(const DevPlan& plan, ScanCtl& ctl, const SmemLayout& L, uint8_t* smem, const DevScanArgs& a,
@@ -1265,8 +1104,6 @@ k_scan(const __grid_constant__ DevPlan plan, const __grid_constant__ SmemLayout 
   if (tid == 0) {
     mbar_init(&ctl.mbar[0], 1);
     mbar_init(&ctl.mbar[1], 1);
-    mbar_init(&ctl.empty[0], kScanWarps);
-    mbar_init(&ctl.empty[1], kScanWarps);
     mbar_fence_init();
     ctl.error = 0;
   }
@@ -1287,7 +1124,6 @@ k_scan(const __grid_constant__ DevPlan plan, const __grid_constant__ SmemLayout 
   const uint32_t nslots = plan.nslots;
 
   uint32_t phases = 0;   // bit b: parity to wait for on mbar[b]
-  uint32_t ephases = 0;  // bit b: parity of the next completion of empty[b]
 
   for (;;) {
     __syncthreads();
@@ -1298,126 +1134,6 @@ k_scan(const __grid_constant__ DevPlan plan, const __grid_constant__ SmemLayout 
     const DevItem& item = a.items[item_id];
     if ((item.fast & kItemFlat) && !plan.no_flat) continue;   // the flat kernels own this item
     if (a.rg_live && !a.rg_live[item.rg]) continue;            // row group pruned by statistics (counts stay 0)
-
-    if (item.fast & kItemSlabIndexed) {
-      // ---------------- fast item: the table's slab index holds every slab's run directory ----------------
-      // no header walk, no cursor: per slab one wait for the staged bytes, the row phase, and the
-      // bulk copies of the slab after next
-      if (tid < ncols) {
-        const DevChunk ch = a.chunks[item.rg * ncols + tid];
-        for (uint32_t b = 0; b < 2; b++) {
-          SlabCol& s = ctl.slab[b][tid];
-          s.lut_base = ch.lut_base;
-          s.dict_off = ch.dict_off;
-          s.present = ch.present;
-          s.ndef = 0;
-          s.all_valid = 1;
-        }
-      }
-      if (tid == 0) ctl.sel_count = 0;
-      fill_lut_cache(plan, ctl, L, smem, a, item.rg);
-      DevSlabRec* recs = smem_at<DevSlabRec>(smem, L.recs);
-      const uint32_t nslabs = (item.nrows + kSlabRows - 1) / kSlabRows;
-      uint32_t r_item = 0;
-      for (uint32_t k0 = 0; k0 < nslabs; k0 += kRecBatch) {
-        const uint32_t nb = nslabs - k0 < (uint32_t)kRecBatch ? nslabs - k0 : (uint32_t)kRecBatch;
-        // this batch's slab records -> shared memory, one thread per (slab, column); the first batch
-        // runs in the same phase as the item setup above, so every thread looks up its page itself
-        for (uint32_t i = tid; i < nb * ncols; i += kScanThreads) {
-          const uint32_t k = i / ncols, c = i % ncols;
-          DevSlabRec rc{};
-          rc.enc = DE_PLAIN;
-          if (a.chunks[item.rg * ncols + c].present) rc = a.slab_recs[a.pages[item.page[c]].slab0 + k0 + k];
-          recs[i] = rc;
-        }
-        __syncthreads();
-        // can every slab of the batch take the conjunction pass?  Then the warps need no block
-        // barrier at all: each waits for the staged bytes itself and hands the buffer back through
-        // an mbarrier, so a slow warp (short runs, many survivors) no longer stalls the other seven
-        bool conj = plan.fast_and != 0;
-        if (conj && tid < nb)
-          for (uint32_t l = 0; conj && l < plan.nleaves; l++) {
-            const uint32_t c = plan.leaves[l].col;
-            const DevSlabRec& rc = recs[tid * ncols + c];
-            conj = ctl.slab[0][c].present && rc.enc == DE_DICT && rc.nent > 0;
-          }
-        if (__syncthreads_and(conj)) {
-          const uint32_t row00 = r_item;
-          uint32_t cnt_batch = 0;   // selected rows of this thread's octets over the whole batch
-          if (tid == 0) {
-            for (uint32_t k = 0; k < 2 && k < nb; k++) {
-              fast_view(ctl, recs, k, ncols, k, item.nrows - row00 - k * kSlabRows);
-              fast_issue(ctl, L, smem, a, recs, k0, k, ncols, k);
-            }
-          }
-          for (uint32_t k = 0; k < nb; k++) {
-            const uint32_t buf = k & 1u;
-            const uint32_t R = item.nrows - r_item < (uint32_t)kSlabRows ? item.nrows - r_item : (uint32_t)kSlabRows;
-            if (lane_id() == 0) mbar_wait(&ctl.mbar[buf], (phases >> buf) & 1u);
-            __syncwarp();
-            phases ^= 1u << buf;
-            cnt_batch += fast_and_rows(plan, ctl, L, smem, a, item, buf, R, r_item, acc, agg_mode);
-            __syncwarp();
-            if (lane_id() == 0) mbar_arrive(&ctl.empty[buf]);   // this warp is done with buffer `buf`
-            const uint32_t epar = (ephases >> buf) & 1u;
-            ephases ^= 1u << buf;
-            r_item += R;
-            if (tid == 0 && k + 2 < nb) {   // refill the buffer once all eight warps let go of it
-              mbar_wait(&ctl.empty[buf], epar);
-              fast_view(ctl, recs, k + 2, ncols, buf, item.nrows - row00 - (k + 2) * kSlabRows);
-              fast_issue(ctl, L, smem, a, recs, k0, k + 2, ncols, buf);
-            }
-            __syncwarp();
-          }
-          for (int o = 16; o; o >>= 1) cnt_batch += __shfl_xor_sync(0xffffffffu, cnt_batch, o);
-          if (lane_id() == 0 && cnt_batch) atomicAdd(&ctl.sel_count, cnt_batch);
-          __syncthreads();
-          continue;
-        }
-        if (tid == 0) {
-          fast_issue(ctl, L, smem, a, recs, k0, 0, ncols, 0);
-          if (nb > 1) fast_issue(ctl, L, smem, a, recs, k0, 1, ncols, 1);
-        }
-        for (uint32_t k = 0; k < nb; k++) {
-          const uint32_t buf = k & 1u;
-          const uint32_t R = item.nrows - r_item < (uint32_t)kSlabRows ? item.nrows - r_item : (uint32_t)kSlabRows;
-          if (tid < ncols) {
-            const DevSlabRec& rc = recs[k * ncols + tid];
-            SlabCol& s = ctl.slab[buf][tid];
-            s.val_base = rc.val_base;
-            s.vals_done = rc.vals_done;
-            s.enc = rc.enc;
-            s.bw = rc.bw;
-            s.nval = rc.nent;
-            s.nv = s.present ? R : 0;
-          }
-          if (tid == 0) {
-            uint32_t mode = MODE_GENERIC;
-            bool fa = plan.fast_and != 0;
-            for (uint32_t l = 0; fa && l < plan.nleaves; l++) {
-              const uint32_t c = plan.leaves[l].col;
-              const DevSlabRec& rc = recs[k * ncols + c];
-              fa = ctl.slab[buf][c].present && rc.enc == DE_DICT && rc.nent > 0;
-            }
-            if (fa) mode = MODE_FAST_AND;
-            else if (plan.row_major) mode = MODE_ROW_MAJOR;
-            ctl.mode = mode;
-            mbar_wait(&ctl.mbar[buf], (phases >> buf) & 1u);
-          }
-          phases ^= 1u << buf;
-          __syncthreads();
-          row_phase(plan, ctl, L, smem, a, item, ctl.mode, 0, buf, R, r_item, acc, agg_mode);
-          r_item += R;
-          __syncthreads();
-          if (tid == 0 && k + 2 < nb) fast_issue(ctl, L, smem, a, recs, k0, k + 2, ncols, buf);
-        }
-      }
-      if (tid == 0) {
-        if (a.item_counts) a.item_counts[item_id] = ctl.sel_count;
-        if (ctl.sel_count) atomicAdd(&a.counters[0], (unsigned long long)ctl.sel_count);
-      }
-      continue;
-    }
 
     if (tid < ncols) {
       ColCursor& c = ctl.cur[tid];

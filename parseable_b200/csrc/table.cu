@@ -261,9 +261,6 @@ Table::~Table() {
   // stream-ordered frees into the pool: a per-query table costs no device-wide synchronisation
   if (d_arena) cudaFreeAsync(d_arena, cudaStreamPerThread);
   if (d_pages) cudaFreeAsync(d_pages, cudaStreamPerThread);
-  if (d_slab_recs) cudaFreeAsync(d_slab_recs, cudaStreamPerThread);
-  if (d_slab_dirs) cudaFreeAsync(d_slab_dirs, cudaStreamPerThread);
-  if (d_slab_flat) cudaFreeAsync(d_slab_flat, cudaStreamPerThread);
   if (d_strmat) cudaFreeAsync(d_strmat, cudaStreamPerThread);
   if (d_flat) cudaFreeAsync(d_flat, cudaStreamPerThread);
   if (d_flat_pages) cudaFreeAsync(d_flat_pages, cudaStreamPerThread);
@@ -799,15 +796,9 @@ void Table::open(const PqFile* in_files, uint32_t n_files, const std::vector<std
       TableChunk& tc = row_groups[jobs[j].rg].chunks[jobs[j].col];
       tc.pages.first_page = uint32_t(pages.size());
       tc.pages.n_pages = uint32_t(out[j].size());
-      for (DevPage& dp : out[j]) {
-        dp.chunk_slot = uint16_t(jobs[j].col);
-        dp.slab0 = uint32_t(total_slabs);
-        dp.flags = 0;
-        total_slabs += (dp.num_rows + kSlabRows - 1) / kSlabRows;
-      }
+      for (DevPage& dp : out[j]) dp.chunk_slot = uint16_t(jobs[j].col);
       pages.insert(pages.end(), out[j].begin(), out[j].end());
     }
-    if (total_slabs > 0xfffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "too many slabs for one table");
   }
   mark("page headers walked");
   if (!pages.empty()) {
@@ -921,60 +912,6 @@ void Table::open(const PqFile* in_files, uint32_t n_files, const std::vector<std
     }
     rg.pages_aligned = same && first != nullptr;
   }
-  // ---- slab index: every page's run headers walked once, all pages at the same time ----
-  col_valwin_cap.assign(columns.size(), 0);
-  for (const TableRowGroup& rg : row_groups)
-    for (size_t c = 0; c < rg.chunks.size(); c++)
-      if (rg.chunks[c].present && rg.chunks[c].has_dict_pages)
-        col_valwin_cap[c] = std::max(col_valwin_cap[c], valwin_cap_for_bw(rg.chunks[c].max_bw));
-  // The slab index was round 1's fast path (run directories per 2048 rows for k_scan).  Every page it
-  // can cover now has a flat-store copy and goes to the flat kernels, so it is only built on request
-  // (PQB_SLAB_INDEX=1: the A/B of DESIGN.md §4).
-  const bool want_index = getenv("PQB_SLAB_INDEX") && getenv("PQB_SLAB_INDEX")[0] == '1';
-  if (want_index && !pages.empty() && !columns.empty()) {
-    uint32_t* d_caps = nullptr;
-    uint8_t* d_fast = nullptr;
-    PQB_CUDA(cudaMallocAsync((void**)&d_caps, col_valwin_cap.size() * 4, stream));
-    PQB_CUDA(cudaMemcpyAsync(d_caps, col_valwin_cap.data(), col_valwin_cap.size() * 4, cudaMemcpyHostToDevice, stream));
-    PQB_CUDA(cudaMallocAsync((void**)&d_fast, pages.size(), stream));
-    PQB_CUDA(cudaMallocAsync((void**)&d_slab_recs, std::max<uint64_t>(total_slabs, 1) * sizeof(DevSlabRec), stream));
-    PQB_CUDA(cudaMallocAsync((void**)&d_slab_dirs, std::max<uint64_t>(total_slabs, 1) * kFastDirEntries * sizeof(DirEntry), stream));
-    launch_slab_index(d_arena, d_pages, uint32_t(pages.size()), d_caps, d_slab_recs, d_slab_dirs, d_fast, stream);
-    std::vector<uint8_t> fast(pages.size());
-    PQB_CUDA(cudaMemcpyAsync(fast.data(), d_fast, fast.size(), cudaMemcpyDeviceToHost, stream));
-    PQB_CUDA(cudaStreamSynchronize(stream));
-    // run-heavy pages (skewed low-cardinality columns): a flat bit-packed copy replaces the directory
-    std::vector<FlatJob> fjobs;
-    uint64_t side = 0;
-    for (size_t i = 0; i < pages.size(); i++)
-      if (fast[i] == 5) {
-        fjobs.push_back({uint32_t(i), 0, side});
-        side += ((uint64_t(pages[i].num_rows) * pages[i].bit_width + 31) / 32 * 4 + 255 + 256) & ~255ull;
-      }
-    if (!fjobs.empty()) {
-      uint32_t max_cap = 0;
-      for (uint32_t c : col_valwin_cap) max_cap = std::max(max_cap, c);
-      slab_flat_bytes = side + max_cap + 256;   // staged windows over-read past the last slab
-      void* d_jobs = nullptr;
-      PQB_CUDA(cudaMallocAsync((void**)&d_slab_flat, slab_flat_bytes, stream));
-      PQB_CUDA(cudaMemsetAsync(d_slab_flat + side, 0, slab_flat_bytes - side, stream));
-      PQB_CUDA(cudaMallocAsync(&d_jobs, fjobs.size() * sizeof(FlatJob), stream));
-      PQB_CUDA(cudaMemcpyAsync(d_jobs, fjobs.data(), fjobs.size() * sizeof(FlatJob), cudaMemcpyHostToDevice, stream));
-      launch_flatten_pages(d_arena, d_pages, d_jobs, uint32_t(fjobs.size()), d_slab_flat, d_slab_recs, d_slab_dirs, d_fast, stream);
-      PQB_CUDA(cudaMemcpyAsync(fast.data(), d_fast, fast.size(), cudaMemcpyDeviceToHost, stream));
-      PQB_CUDA(cudaStreamSynchronize(stream));
-      dev_drop(d_jobs, stream);
-    }
-    dev_drop(d_caps, stream);
-    dev_drop(d_fast, stream);
-    for (size_t i = 0; i < pages.size(); i++) pages[i].flags = fast[i] == 1 ? 1u : 0u;
-    if (getenv("PQB_VERBOSE")) {
-      size_t h[5] = {0, 0, 0, 0, 0};
-      for (uint8_t f : fast) h[f < 5 ? f : 0]++;
-      fprintf(stderr, "[pqb] slab index: %zu pages indexed (%zu of them as flat bit-packed copies, %llu bytes), not indexed: %zu DELTA, %zu NULLs, %zu corrupt; %llu slabs\n",
-              h[1], fjobs.size(), (unsigned long long)slab_flat_bytes, h[2], h[3], h[4], (unsigned long long)total_slabs);
-    }
-  }
   // ---- per-column entry numbering (query independent): entries of the column in earlier row groups ----
   sides.assign(columns.size(), ColSide{});
   for (size_t c = 0; c < columns.size(); c++) {
@@ -1000,8 +937,7 @@ void Table::build_flat_store(cudaStream_t stream) {
   FlatPageRec blank{};
   blank.voff = ~0ull;
   flat_pages.assign(pages.size(), blank);
-  const char* sw = getenv("PQB_FLAT");
-  if ((sw && sw[0] == '0') || pages.empty()) return;   // A/B switch: everything through k_scan
+  if (pages.empty()) return;
   // which pages hold NULLs (their definition levels are not all 1)?
   // A chunk whose footer promises null_count == 0 (or whose column cannot hold NULLs: no definition levels) needs no
   // look at the data: when that settles every page, nothing below waits for the upload -- the jobs are built and the
@@ -1013,7 +949,6 @@ void Table::build_flat_store(cudaStream_t stream) {
     for (const TableChunk& tc : rg.chunks)
       if (tc.present && tc.meta->stats.null_count != 0)
         for (uint32_t k = 0; k < tc.pages.n_pages && !need_look; k++) need_look = pages[tc.pages.first_page + k].def_len != 0;
-  nulls_classified = true;
   if (need_look) {
     uint8_t* d_nf = nullptr;
     PQB_CUDA(cudaMallocAsync((void**)&d_nf, pages.size(), stream));
@@ -1131,11 +1066,9 @@ void Table::build_flat_store(cudaStream_t stream) {
       cs.max_plain_len = std::max(cs.max_plain_len, maxlen[i]);
     }
   size_t n_ok = 0, n_nul = 0;
-  const bool lenient = getenv("PQB_FLAT_LENIENT") != nullptr;   // debugging: keep a refused page on the k_scan path instead of failing the file
   for (size_t i = 0; i < dj.size(); i++) {
     if (dj[i].kind == 4u) continue;
     if (ok[i]) { n_ok += dj[i].kind != 5u; n_nul += dj[i].vdst != kNone; }
-    else if (lenient) { flat_pages[dj[i].page].fkind = FK_NONE; flat_pages[dj[i].page].voff = kNone; }
     else {
       // a run header past the page, a length prefix past the page, a stream that stops early: the reference's reader fails such a file
       const DevPage& pg = pages[dj[i].page];
@@ -1193,7 +1126,6 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
   std::vector<DevChunk> chunks(size_t(nrg) * std::max<uint32_t>(ncols, 1));
   std::vector<std::vector<uint32_t>> bounds;
   std::vector<uint32_t> common;
-  const bool use_slab_index = ncols > 0 && d_slab_recs != nullptr;
   const bool use_flat = d_flat_pages != nullptr || ncols == 0;
   sh->items.reserve(size_t(nrg) * 16);
   for (uint32_t g = 0; g < nrg; g++) {
@@ -1250,7 +1182,7 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
       }
       return tc.pages.first_page + lo;
     };
-    auto push_item = [&](DevItem& it, bool flat, bool fast) {
+    auto push_item = [&](DevItem& it, bool flat) {
       it.bitmap_word0 = sh->bitmap_words;
       sh->bitmap_words += (it.nrows + 31) / 32 + 1;
       if (flat)
@@ -1261,9 +1193,8 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
           else sh->flat_max_bw[s] = std::max<uint32_t>(sh->flat_max_bw[s], fr.bw);
           if (fr.voff != ~0ull) sh->flat_nullable[s] = 1;
         }
-      it.fast = (flat ? kItemFlat : (fast ? kItemSlabIndexed : 0u));
+      it.fast = flat ? kItemFlat : 0u;
       sh->n_flat += flat ? 1 : 0;
-      sh->n_slab_fast += (!flat && fast) ? 1 : 0;
       sh->n_general += flat ? 0 : 1;
       sh->items.push_back(it);
     };
@@ -1275,15 +1206,12 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
       it.nrows = (i + 1 < common.size() ? common[i + 1] : rg.num_rows) - common[i];
       it.global_row0 = rg.global_row0 + common[i];
       const uint32_t row_end = it.row0 + it.nrows;
-      bool fast = use_slab_index, copied = use_flat && it.nrows != 0;
+      bool copied = use_flat && it.nrows != 0;
       cuts.clear();
       for (uint32_t s = 0; s < ncols; s++) {
         const TableChunk& tc = rg.chunks[tcols[s]];
         if (!tc.present) { it.absent |= 1u << s; continue; }   // missing from this file: all NULL (schema adapter behaviour)
         it.page[s] = page_of(s, it.row0, uint32_t(i));
-        const DevPage& pg = pages[it.page[s]];
-        const bool whole = pg.first_row == it.row0 && pg.num_rows == it.nrows;
-        if (!whole || !(pg.flags & 1u)) fast = false;
         // every page of this column under the item needs a flat copy; their starts cut the item into pieces
         for (uint32_t pi = it.page[s]; pi < tc.pages.first_page + tc.pages.n_pages && pages[pi].first_row < row_end; pi++) {
           if (flat_pages.empty() || flat_pages[pi].fkind == FK_NONE) {
@@ -1295,9 +1223,8 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
           if (pages[pi].first_row > it.row0) cuts.push_back(pages[pi].first_row);
         }
       }
-      if (!it.nrows) fast = false;
       sh->n_uncopied += copied ? 0 : 1;
-      if (!copied || !pieces) { push_item(it, false, fast); continue; }
+      if (!copied || !pieces) { push_item(it, false); continue; }
       // flat: one piece per stretch between page starts of ANY column (a piece lies in one page of every column)
       std::sort(cuts.begin(), cuts.end());
       cuts.erase(std::unique(cuts.begin(), cuts.end()), cuts.end());
@@ -1315,7 +1242,7 @@ std::shared_ptr<Shape> Table::shape_for(const std::vector<int>& tcols, cudaStrea
           pc.page[s] = page_of(s, r, uint32_t(i));
           pc.poff[s] = r - pages[pc.page[s]].first_row;
         }
-        push_item(pc, true, false);
+        push_item(pc, true);
         r = cut;
       }
     }
@@ -1343,8 +1270,6 @@ void Table::ensure_plain8(int tcol, cudaStream_t stream) const {
   std::lock_guard<std::mutex> lk(side_mu);
   ColSide& cs = sides[tcol];
   if (cs.delta_ready || !cs.has_delta) return;
-  const char* sw = getenv("PQB_FLAT");
-  if (sw && sw[0] == '0') { cs.delta_ready = true; return; }
   struct Job { uint32_t page, pad; uint64_t dst, vsrc, tmp; };   // == DeltaJob; offsets relative to d_flat
   std::vector<Job> jobs;
   uint64_t off = 0;
@@ -1358,7 +1283,6 @@ void Table::ensure_plain8(int tcol, cudaStream_t stream) const {
     for (uint32_t k = 0; k < tc.pages.n_pages; k++) {
       const uint32_t pi = tc.pages.first_page + k;
       if (pages[pi].enc != DE_DELTA || flat_pages[pi].fkind != FK_NONE) continue;
-      if (pages[pi].def_len && !nulls_classified) continue;   // nobody looked at the definition levels: the page may hold NULLs
       Job j{pi, 0u, take(uint64_t(pages[pi].num_rows) * 8), flat_pages[pi].voff, ~0ull};
       if (j.vsrc != ~0ull) j.tmp = take(uint64_t(pages[pi].num_rows) * 8);
       jobs.push_back(j);

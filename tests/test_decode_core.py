@@ -104,57 +104,45 @@ def test_hybrid_tiny_windows_force_slab_shrink(dc, bw, cap, max_ent):
     assert np.array_equal(out.astype(np.uint64), vals)
 
 
-@pytest.mark.parametrize("bw", [0, 1, 3, 5, 8, 13, 17, 32])
-def test_transcode_to_flat_bitpacked(dc, bw):
-    """Run-heavy pages are kept in the slab index as a flat bit-packed copy (transcode_values)."""
-    rng = np.random.default_rng(1234 + bw)
-    n = 20000
-    hi = (1 << bw) if bw else 1
-    vals = np.repeat(rng.integers(0, hi, n, dtype=np.uint64), rng.integers(1, 25, n))[:n].astype(np.uint64)
-    enc = encode_hybrid(vals, bw, rng, rle_bias=0.6)
-    words = np.zeros(n * max(bw, 1) // 32 + 8, np.uint32)
-    dc.dc_transcode.restype = C.c_int64
-    got = dc.dc_transcode(enc, C.c_uint64(len(enc)), bw, n, 2048, words.ctypes.data_as(C.c_void_p))
-    assert got == n
-    if bw == 0:
-        return
-    bits = np.unpackbits(words.view(np.uint8), bitorder="little")[: n * bw].reshape(n, bw).astype(np.uint64)
-    back = (bits << np.arange(bw, dtype=np.uint64)).sum(axis=1)
-    assert np.array_equal(back, vals)
-
-
-@pytest.mark.parametrize("pattern", ["random", "skewed", "long_runs", "mixed"])
+@pytest.mark.parametrize("pattern", ["random", "skewed", "long_runs", "mixed", "short_runs"])
 @pytest.mark.parametrize("bw", [0, 1, 3, 6, 8, 9, 11, 14, 17])
-def test_slab_index_and_octet_pass_replica(dc, bw, pattern):
-    """CPU replica of k_slab_index / k_flatten_pages / the octet pass (tools/decode_core_host.cpp): the
-    selection bytes of a dictionary-LUT leaf over one 20 000-row page must equal LUT[value] for every
-    run structure — bit-packed only, a skewed column (hundreds of tiny runs: flat copy), long RLE runs,
-    and a mix whose octets straddle directory entries."""
+def test_walker_directory_and_octet_pass_replica(dc, bw, pattern):
+    """CPU replica of k_scan's per-slab walk and the octet pass (tools/decode_core_host.cpp): the
+    selection bits of a dictionary-LUT leaf over one 20 000-row page must equal LUT[value] for every
+    run structure — bit-packed only, a skewed column (many short runs), long RLE runs, a mix whose
+    octets straddle directory entries, and RLE runs of 1-4 values, more than one directory holds, so
+    that slabs shrink and later slabs start inside a byte or word of the bitmap."""
     rng = np.random.default_rng(100 * bw + len(pattern))
     n = 20000
     hi = (1 << bw) if bw else 1
+    rle_bias = 0.5
     if pattern == "random":
         vals = rng.integers(0, hi, n, dtype=np.uint64)
     elif pattern == "skewed":
         vals = np.where(rng.random(n) < 0.8, 0, rng.integers(0, hi, n)).astype(np.uint64)
     elif pattern == "long_runs":
         vals = np.repeat(rng.integers(0, hi, n // 150 + 2, dtype=np.uint64), rng.integers(100, 400, n // 150 + 2))[:n]
-    else:
+    elif pattern == "mixed":
         vals = np.repeat(rng.integers(0, hi, n // 5 + 2, dtype=np.uint64), rng.integers(1, 30, n // 5 + 2))[:n]
+    else:
+        vals = np.repeat(rng.integers(0, hi, n // 2 + 2, dtype=np.uint64), rng.integers(1, 5, n // 2 + 2))[:n]
+        rle_bias = 1.0
     vals = vals.astype(np.uint64)
-    enc = encode_hybrid(vals, bw, rng, rle_bias=0.5)
+    enc = encode_hybrid(vals, bw, rng, rle_bias=rle_bias)
     smem = 1 if hi <= 2048 else 0
     lut = (rng.random(max(hi, 2048)) < 0.3).astype(np.uint8)
-    out = np.zeros((n + 7) // 8 + 256, np.uint8)
-    flat = C.c_int32(0)
-    dc.dc_index_octet_scan.restype = C.c_int64
-    got = dc.dc_index_octet_scan(enc, C.c_uint64(len(enc)), bw, n, lut.ctypes.data_as(C.c_void_p), smem, 16,
-                                 out.ctypes.data_as(C.c_void_p), C.byref(flat))
+    bitmap = np.zeros((n + 31) // 32 + 1, np.uint32)
+    shrunk = C.c_uint32(0)
+    dc.dc_walk_octet_scan.restype = C.c_int64
+    got = dc.dc_walk_octet_scan(enc, C.c_uint64(len(enc)), bw, n, lut.ctypes.data_as(C.c_void_p), smem,
+                                bitmap.ctypes.data_as(C.c_void_p), C.byref(shrunk))
     assert got == n
     exp = np.packbits(lut[vals.astype(np.int64)].astype(bool), bitorder="little")
-    assert np.array_equal(out[: len(exp)], exp), (bw, pattern, flat.value)
+    assert np.array_equal(bitmap.view(np.uint8)[: len(exp)], exp), (bw, pattern, shrunk.value)
     if pattern == "long_runs" and bw >= 1:
-        assert flat.value == 0      # a handful of long runs per slab fits the directory budget
+        assert shrunk.value == 0    # a handful of long runs per slab fits one directory
+    if pattern == "short_runs" and bw >= 1:
+        assert shrunk.value >= 1    # the octet pass runs over shrunk slabs
 
 
 def test_f64_order_key_is_total_order(dc):

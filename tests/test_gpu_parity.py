@@ -287,8 +287,8 @@ def test_arrow_default_pages_and_v2(data_dir, built):
         for flt in ([col("k") == 7], [(col("v") > 0) & (col("s") == "ccc")], [col("f") < -1.0], [col("b") == True],  # noqa: E712
                     [~(col("b") == True) | col("f").is_null()]):                                                       # noqa: E712
             assert prov.scan(filters=flt, count_only=True).metrics["rows_selected"] == ora.count(flt), (ver, kw, flt)
-        # one 120 000-row page per row group: a slab-indexed item of 59 slabs (several record batches),
-        # long RLE runs kept as a flat copy; the row ids must come out exactly
+        # with the default page size, one 120 000-row page per row group: a work item of 59 slabs over
+        # long RLE runs; the row ids must come out exactly
         for flt in ([col("k") == 7], [(col("k") == 7) & (col("s") == "ccc")]):
             res = prov.scan(filters=flt)
             ids = np.concatenate([b.column(0).to_numpy() for b in res.batches]) if res.batches else np.array([], np.int64)

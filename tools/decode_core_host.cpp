@@ -40,23 +40,6 @@ int64_t dc_decode_hybrid(const uint8_t* stream, uint64_t len, uint32_t bw, uint3
   }
   return done;
 }
-// hybrid stream -> flat bit-packed words (the slab index's copy of run-heavy pages), `slab` values per call
-int64_t dc_transcode(const uint8_t* stream, uint64_t len, uint32_t bw, uint32_t n, uint32_t slab, uint32_t* out_words) {
-  std::vector<uint8_t> padded(len + 64 + 16, 0);
-  std::memcpy(padded.data() + 16, stream, len);
-  StreamState st;
-  stream_init(st, 16, 16 + len, bw);
-  BitWriter b{out_words, 0, 0};
-  uint32_t done = 0;
-  while (done < n) {
-    uint32_t need = n - done < slab ? n - done : slab;
-    uint32_t got = transcode_values(st, padded.data(), need, b);
-    done += got;
-    if (got < need) return -int64_t(done) - 1;
-  }
-  bitwriter_flush(b);
-  return done;
-}
 // DELTA_BINARY_PACKED page payload -> int64 values, through the kernel's window / directory geometry
 int64_t dc_decode_delta(const uint8_t* stream, uint64_t len, uint32_t n, uint32_t slab, uint32_t win_cap,
                         uint32_t max_ent, int64_t* out) {
@@ -110,11 +93,12 @@ int dc_like(const uint8_t* s, uint32_t n, const uint8_t* p, uint32_t m, uint32_t
 uint64_t dc_load_u64(const uint8_t* base, uint32_t off) { return load_u64_unaligned(base + off); }
 }
 
-// ---- replica of the slab index + the octet pass (TEST ONLY) ------------------------------------
-// k_slab_index / k_flatten_pages / octet_leaf live in scan_kernel.cuh as device code; this is the
-// same algorithm over one page on the CPU (octet_leaf_replica is the device function's text with the
-// funnel-shift intrinsic spelled out), so random run structures, every bit width, the entry budget,
-// the flat-copy fallback and the straddling-octet path are exercised without a GPU.
+// ---- replica of k_scan's per-slab run directory + the octet pass (TEST ONLY) --------------------
+// k_scan's slab control and octet_leaf / fast_and_rows live in scan_kernel.cuh as device code; this is
+// the same algorithm over one NULL-free dictionary page on the CPU (octet_leaf_replica is the device
+// function's text with the funnel-shift intrinsic spelled out), so random run structures, every bit
+// width, the directory budget, slabs shrunk to what the walker covered and the straddling-octet path
+// are exercised without a GPU.
 static inline uint32_t host_funnelshift_r(uint32_t lo, uint32_t hi, uint32_t sh) {
   const uint64_t both = (uint64_t(hi) << 32) | lo;
   return uint32_t(both >> (sh & 31));
@@ -205,68 +189,68 @@ static inline uint32_t octet_leaf_replica(const uint32_t* dirw, uint32_t nent, c
   return m;
 }
 
-extern "C" int64_t dc_index_octet_scan(const uint8_t* stream, uint64_t len, uint32_t bw, uint32_t n, const uint8_t* lut,
-                                       uint32_t smem_lut, uint32_t budget_per_slab, uint8_t* out_bytes, int32_t* used_flat) {
-  const uint32_t cap = ((kSlabRows * bw / 8 + kSlabRows / 8 + 64) + 15u) & ~15u;   // valwin_cap_for_bw
+// One page through k_scan's general path as MODE_FAST_AND runs it: per slab, issue_windows stages
+// valwin_cap_for_bw(bw) bytes from the stream's window start, the walker builds the directory
+// (kMaxDirEntries - 2 entries, two sentinels behind), and when it covers fewer rows than the slab's
+// target, general_walk shrinks the slab to what it covered and walks again from the same cursor.  The
+// octet pass then places the slab's selection bits in the page's bitmap the way fast_and_rows does.
+// Returns the rows scanned (-1: the walker made no progress); *shrunk = slabs that were shrunk.
+extern "C" int64_t dc_walk_octet_scan(const uint8_t* stream, uint64_t len, uint32_t bw, uint32_t n, const uint8_t* lut,
+                                      uint32_t smem_lut, uint32_t* bitmap, uint32_t* shrunk) {
+  const uint32_t cap = valwin_cap_for_bw(bw);
   std::vector<uint8_t> arena(16 + len + cap + 64, 0);
   std::memcpy(arena.data() + 16, stream, len);
-  const uint32_t nslabs = (n + kSlabRows - 1) / kSlabRows;
-  struct Rec { const uint8_t* win; uint32_t nent, ent0; };
-  std::vector<Rec> recs(nslabs);
-  const uint32_t budget = nslabs * budget_per_slab;
-  std::vector<DirEntry> dirs(budget + 3 * nslabs + 8);
-  std::vector<uint32_t> side;
   StreamState st;
   stream_init(st, 16, 16 + len, bw);
-  uint32_t used = 0, rows_left = n;
-  bool flat = false;
-  for (uint32_t k = 0; k < nslabs && !flat; k++) {      // k_slab_index
-    const uint32_t R = rows_left < (uint32_t)kSlabRows ? rows_left : (uint32_t)kSlabRows;
-    const uint64_t base = stream_window_start(st) & ~15ull;
-    const Window w{arena.data() + base, base, cap};
-    uint32_t m = 0, got = 0;
-    if (used + 3 <= budget) {
-      const uint32_t room = budget - used - 2;
-      got = walk_stream(st, w, R, dirs.data() + used, m, room < uint32_t(kMaxDirEntries - 2) ? room : uint32_t(kMaxDirEntries - 2));
+  std::vector<uint32_t> win(cap / 4 + 8);
+  std::vector<DirEntry> dir(kMaxDirEntries);
+  uint32_t r_item = 0;
+  *shrunk = 0;
+  while (r_item < n) {
+    const uint32_t target = n - r_item < (uint32_t)kSlabRows ? n - r_item : (uint32_t)kSlabRows;
+    const uint64_t base = stream_window_start(st) & ~15ull;        // issue_windows: the TMA copy of the window
+    std::memset(win.data(), 0, win.size() * 4);
+    std::memcpy(win.data(), arena.data() + base, cap);
+    const Window w{reinterpret_cast<const uint8_t*>(win.data()), base, cap};
+    const StreamState snap = st;
+    uint32_t nent = 0;
+    uint32_t R = walk_stream(st, w, target, dir.data(), nent, kMaxDirEntries - 2);
+    if (R < target) {                                                 // general_walk: shrink, walk again
+      if (R == 0) return -1;
+      ++*shrunk;
+      st = snap;
+      nent = 0;
+      if (walk_stream(st, w, R, dir.data(), nent, kMaxDirEntries - 2) != R) return -1;
     }
-    if (got < R || m == 0) { flat = true; break; }
-    DirEntry* d = dirs.data() + used;
-    d[m].start = 0xffffffffu; d[m].count = 0; d[m].kind = 0; d[m].chunk0 = 0; d[m].payload = 0; d[m]._pad = 0; d[m + 1] = d[m];
-    recs[k] = {arena.data() + base, m, used};
-    used += m + 2;
-    rows_left -= R;
-  }
-  *used_flat = flat ? 1 : 0;
-  if (flat) {                                           // k_flatten_pages
-    side.assign(size_t(n) * (bw ? bw : 1) / 32 + cap / 4 + 64, 0);
-    stream_init(st, 16, 16 + len, bw);
-    BitWriter b{side.data(), 0, 0};
-    rows_left = n;
-    for (uint32_t k = 0; k < nslabs; k++) {
-      const uint32_t R = rows_left < (uint32_t)kSlabRows ? rows_left : (uint32_t)kSlabRows;
-      if (transcode_values(st, arena.data(), R, b) < R) return -1;
-      DirEntry* d = dirs.data() + 3 * k;
-      d[0].start = 0; d[0].count = uint16_t(R); d[0].kind = bw ? 1 : 0; d[0].chunk0 = 0; d[0].payload = 0; d[0]._pad = 0;
-      d[1].start = 0xffffffffu; d[1].count = 0; d[1].kind = 0; d[1].chunk0 = 0; d[1].payload = 0; d[1]._pad = 0; d[2] = d[1];
-      recs[k] = {reinterpret_cast<const uint8_t*>(side.data()) + size_t(k) * (kSlabRows / 8) * bw, 1, 3 * k};
-      rows_left -= R;
-    }
-    bitwriter_flush(b);
-  }
-  // the octet pass over every slab: 256 "threads" x 8 rows, windows and directories staged like the TMA copies
-  std::vector<uint32_t> win(cap / 4 + 8), dirw(size_t(kMaxDirEntries) * kDirWords);
-  rows_left = n;
-  for (uint32_t k = 0; k < nslabs; k++) {
-    const uint32_t R = rows_left < (uint32_t)kSlabRows ? rows_left : (uint32_t)kSlabRows;
-    std::memcpy(win.data(), recs[k].win, cap);
-    std::memcpy(dirw.data(), dirs.data() + recs[k].ent0, (recs[k].nent + 2) * sizeof(DirEntry));
-    for (uint32_t t = 0; t < 256; t++) {
+    DirEntry* d = dir.data();                                         // dir_sentinels
+    d[nent].start = 0xffffffffu; d[nent].count = 0; d[nent].kind = 0; d[nent].chunk0 = 0; d[nent].payload = 0; d[nent]._pad = 0;
+    d[nent + 1] = d[nent];
+    const uint32_t* dirw = reinterpret_cast<const uint32_t*>(d);
+    // fast_and_rows: 256 threads x 8 rows; byte stores when the slab starts on a byte, else 32-row words ORed in
+    uint8_t sel[kSlabRows / 8];
+    for (uint32_t t = 0; t < kSlabRows / 8; t++) {
       const uint32_t r8 = t * 8;
       uint32_t sel8 = r8 >= R ? 0u : (R - r8 >= 8 ? 0xffu : ((1u << (R - r8)) - 1u));
-      if (sel8) sel8 &= octet_leaf_replica(dirw.data(), recs[k].nent, win.data(), bw, r8, sel8, smem_lut != 0, lut, lut);
-      if (size_t(k) * 256 + t < (size_t(n) + 7) / 8) out_bytes[size_t(k) * 256 + t] = uint8_t(sel8);
+      if (sel8) sel8 &= octet_leaf_replica(dirw, nent, win.data(), bw, r8, sel8, smem_lut != 0, lut, lut);
+      sel[t] = uint8_t(sel8);
     }
-    rows_left -= R;
+    if ((r_item & 7u) == 0) {
+      for (uint32_t t = 0; t < kSlabRows / 8; t++)
+        if (sel[t]) reinterpret_cast<uint8_t*>(bitmap)[(r_item + t * 8) >> 3] = sel[t];
+    } else {
+      for (uint32_t wd = 0; wd < (uint32_t)kSlabWords; wd++) {
+        const uint32_t v = sel[4 * wd] | (sel[4 * wd + 1] << 8) | (sel[4 * wd + 2] << 16) | (uint32_t(sel[4 * wd + 3]) << 24);
+        if (v == 0) continue;
+        const uint32_t pos = r_item + wd * 32, sh = pos & 31;
+        uint32_t* dst = bitmap + (pos >> 5);
+        if (sh == 0) *dst = v;
+        else {
+          dst[0] |= v << sh;
+          if (v >> (32 - sh)) dst[1] |= v >> (32 - sh);
+        }
+      }
+    }
+    r_item += R;
   }
   return n;
 }

@@ -13,12 +13,16 @@ namespace pqb {
 
 constexpr int kSlotTile = 1024;
 
-// non-empty groups per tile of kSlotTile slots
-__global__ void k_slot_tile_counts(const unsigned long long* __restrict__ rows, uint32_t nslots, uint32_t* __restrict__ tile_counts) {
+// The slot at list position p: order[p] (a permutation of the slots), or p itself when order is nullptr
+__device__ __forceinline__ uint32_t slot_at(const uint32_t* __restrict__ order, uint32_t p) { return order ? order[p] : p; }
+
+// non-empty groups per tile of kSlotTile list positions
+__global__ void k_slot_tile_counts(const unsigned long long* __restrict__ rows, uint32_t nslots, uint32_t* __restrict__ tile_counts,
+                                   const uint32_t* __restrict__ order) {
   __shared__ uint32_t ws[8];
   const uint32_t s0 = blockIdx.x * kSlotTile;
   uint32_t c = 0;
-  for (uint32_t i = threadIdx.x; i < (uint32_t)kSlotTile; i += blockDim.x) c += (s0 + i < nslots && rows[s0 + i] != 0) ? 1u : 0u;
+  for (uint32_t i = threadIdx.x; i < (uint32_t)kSlotTile; i += blockDim.x) c += (s0 + i < nslots && rows[slot_at(order, s0 + i)] != 0) ? 1u : 0u;
   c = __reduce_add_sync(0xffffffffu, c);
   if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = c;
   __syncthreads();
@@ -29,14 +33,15 @@ __global__ void k_slot_tile_counts(const unsigned long long* __restrict__ rows, 
   }
 }
 
-// ascending slot order: out_slot[base[tile] + rank inside the tile]; 256 threads x 4 consecutive slots
+// list order (ascending slot, or order[]): out_slot[base[tile] + rank inside the tile]; 256 threads x 4 consecutive positions
 __global__ void __launch_bounds__(256) k_slot_compact(const unsigned long long* __restrict__ rows, uint32_t nslots,
-                                                      const unsigned long long* __restrict__ tile_base, uint32_t* __restrict__ out_slot) {
+                                                      const unsigned long long* __restrict__ tile_base, uint32_t* __restrict__ out_slot,
+                                                      const uint32_t* __restrict__ order) {
   __shared__ uint32_t ws[8];
   const uint32_t s0 = blockIdx.x * kSlotTile + threadIdx.x * 4;
   uint32_t f[4], c = 0;
 #pragma unroll
-  for (int k = 0; k < 4; k++) { f[k] = (s0 + k < nslots && rows[s0 + k] != 0) ? 1u : 0u; c += f[k]; }
+  for (int k = 0; k < 4; k++) { f[k] = (s0 + k < nslots && rows[slot_at(order, s0 + k)] != 0) ? 1u : 0u; c += f[k]; }
   uint32_t incl = c;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int o = 1; o < 32; o <<= 1) {
@@ -50,7 +55,7 @@ __global__ void __launch_bounds__(256) k_slot_compact(const unsigned long long* 
   unsigned long long pos = tile_base[blockIdx.x] + wbase + incl - c;
 #pragma unroll
   for (int k = 0; k < 4; k++)
-    if (f[k]) out_slot[pos++] = s0 + k;
+    if (f[k]) out_slot[pos++] = slot_at(order, s0 + k);
 }
 
 struct FinishKey {

@@ -210,6 +210,25 @@ struct Shape {
   ~Shape();
 };
 
+// Tuple id pages of one GROUP BY key tuple (Table::ensure_tuple_pages): the groups that occur in the table, numbered by
+// row count (descending, ties by mixed-radix id), and one bit-packed page of tuple ids per page of the lead key column.
+// A query that holds the entry keeps its device memory alive.
+struct TuplePages {
+  uint32_t n_tuples = 0, bw = 0;
+  int lead = -1;                        // table column whose pages the tuple pages follow
+  uint8_t* d_buf = nullptr;             // the pages (FlatPageRec.off relative to d_flat, like every flat page)
+  std::vector<std::pair<uint32_t, FlatPageRec>> recs;   // lead page index -> its tuple page
+  unsigned long long* d_wide = nullptr; // tuple id -> mixed-radix id
+  uint32_t* d_order = nullptr;          // position -> tuple id, ascending mixed-radix id
+  uint64_t bytes = 0;
+  double build_ms = 0;
+  // the table's agg page table with the lead pages replaced by the tuple pages, for the agg pages version it copies
+  // (Table::tuple_page_table; guarded by the table's side_mu)
+  mutable std::shared_ptr<const FlatPageRec> d_pages;
+  mutable uint64_t pages_ver = ~0ull;
+  ~TuplePages();
+};
+
 // Encoded column chunks of a set of files, resident in HBM ("hot tier in HBM").
 class Table {
  public:
@@ -266,6 +285,15 @@ class Table {
   mutable FlatPageRec* d_agg_pages = nullptr;
   bool ensure_for_pages(int tcol, bool f64, cudaStream_t stream) const;
   bool ensure_id_pages(int tcol, cudaStream_t stream) const;
+  mutable uint64_t agg_pages_ver = 0;   // counts the agg page builds (a tuple entry's page table copies one version)
+  // tuple id pages of a GROUP BY key tuple in the local numbering, keyed by (table column, mixed-radix stride) per key:
+  // built once per tuple (nullptr: the one attempt failed, the query keeps per-key pages), at most kMaxTupleEntries
+  static constexpr size_t kMaxTupleEntries = 16;
+  mutable std::map<std::vector<std::pair<int, uint64_t>>, std::shared_ptr<const TuplePages>> tuples;
+  std::shared_ptr<const TuplePages> ensure_tuple_pages(const std::vector<std::pair<int, uint64_t>>& keys, bool verbose,
+                                                       cudaStream_t stream) const;
+  // the tuple entry's page table for the current agg pages (built on first use after an agg page build)
+  std::shared_ptr<const FlatPageRec> tuple_page_table(const TuplePages& tp, cudaStream_t stream) const;
 
  private:
   void build_flat_store(cudaStream_t stream);

@@ -499,6 +499,86 @@ __global__ void __launch_bounds__(128) k_agg_form_pack(uint8_t* __restrict__ fla
   }
 }
 
+// ---- tuple id pages: one id per GROUP BY key tuple (Table::ensure_tuple_pages) ----
+// A job is a row range of one lead-column page over which every key column stays inside one page.  The row's group is
+// the mixed radix of its keys' ids, exactly as k_flat_agg forms it from per-key pages (NULL and an absent chunk: id
+// card).  k_tuple_count counts the rows of every group that occurs; k_tuple_pack writes each row's tuple id (the
+// group's rank by count) into the lead page's tuple page at w bits, ORing into a zeroed buffer where jobs share a word.
+struct TupleKeySrc {
+  uint64_t src;        // the key's FK_INDEX page (flat offset)
+  uint64_t voff;       // its validity bitmap, or ~0
+  const uint32_t* gid; // gid LUT of the chunk (device address of gid + the row group's base); nullptr: chunk absent
+  uint32_t row0, sbw, dict_n, _pad;
+};
+struct TupleJob {
+  uint64_t dst;        // the lead page's tuple page (flat offset, may wrap: a buffer of its own)
+  uint32_t row0, rows; // rows [row0, row0 + rows) of the lead page
+  TupleKeySrc k[kMaxKeys];
+};
+struct TupleArgs {
+  const TupleJob* jobs;
+  uint32_t n_jobs, nkeys, w;
+  uint32_t card[kMaxKeys], stride[kMaxKeys];
+  unsigned int* counts;   // k_tuple_count: rows per mixed-radix id
+  const uint32_t* rank;   // k_tuple_pack: tuple id per mixed-radix id
+};
+__device__ __forceinline__ uint32_t tuple_mixed(const uint8_t* __restrict__ flat, const TupleArgs& a, const TupleJob& j, uint32_t r) {
+  uint32_t m = 0;
+  for (uint32_t k = 0; k < a.nkeys; k++) {
+    const TupleKeySrc& s = j.k[k];
+    uint32_t id = a.card[k];
+    const uint32_t rr = s.row0 + r;
+    if (s.gid && (s.voff == ~0ull || ((reinterpret_cast<const uint32_t*>(flat + s.voff)[rr >> 5] >> (rr & 31)) & 1u))) {
+      const uint32_t smask = s.sbw >= 32 ? 0xffffffffu : ((1u << s.sbw) - 1u), dict_max = s.dict_n ? s.dict_n - 1 : 0u;
+      uint32_t idx = s.sbw ? (bits32_at(reinterpret_cast<const uint32_t*>(flat + s.src), rr * s.sbw) & smask) : 0u;
+      idx = idx < dict_max ? idx : dict_max;   // as col_index: a corrupt index never leaves the dictionary
+      id = s.gid[idx];
+    }
+    m += id * a.stride[k];
+  }
+  return m;
+}
+// one warp per job; lanes that meet the same group add once
+__global__ void __launch_bounds__(128) k_tuple_count(const uint8_t* __restrict__ flat, const __grid_constant__ TupleArgs a) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t ji = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (ji >= a.n_jobs) return;
+  const TupleJob& j = a.jobs[ji];
+  for (uint32_t r0 = 0; r0 < j.rows; r0 += 32) {
+    const uint32_t r = r0 + lane;
+    const bool live = r < j.rows;
+    const uint32_t m = live ? tuple_mixed(flat, a, j, r) : ~0u;
+    const uint32_t peers = __match_any_sync(0xffffffffu, m);
+    if (live && lane == uint32_t(__ffs(peers) - 1)) atomicAdd(a.counts + m, uint32_t(__popc(peers)));
+  }
+}
+// one warp per job; a lane writes whole groups of 32 rows of the lead page (w words each)
+__global__ void __launch_bounds__(128) k_tuple_pack(uint8_t* __restrict__ flat, const __grid_constant__ TupleArgs a) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t ji = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (ji >= a.n_jobs) return;
+  const TupleJob& j = a.jobs[ji];
+  uint32_t* __restrict__ dst = reinterpret_cast<uint32_t*>(flat + j.dst);
+  const uint32_t g0 = j.row0 / 32, g1 = (j.row0 + j.rows + 31) / 32;
+  for (uint32_t g = g0 + lane; g < g1; g += 32) {
+    uint32_t* out = dst + size_t(g) * a.w;
+    uint64_t acc = 0;
+    uint32_t nacc = 0;
+    for (uint32_t k = 0; k < 32; k++) {
+      const uint32_t p = g * 32 + k;   // row of the lead page
+      const uint32_t x = (p >= j.row0 && p < j.row0 + j.rows) ? a.rank[tuple_mixed(flat, a, j, p - j.row0)] : 0u;
+      acc |= uint64_t(x) << nacc;
+      nacc += a.w;
+      if (nacc >= 32) {
+        if (uint32_t(acc)) atomicOr(out, uint32_t(acc));
+        out++;
+        acc >>= 32;
+        nacc -= 32;
+      }
+    }
+  }
+}
+
 // ---- DELTA_BINARY_PACKED (Parseable's p_timestamp, streams.rs:587-590) -> aligned 8-byte values ----
 // Only built when a query needs the VALUES of such a column (a time range that cuts a row group, a
 // projection of p_timestamp): footer statistics decide the injected range for every other query and

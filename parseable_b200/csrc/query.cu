@@ -345,6 +345,7 @@ static uint8_t* build_agg_pages(const Table& t, std::vector<AggFormJob>& jobs, c
   }
   PQB_CUDA(cudaStreamSynchronize(stream));
   bytes = off;
+  t.agg_pages_ver++;
   return buf;
 }
 
@@ -422,6 +423,182 @@ bool Table::ensure_id_pages(int tcol, cudaStream_t stream) const {
   cs.d_ids = build_agg_pages(*this, jobs, page_of, FK_IDS, cs.ids_bytes, stream);
   cs.ids_bw = w;
   return cs.d_ids != nullptr;
+}
+
+TuplePages::~TuplePages() {
+  if (d_buf) cudaFree(d_buf);
+  if (d_wide) cudaFree(d_wide);
+  if (d_order) cudaFree(d_order);
+}
+
+// Tuple id pages of the key columns `keys` (table column, mixed-radix stride), every one a dictionary key in the local
+// numbering (after ensure_key) whose pages all have flat-store index pages.  The lead column is the first key present
+// in every row group; none: no tuple pages.  Counts on the device, ranks on the host, packs on the device.
+std::shared_ptr<const TuplePages> Table::ensure_tuple_pages(const std::vector<std::pair<int, uint64_t>>& keys, bool verbose,
+                                                            cudaStream_t stream) const {
+  std::lock_guard<std::mutex> lk(side_mu);
+  auto it = tuples.find(keys);
+  if (it != tuples.end()) return it->second;
+  if (tuples.size() >= kMaxTupleEntries) return nullptr;
+  std::shared_ptr<const TuplePages>& slot = tuples[keys];   // one attempt: a failure stays nullptr
+  const auto t0 = std::chrono::steady_clock::now();
+  const uint32_t nk = uint32_t(keys.size());
+  TupleArgs ta{};
+  ta.nkeys = nk;
+  uint64_t space = 1;
+  int lead = -1;
+  for (uint32_t k = 0; k < nk; k++) {
+    const ColSide& cs = sides[keys[k].first];
+    if (!cs.key_ready || !cs.key_row_pages.empty()) return nullptr;
+    ta.card[k] = cs.card;
+    ta.stride[k] = uint32_t(keys[k].second);
+    space = std::max<uint64_t>(space, keys[k].second * (uint64_t(cs.card) + 1));
+    bool everywhere = true;
+    for (const TableRowGroup& rg : row_groups) everywhere = everywhere && rg.chunks[keys[k].first].present;
+    if (everywhere && lead < 0) lead = int(k);
+  }
+  if (lead < 0 || space > (1ull << 26)) return nullptr;
+  const int lcol = keys[lead].first;
+  // jobs: per row group, the row ranges between the page starts of all key columns
+  std::vector<TupleJob> jobs;
+  std::vector<uint32_t> lead_pages;
+  for (size_t g = 0; g < row_groups.size(); g++) {
+    std::vector<uint32_t> cuts;
+    for (uint32_t k = 0; k < nk; k++) {
+      const TableChunk& tc = row_groups[g].chunks[keys[k].first];
+      if (!tc.present) continue;
+      for (uint32_t p = 0; p < tc.pages.n_pages; p++) {
+        const uint32_t pi = tc.pages.first_page + p;
+        if (flat_pages[pi].fkind != FK_INDEX) return nullptr;   // every page of a key must be a flat-store index page
+        cuts.push_back(pages[pi].first_row);
+      }
+    }
+    cuts.push_back(row_groups[g].num_rows);
+    std::sort(cuts.begin(), cuts.end());
+    cuts.erase(std::unique(cuts.begin(), cuts.end()), cuts.end());
+    std::vector<uint32_t> at(nk, 0);   // current page of each key
+    for (size_t c = 0; c + 1 < cuts.size(); c++) {
+      const uint32_t r0 = cuts[c], r1 = cuts[c + 1];
+      if (r1 <= r0) continue;
+      TupleJob j{};
+      j.rows = r1 - r0;
+      for (uint32_t k = 0; k < nk; k++) {
+        const TableChunk& tc = row_groups[g].chunks[keys[k].first];
+        if (!tc.present) continue;
+        while (at[k] + 1 < tc.pages.n_pages && pages[tc.pages.first_page + at[k] + 1].first_row <= r0) at[k]++;
+        const uint32_t pi = tc.pages.first_page + at[k];
+        const FlatPageRec& fr = flat_pages[pi];
+        if (r1 > pages[pi].first_row + fr.rows) return nullptr;   // pages must cover the row group
+        j.k[k] = TupleKeySrc{fr.off, fr.voff, sides[keys[k].first].d_gid + sides[keys[k].first].base_per_rg[g], r0 - pages[pi].first_row,
+                             fr.bw, tc.dict_n, 0};
+        if (int(k) == lead) {
+          j.row0 = r0 - pages[pi].first_row;
+          if (lead_pages.empty() || lead_pages.back() != pi) lead_pages.push_back(pi);
+          j.dst = pi;   // the lead page for now; its tuple page's offset below
+        }
+      }
+      jobs.push_back(j);
+    }
+  }
+  if (jobs.empty()) return nullptr;
+  // 1. rows per group
+  std::vector<unsigned int> counts(space, 0u);
+  {
+    DevBuf<unsigned int> d_counts;
+    DevBuf<TupleJob> d_jobs;
+    if (cudaMallocAsync((void**)&d_counts.p, space * 4, stream) != cudaSuccess) { (void)cudaGetLastError(); return nullptr; }
+    d_counts.n = space;
+    d_counts.s = stream;
+    d_counts.zero();
+    d_jobs.upload(jobs, stream);
+    ta.jobs = d_jobs.p;
+    ta.n_jobs = uint32_t(jobs.size());
+    ta.counts = d_counts.p;
+    k_tuple_count<<<uint32_t((jobs.size() + 3) / 4), 128, 0, stream>>>(d_flat, ta);
+    PQB_CUDA(cudaGetLastError());
+    PQB_CUDA(cudaMemcpyAsync(counts.data(), d_counts.p, space * 4, cudaMemcpyDeviceToHost, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+  }
+  // 2. rank: count descending, mixed-radix id ascending
+  std::vector<uint32_t> occurring;
+  for (uint32_t m = 0; m < space; m++) if (counts[m]) occurring.push_back(m);
+  if (occurring.empty()) return nullptr;
+  std::vector<uint32_t> wide = occurring;
+  std::stable_sort(wide.begin(), wide.end(), [&](uint32_t a, uint32_t b) { return counts[a] > counts[b]; });
+  std::vector<uint32_t> rank(space, 0u);
+  for (uint32_t t = 0; t < wide.size(); t++) rank[wide[t]] = t;
+  std::vector<uint32_t> order(occurring.size());
+  for (size_t p = 0; p < occurring.size(); p++) order[p] = rank[occurring[p]];
+  auto tp = std::make_shared<TuplePages>();
+  tp->n_tuples = uint32_t(wide.size());
+  tp->bw = std::max<uint32_t>(1, bit_width_u64(tp->n_tuples - 1u));
+  tp->lead = lcol;
+  // 3. the pages: one per lead page, 16-byte aligned, zeroed (jobs that share a word OR into it)
+  std::unordered_map<uint32_t, uint64_t> page_off;
+  uint64_t off = 0;
+  for (uint32_t pi : lead_pages) {
+    page_off[pi] = off;
+    off += ((uint64_t(flat_pages[pi].rows) + 31) / 32 * tp->bw * 4 + 15) & ~15ull;
+  }
+  std::vector<unsigned long long> wide64(wide.begin(), wide.end());
+  if (!try_alloc((void**)&tp->d_buf, off + 64, stream)) return nullptr;   // + the over-read of a slab's last staged word
+  if (!try_alloc((void**)&tp->d_wide, wide64.size() * 8, stream) || !try_alloc((void**)&tp->d_order, order.size() * 4, stream)) return nullptr;
+  PQB_CUDA(cudaMemsetAsync(tp->d_buf, 0, off + 64, stream));
+  PQB_CUDA(cudaMemcpyAsync(tp->d_wide, wide64.data(), wide64.size() * 8, cudaMemcpyHostToDevice, stream));
+  PQB_CUDA(cudaMemcpyAsync(tp->d_order, order.data(), order.size() * 4, cudaMemcpyHostToDevice, stream));
+  const uint64_t rel = uint64_t(tp->d_buf) - uint64_t(d_flat);   // the subtraction may wrap, d_flat + offset does not
+  for (TupleJob& j : jobs) j.dst = rel + page_off[uint32_t(j.dst)];
+  {
+    DevBuf<uint32_t> d_rank;
+    DevBuf<TupleJob> d_jobs;
+    d_rank.upload(rank, stream);
+    d_jobs.upload(jobs, stream);
+    ta.jobs = d_jobs.p;
+    ta.rank = d_rank.p;
+    ta.counts = nullptr;
+    ta.w = tp->bw;
+    k_tuple_pack<<<uint32_t((jobs.size() + 3) / 4), 128, 0, stream>>>(d_flat, ta);
+    PQB_CUDA(cudaGetLastError());
+    PQB_CUDA(cudaStreamSynchronize(stream));
+  }
+  for (uint32_t pi : lead_pages) {
+    FlatPageRec r = flat_pages[pi];
+    r.off = rel + page_off[pi];
+    r.voff = ~0ull;   // a NULL key is part of its tuple
+    r.bw = uint8_t(tp->bw);
+    r.fkind = FK_IDS;
+    tp->recs.emplace_back(pi, r);
+  }
+  tp->bytes = off + wide64.size() * 8 + order.size() * 4;
+  tp->build_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  if (verbose)
+    fprintf(stderr, "[pqb] tuple pages: %u keys, lead column %s, %u tuples of %llu slots, %u bits, %zu jobs over %zu lead pages, "
+            "%.1f MB, built in %.2f ms\n", nk, columns[lcol].name.c_str(), tp->n_tuples, (unsigned long long)space, tp->bw, jobs.size(),
+            lead_pages.size(), double(tp->bytes) / 1e6, tp->build_ms);
+  if (const char* vb = getenv("PQB_VERBOSE"); vb && vb[0] == '2')   // the numbering itself (first 4 096 tuples)
+    for (uint32_t t = 0; t < std::min<uint32_t>(tp->n_tuples, 4096); t++)
+      fprintf(stderr, "[pqb] tuple %u: mixed-radix id %u, %u rows\n", t, wide[t], counts[wide[t]]);
+  slot = tp;
+  return tp;
+}
+
+std::shared_ptr<const FlatPageRec> Table::tuple_page_table(const TuplePages& tp, cudaStream_t stream) const {
+  std::lock_guard<std::mutex> lk(side_mu);
+  if (tp.d_pages && tp.pages_ver == agg_pages_ver) return tp.d_pages;
+  std::vector<FlatPageRec> recs = agg_pages;
+  if (recs.empty()) {
+    FlatPageRec blank{};
+    blank.voff = ~0ull;
+    recs.assign(pages.size(), blank);
+  }
+  for (const auto& pr : tp.recs) recs[pr.first] = pr.second;
+  FlatPageRec* p = nullptr;
+  if (!try_alloc((void**)&p, recs.size() * sizeof(FlatPageRec), stream)) return nullptr;
+  PQB_CUDA(cudaMemcpyAsync(p, recs.data(), recs.size() * sizeof(FlatPageRec), cudaMemcpyHostToDevice, stream));
+  PQB_CUDA(cudaStreamSynchronize(stream));
+  tp.d_pages = std::shared_ptr<const FlatPageRec>(p, [](const FlatPageRec* q) { cudaFree(const_cast<FlatPageRec*>(q)); });
+  tp.pages_ver = agg_pages_ver;
+  return tp.d_pages;
 }
 
 void launch_entry_offsets(const Table& t, int tcol, uint64_t* d_out, uint32_t* max_len, cudaStream_t stream) {
@@ -1983,12 +2160,43 @@ void Query::run(const PqQueryDesc& d) {
   std::vector<uint32_t> form_bw(ncols, 0);   // marked slots: widest page the slot stages
   uint32_t value_forms = 0;                  // the marked slots that read value pages (FK_FOR)
   plan.agg_forms = 0;
+  // ---- tuple id pages: a GROUP BY of two or more dictionary keys whose columns have no other role reads ONE id per row,
+  // the group's rank by row count in the table, from pages that follow the lead key's pages.  k_flat_agg sees a one-key
+  // plan (tkey) over n_tuples slots, so the hottest GROUPS (not the hottest values of the largest key) own the hot
+  // table; the result keeps the real keys, decoded from tuple->d_wide, and comes out in mixed-radix order (d_order) ----
+  std::shared_ptr<const TuplePages> tuple;
+  std::shared_ptr<const FlatPageRec> tuple_pages_tbl;
+  DevKey tkey{};
+  uint32_t tuple_keyslots = 0;   // column slots of the tuple's keys
+  {
+    const char* tw = getenv("PQB_TUPLE_PAGES");   // A/B switch: 0 = per-key id pages
+    const char* sw = getenv("PQB_AGG_FORMS");
+    bool ok = !(tw && tw[0] == '0') && !(sw && sw[0] == '0') && agg_kernel && n_flat && !n_general && d.table && !plan.ndist &&
+              !plan.npct && !plan.hashed && !allreduce && !multi && d.n_group_by >= 2;
+    std::vector<std::pair<int, uint64_t>> tkeys;
+    for (uint32_t k = 0; ok && k < d.n_group_by; k++) {
+      const DevKey& key = plan.keys[k];
+      const uint32_t s = key.col;
+      const ColSide& cs = table->sides[shape_cols[s]];
+      ok = key.kind == KK_DICT_LUT && key.gid == cs.d_gid && cs.key_row_pages.empty() && !((tuple_keyslots >> s) & 1u);
+      for (uint32_t l = 0; ok && l < nleaves; l++) ok = plan.leaves[l].col != s;
+      for (uint32_t a = 0; ok && a < d.n_aggs; a++) ok = plan.aggs[a].fn == AG_COUNT_STAR || plan.aggs[a].col != s;
+      tuple_keyslots |= 1u << s;
+      tkeys.emplace_back(shape_cols[s], key.wstride);
+    }
+    if (ok) {
+      std::sort(tkeys.begin(), tkeys.end());
+      tuple = table->ensure_tuple_pages(tkeys, verbose, stream);
+    }
+    if (!tuple) tuple_keyslots = 0;
+  }
   {
     const char* sw = getenv("PQB_AGG_FORMS");   // A/B switch: 0 = every slot reads its index pages
     // not with COUNT(DISTINCT) or MEDIAN / PERCENTILE_CONT: their kernel instantiations carry no agg-page paths (their
     // registers would spill there)
     if (!(sw && sw[0] == '0') && agg_kernel && n_flat && d.table && !plan.ndist && !plan.npct) {
       for (uint32_t s = 0; s < ncols; s++) {
+        if ((tuple_keyslots >> s) & 1u) continue;   // the tuple pages serve the key slots
         bool as_key = false, as_value = false, other = false;
         for (uint32_t l = 0; l < nleaves; l++) other |= plan.leaves[l].col == s;
         int key = -1;
@@ -2027,6 +2235,29 @@ void Query::run(const PqQueryDesc& d) {
       }
     }
   }
+  // the tuple query's page table copies the agg pages as they stand after this query's last ensure_* above, so that every
+  // value page a marked slot's stage was sized for is in it.  Without the memory for the copy the key slots read their
+  // index pages through the gid LUT (they asked for no id pages above)
+  if (tuple) tuple_pages_tbl = table->tuple_page_table(*tuple, stream);
+  if (tuple && tuple_pages_tbl) {
+    for (uint32_t k = 0; k < d.n_group_by; k++)
+      if (shape_cols[plan.keys[k].col] == tuple->lead) tkey = plan.keys[k];
+    tkey.card = tuple->n_tuples;
+    tkey.stride = 1;
+    tkey.wstride = 1;
+    for (uint32_t s = 0; s < ncols; s++)
+      if (((tuple_keyslots >> s) & 1u) && s != tkey.col) plan.cols[s].staged = 0;
+    plan.nslots = tuple->n_tuples;
+    plan.agg_forms |= 1u << tkey.col;
+    form_bw[tkey.col] = tuple->bw;
+  } else {
+    tuple.reset();
+  }
+  if (verbose && tuple)
+    fprintf(stderr, "[pqb] group slots: tuple pages, lead column %s, %u tuples, %u bits, built in %.2f ms\n",
+            table->columns[tuple->lead].name.c_str(), tuple->n_tuples, tuple->bw, tuple->build_ms);
+  else if (verbose && agg_kernel && d.n_group_by >= 2)
+    fprintf(stderr, "[pqb] group slots: per-key ids (mixed radix)\n");
   mark("side tables ready");
   // ---- shared-memory layout of k_scan (items the flat kernels do not take) ----
   SmemLayout L{};
@@ -2249,7 +2480,7 @@ void Query::run(const PqQueryDesc& d) {
   sa.rg_live = pruned ? d_live.p : nullptr;
   sa.flat = table->d_flat;
   sa.fpages = d_kpages.p ? d_kpages.p : table->d_flat_pages;
-  sa.apages = plan.agg_forms ? table->d_agg_pages : nullptr;
+  sa.apages = tuple ? tuple_pages_tbl.get() : plan.agg_forms ? table->d_agg_pages : nullptr;
   sa.bitmap = d_bitmap.p;
   sa.item_counts = d_item_counts.p;
   sa.acc = d_acc.p;
@@ -2261,9 +2492,14 @@ void Query::run(const PqQueryDesc& d) {
     if (agg_kernel) {
       grid = std::min<uint32_t>(n_flat, uint32_t(ctx.sm_count()));
       if (const char* g = getenv("PQB_GRID")) grid = std::max(1, atoi(g));
+      DevPlan kplan = plan;   // tuple pages: the kernel's plan has the one key tkey
+      if (tuple) {
+        kplan.nkeys = 1;
+        kplan.keys[0] = tkey;
+      }
       auto go = [&](auto kern) {
         PQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(ctx.smem_optin())));
-        kern<<<grid, kAggThreads, FL.total, stream>>>(plan, FL, sa);
+        kern<<<grid, kAggThreads, FL.total, stream>>>(kplan, FL, sa);
       };
       if (rx_bytes) {   // a regular expression over pages without a dictionary: the instantiations with the DFA walk
         if (plan.npct) {
@@ -2378,9 +2614,10 @@ void Query::run(const PqQueryDesc& d) {
     d_tile_base.alloc(ntiles, stream);
     d_totals.alloc(2, stream);
     d_out_slot.alloc(out_cap, stream);
-    k_slot_tile_counts<<<ntiles, 256, 0, stream>>>(d_acc.p, plan.nslots, d_tile_counts.p);
+    const uint32_t* order = tuple ? tuple->d_order : nullptr;   // tuple slots: listed in the order of their mixed-radix ids
+    k_slot_tile_counts<<<ntiles, 256, 0, stream>>>(d_acc.p, plan.nslots, d_tile_counts.p, order);
     k_item_prefix<<<1, 1024, 0, stream>>>(d_tile_counts.p, ntiles, d_tile_base.p, d_totals.p);
-    k_slot_compact<<<ntiles, 256, 0, stream>>>(d_acc.p, plan.nslots, d_tile_base.p, d_out_slot.p);
+    k_slot_compact<<<ntiles, 256, 0, stream>>>(d_acc.p, plan.nslots, d_tile_base.p, d_out_slot.p, order);
     // rows this rank selected (its own items)
     DevBuf<unsigned long long> d_item_base;
     d_item_base.alloc(std::max<size_t>(items.size(), 1), stream);
@@ -2503,7 +2740,7 @@ void Query::run(const PqQueryDesc& d) {
         std::swap(d_out_slot.n, slots.n);
       }
       fa.acc = d_acc.p;
-      fa.wide = plan.hashed ? d_hkeys.p : nullptr;
+      fa.wide = plan.hashed ? d_hkeys.p : tuple ? tuple->d_wide : nullptr;
       fa.out_slot = d_out_slot.p;
       fa.out = d_block.p;
       fa.nulls = reinterpret_cast<uint32_t*>(d_block.p + nulls_off);
@@ -2556,7 +2793,7 @@ void Query::run(const PqQueryDesc& d) {
     const bool tail_hint = d.n_group_by && !ordered && !plan.npct;
     uint64_t tail_key = 0;
     if (tail_hint) {
-      tail_key = plan_hash(plan, lit_pool, batch_rows);
+      tail_key = plan_hash(plan, lit_pool, batch_rows) ^ (tuple ? 0x9e3779b97f4a7c15ull : 0ull);   // a tuple plan is not its per-key plan
       uint32_t cap = 0;
       {
         std::lock_guard<std::mutex> lk(shape->hint_mu);
@@ -2640,7 +2877,7 @@ void Query::run(const PqQueryDesc& d) {
         OrderArgs oa{};
         uint8_t nulls_first[kMaxOrder];
         oa.acc = d_acc.p;
-        oa.wide = plan.hashed ? d_hkeys.p : nullptr;
+        oa.wide = plan.hashed ? d_hkeys.p : tuple ? tuple->d_wide : nullptr;
         oa.out_slot = d_out_slot.p;
         oa.n = n_out;
         oa.nslots = plan.nslots;

@@ -220,6 +220,18 @@ __global__ void k_offsets_scan(const uint32_t* __restrict__ lens, uint32_t n, co
   if (threadIdx.x == 0) offs[n] = int32_t(carry);
 }
 
+// the exact string bytes of key k over the output rows (for a result whose count-free bound is too large to allocate)
+__global__ void k_key_bytes_total(const __grid_constant__ FinishArgs f, uint32_t k, unsigned long long* __restrict__ total) {
+  const FinishKey& key = f.keys[k];
+  unsigned long long s = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < finish_rows(f); i += gridDim.x * blockDim.x) {
+    const uint32_t gid = key_gid_of_slot(f.wide, f.out_slot[i], key.wstride, key.card);
+    if (gid != key.card) s += key.kd_offs[gid + 1] - key.kd_offs[gid];
+  }
+  for (int o = 16; o; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0 && s) atomicAdd(total, s);
+}
+
 // string key bytes: one warp per output row
 __global__ void k_key_gather(const __grid_constant__ FinishArgs f, uint32_t k) {
   const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;

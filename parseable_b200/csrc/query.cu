@@ -58,6 +58,7 @@ struct DevBuf {
 };
 
 constexpr uint64_t kKeepDeviceResult = 1ull << 30;   // result blocks up to this size stay on the device until the query closes
+constexpr uint64_t kExactKeyBytes = 64ull << 20;     // a string key whose byte bound exceeds this is counted exactly first
 // COUNT(DISTINCT): the dense presence bitmap of one distinct column may take this much HBM (and at most a quarter of
 // the free HBM); above it the column gets a pair set, of at most kDistinctPairsMax 8-byte entries (2 GiB)
 constexpr uint64_t kDistinctDenseBudget = 1ull << 30;
@@ -669,7 +670,7 @@ void build_key_side(const Table& t, int tcol, ColSide& side, cudaStream_t stream
   while (cap < 4ull * maxn) cap <<= 1;
   while (cap < std::min<uint64_t>(2 * row_entries, 1ull << 22)) cap <<= 1;   // rows: start where a column of mostly distinct values needs few redos
   DevBuf<uint32_t> rep;
-  uint32_t card = 0;
+  uint32_t card = 0, rebuilds = 0;
   for (;;) {
     DevBuf<unsigned long long> slots; slots.alloc(cap, stream); slots.zero();
     DevBuf<uint32_t> gid_of_slot; gid_of_slot.alloc(cap, stream);
@@ -692,6 +693,7 @@ void build_key_side(const Table& t, int tcol, ColSide& side, cudaStream_t stream
     if (cnt[1] == 1 || cnt[0] * 2ull > cap) {  // table too full: grow and redo
       if (cap > (1ull << 30)) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY key table overflow");
       cap <<= 2;
+      rebuilds++;
       continue;
     }
     if (cnt[1]) throw Error(PQ_ERR_CUDA, "group key lookup failed");
@@ -702,6 +704,9 @@ void build_key_side(const Table& t, int tcol, ColSide& side, cudaStream_t stream
     break;
   }
   side.card = card;
+  if (const char* vb = getenv("PQB_VERBOSE"); vb && vb[0] && vb[0] != '0')
+    fprintf(stderr, "[pqb] key column %s: card %u, %u dictionary entries + %llu rows, table capacity %llu, %u rebuilds\n",
+            t.columns[tcol].name.c_str(), card, n, (unsigned long long)row_entries, (unsigned long long)cap, rebuilds);
   // ---- hot-first numbering: occurrences of every id over a sample of the column's flat pages ----
   if (card > 1 && t.d_flat_pages) {
     std::vector<KeySamplePage> sp;
@@ -2094,6 +2099,12 @@ void Query::run(const PqQueryDesc& d) {
   for (uint32_t k = 0; agg_kernel && k < d.n_group_by; k++)
     if (plan.keys[k].kind == KK_BIN && n_general)
       throw Error(PQ_ERR_UNSUPPORTED, "DATE_BIN keys need a flat-store copy of every page the query reads: " + shape->why_general);
+  // k_scan reads a key's dictionary index of every row; the rows of pages without a dictionary have none (their ids are
+  // staged as id pages by k_flat_agg only)
+  for (uint32_t k = 0; agg_kernel && k < d.n_group_by; k++)
+    if (row_keys[k] && n_general)
+      throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[shape_cols[plan.keys[k].col]].name +
+                                      "' has pages without a dictionary, which need a flat-store copy of every page the query reads: " + shape->why_general);
   if (agg_kernel && plan.hashed && n_general)
     throw Error(PQ_ERR_UNSUPPORTED, "a hashed GROUP BY needs a flat-store copy of every page the query reads: " + shape->why_general);
   for (uint32_t i = 0; agg_kernel && i < plan.ndist; i++)
@@ -2640,7 +2651,7 @@ void Query::run(const PqQueryDesc& d) {
       std::unique_ptr<DevBuf<uint8_t>> d_block;
       std::shared_ptr<PinnedBlock> block;
     };
-    auto assemble = [&](uint32_t n_out, const unsigned long long* n_dev, bool cut) -> Assembled {
+    auto assemble = [&](uint32_t n_out, const unsigned long long* n_dev) -> Assembled {
       Assembled r;
       r.rows = n_out;
       FinishArgs& fa = r.fa;
@@ -2702,18 +2713,36 @@ void Query::run(const PqQueryDesc& d) {
       }
       uint64_t win_off[2] = {0, 0};
       for (size_t w = 0; w < win_names.size(); w++) win_off[w] = take(uint64_t(n_out) * 8);
-      // string key bytes: an upper bound (rows x the longest distinct value) keeps the copy to one round trip
+      // string key bytes: an upper bound keeps the copy to one round trip.  Rows x the longest distinct value; or, as one
+      // value of key k sits in at most prod_{j != k}(card_j + 1) groups, that many copies of all its distinct values.
+      // Both hold for any subset of the groups (a result cut by ORDER BY ... LIMIT).  Where that bound is large, the
+      // exact bytes of the output rows are counted on the device first (one more round trip)
       for (uint32_t k = 0; k < d.n_group_by; k++) {
         FinishKey& fk = fa.keys[k];
         if (fk.kind != DK_STR) continue;
         uint64_t max_len = 0;
         const KeyDict* kd = qk[k].kd;
         max_len = multi ? table->sides[shape_cols[plan.keys[k].col]].glob_max_len : table->sides[shape_cols[plan.keys[k].col]].kd_max_len;
-        // the count-based bound is over all the groups; a result cut by ORDER BY ... LIMIT may be any subset of them (the
-        // top 5 rows can all hold the one longest value): rows x the longest value there.  A full ORDER BY holds the same
-        // rows as the unordered result, so the count-based bound still holds for it.
-        const uint64_t bound = cut ? uint64_t(n_out) * max_len
-                                       : std::min<uint64_t>(uint64_t(n_out) * max_len, uint64_t(n_out / std::max<uint32_t>(fk.card, 1) + 1) * kd->bytes.size());
+        uint64_t copies = 1;
+        for (uint32_t j = 0; j < d.n_group_by; j++)
+          if (j != k) copies = std::min<uint64_t>(uint64_t(n_out), copies * (uint64_t(qk[j].card) + 1));
+        uint64_t bound = std::min<uint64_t>(uint64_t(n_out) * max_len, copies * kd->bytes.size());
+        if (bound > kExactKeyBytes && !wrun) {
+          fa.wide = plan.hashed ? d_hkeys.p : tuple ? tuple->d_wide : nullptr;
+          fa.out_slot = d_out_slot.p;
+          fa.n_out = n_out;
+          fa.n_dev = n_dev;
+          DevBuf<unsigned long long> total;
+          total.alloc(1, stream);
+          total.zero();
+          k_key_bytes_total<<<std::min<uint32_t>(1024, (n_out + 255) / 256), 256, 0, stream>>>(fa, k, total.p);
+          launches++;
+          PQB_CUDA(cudaGetLastError());
+          unsigned long long exact = 0;
+          PQB_CUDA(cudaMemcpyAsync(&exact, total.p, 8, cudaMemcpyDeviceToHost, stream));
+          PQB_CUDA(cudaStreamSynchronize(stream));
+          bound = exact;
+        }
         if (bound > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "group key strings of one result exceed 2 GiB");
         fk.data_off = take(bound);
       }
@@ -2804,7 +2833,7 @@ void Query::run(const PqQueryDesc& d) {
       cap = uint32_t(std::min<uint64_t>(cap, out_cap));
       if (verbose) fprintf(stderr, "[pqb] result tail: %s\n", cap ? ("one round trip, block for " + std::to_string(cap) + " groups").c_str()
                                                                      : "no earlier answer of this plan: two round trips");
-      if (cap) pre = assemble(cap, d_totals.p, false);
+      if (cap) pre = assemble(cap, d_totals.p);
     }
     unsigned long long totals[2] = {0, 0};
     std::vector<unsigned int> pct_count(plan.npct, 0u);
@@ -2977,7 +3006,7 @@ void Query::run(const PqQueryDesc& d) {
     } else {
       if (pre.rows < n_out) {   // no block yet, or one too small for the groups: lay it out for n_out
         if (pre.rows && verbose) fprintf(stderr, "[pqb] result tail: %u groups, the block had room for %u: second copy\n", n_out, pre.rows);
-        pre = assemble(n_out, nullptr, keep < n_total);
+        pre = assemble(n_out, nullptr);
         PQB_CUDA(cudaStreamSynchronize(stream));
       }
       Assembled& r = pre;

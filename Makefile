@@ -20,8 +20,12 @@ CPP_SRCS  := $(CSRC)/parquet_meta.cpp $(CSRC)/arrow_export.cpp $(CSRC)/capi.cpp 
              $(CSRC)/regex_compile.cpp
 OBJS      := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(CU_SRCS)) $(patsubst $(CSRC)/%.cpp,$(OBJDIR)/%.o,$(CPP_SRCS))
 HDRS      := $(wildcard $(CSRC)/*.hpp $(CSRC)/*.cuh $(CSRC)/*.inc include/*.h)
+# the same library on a host-staged communicator (tools/comm_host.cpp, no NCCL): several ranks as processes on one
+# device, for tests only (PQB_LIB selects it)
+HOSTCOMM_LIB  := tools/libparseable_b200_hostcomm.so
+HOSTCOMM_OBJS := $(filter-out $(OBJDIR)/comm.o,$(OBJS)) $(OBJDIR)/comm_host.o
 
-all: $(LIB) oracle tools
+all: $(LIB) $(HOSTCOMM_LIB) oracle tools
 
 $(OBJDIR)/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -33,6 +37,12 @@ $(OBJDIR)/%.o: $(CSRC)/%.cpp $(HDRS)
 
 $(LIB): $(OBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $(OBJS) -lcudart $(NCCL_LIB)
+
+$(OBJDIR)/comm_host.o: tools/comm_host.cpp $(HDRS)
+	@mkdir -p $(OBJDIR)
+	$(NVCC) $(NVFLAGS) -I$(CSRC) -x cu -c $< -o $@
+$(HOSTCOMM_LIB): $(HOSTCOMM_OBJS)
+	$(NVCC) $(ARCH) -shared -o $@ $(HOSTCOMM_OBJS) -lcudart
 
 oracle: oracle/liboracle.so
 oracle/liboracle.so: oracle/oracle.c
@@ -60,7 +70,7 @@ tools/libdecode_core_host.so: tools/decode_core_host.cpp $(CSRC)/decode_core.cuh
 	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 
 clean:
-	rm -rf $(OBJDIR) $(LIB) oracle/liboracle.so tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so \
+	rm -rf $(OBJDIR) $(LIB) $(HOSTCOMM_LIB) oracle/liboracle.so tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so \
 	      tools/liblz_host.so tools/liblz_host_desc.so tools/libdecomp_dev.so
 
 .PHONY: all oracle tools clean

@@ -1715,6 +1715,19 @@ void Query::run(const PqQueryDesc& d) {
       algo_bytes += uint64_t(tc.meta->total_uncompressed_size);
     }
   }
+  const bool allreduce = (d.flags & PQ_QUERY_ALLREDUCE) != 0;
+  if (allreduce && !comm_active()) throw Error(PQ_ERR_INVALID_ARG, "PQ_QUERY_ALLREDUCE without pq_comm_init_rank");
+  const bool multi = agg_kernel && allreduce && comm_nranks() > 1;
+  // every query that meets the other ranks in a collective (an aggregate table, or COUNT(*)'s total) agrees on refusals
+  const bool agree = has_aggs && allreduce && comm_nranks() > 1;
+  const uint32_t n_flat = flat_ok ? shape->n_flat : 0;
+  const uint32_t n_general = flat_ok ? shape->n_general : uint32_t(items.size());
+  // ---- refusals that depend on what this rank's shard holds (its pages, footers and flat-store copies).  Under a
+  // multi-rank all-reduce every rank must refuse together: a rank that threw while the others went on into a collective
+  // would leave them waiting for it.  So they are all found here, before the first collective, and the tiny all-reduce
+  // below carries "refused" words; without other ranks to meet the first one found is thrown right away ----
+  std::string refusal;
+  auto refuse = [&](const std::string& why) { if (refusal.empty()) refusal = why; };
   for (uint32_t s = 0; s < ncols; s++) {
     const std::string& cname = table->columns[shape_cols[s]].name;
     plan.cols[s].has_delta = shape->has_delta[s];
@@ -1722,28 +1735,100 @@ void Query::run(const PqQueryDesc& d) {
     plan.cols[s].has_plain = shape->has_plain[s];
     plan.cols[s].max_bw = shape->max_bw[s];
     if (shape->has_delta[s] && plan.cols[s].kind != DK_I64)
-      throw Error(PQ_ERR_UNSUPPORTED, "column '" + cname + "': DELTA_BINARY_PACKED is decoded for INT64 columns only");
+      refuse("column '" + cname + "': DELTA_BINARY_PACKED is decoded for INT64 columns only");
     if (shape->has_plain[s] && plan.cols[s].kind == DK_STR && shape->n_uncopied)
-      throw Error(PQ_ERR_UNSUPPORTED, "column '" + cname + "': PLAIN (dictionary-fallback) string pages without a flat-store copy are not decoded on the GPU");
+      refuse("column '" + cname + "': PLAIN (dictionary-fallback) string pages without a flat-store copy are not decoded on the GPU");
   }
+  auto filtered_on = [&](uint32_t s) {
+    for (uint32_t l = 0; l < nleaves; l++)
+      if (plan.leaves[l].col == s && value_leaf(plan.leaves[l].kind)) return true;
+    return false;
+  };
+  // DATE_BIN keys: the bins any scanned row of this rank can fall into, from the footer statistics of its live row groups
+  std::vector<std::pair<int64_t, int64_t>> bin_vrange(d.n_group_by, {INT64_MAX, INT64_MIN});
+  for (uint32_t k = 0; agg_kernel && k < d.n_group_by; k++) {
+    const uint32_t s = uint32_t(slot_of[d.group_by[k]]);
+    const std::string& cname = table->columns[tcol[d.group_by[k]]].name;
+    if (d.group_exprs && d.group_exprs[k].kind == PQ_KEY_DATE_BIN) {
+      const PqKeyExpr& gx = d.group_exprs[k];
+      if (plan.cols[s].kind != DK_I64 || gx.width_ms <= 0) continue;   // refused below, alike on every rank
+      int64_t& vmin = bin_vrange[k].first;
+      int64_t& vmax = bin_vrange[k].second;
+      for (uint32_t g = 0; g < nrg_table; g++) {
+        if (!rg_live[g]) continue;
+        const TableChunk& tc = table->row_groups[g].chunks[shape_cols[s]];
+        if (!tc.present) continue;
+        const ColumnStats& st = tc.meta->stats;
+        if (st.null_count >= 0 && uint64_t(st.null_count) == uint64_t(tc.meta->num_values)) continue;   // all NULL: no bins
+        if (!st.has_min || !st.has_max || st.min.size() != 8 || st.max.size() != 8) {
+          refuse("DATE_BIN over '" + cname + "' needs min / max statistics in the file footers");
+          break;
+        }
+        int64_t mn, mx;
+        std::memcpy(&mn, st.min.data(), 8);
+        std::memcpy(&mx, st.max.data(), 8);
+        vmin = std::min(vmin, mn);
+        vmax = std::max(vmax, mx);
+      }
+      if (vmin <= vmax && (vmin < gx.origin_ms - (int64_t(1) << 52) || vmax > gx.origin_ms + (int64_t(1) << 52)))
+        refuse("DATE_BIN: values more than 2^52 ms away from the origin");
+      if (n_general) refuse("DATE_BIN keys need a flat-store copy of every page the query reads: " + shape->why_general);
+      continue;
+    }
+    if (plan.cols[s].kind == DK_BOOL || !(plan.cols[s].has_plain || plan.cols[s].has_delta)) continue;
+    // Pages without a dictionary (PLAIN fallback of an overflowed dictionary, PLAIN / DELTA numerics): their ROWS are
+    // interned next to the dictionary entries and the aggregate kernel stages the pages' ids instead of their values, so
+    // nothing else of this query may read the column's values, and k_scan, which reads a dictionary index per row, cannot
+    // take them
+    if (filtered_on(s))
+      refuse("GROUP BY column '" + cname + "' has pages without a dictionary and is also filtered on: not on the GPU path");
+    for (uint32_t a = 0; a < d.n_aggs; a++)
+      if (((plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG) || plan.aggs[a].fn >= AG_MEDIAN) && plan.aggs[a].col == s &&
+          !rank_min_max(plan.aggs[a]))
+        refuse("GROUP BY column '" + cname + "' has pages without a dictionary and is also aggregated: not on the GPU path");
+    if (n_general)
+      refuse("GROUP BY column '" + cname + "' has pages without a dictionary, which need a flat-store copy of every page the query reads: " +
+             shape->why_general);
+  }
+  {
+    uint64_t lut_entries = 0;   // the per-leaf LUT regions (side tables below)
+    for (uint32_t l = 0; l < nleaves; l++)
+      if (value_leaf(plan.leaves[l].kind)) lut_entries += table->sides[shape_cols[plan.leaves[l].col]].total_entries;
+    if (lut_entries > 0xfffffff0ull) refuse("leaf LUTs too large");
+  }
+  for (uint32_t a = 0; agg_kernel && a < d.n_aggs; a++) {
+    const DevAgg& ag = plan.aggs[a];
+    if (rank_min_max(ag) && (plan.cols[ag.col].has_plain || plan.cols[ag.col].has_delta) && filtered_on(ag.col))
+      refuse(std::string(ag.fn == AG_MIN ? "MIN(" : "MAX(") + table->columns[shape_cols[ag.col]].name +
+             "): the column has pages without a dictionary and is also filtered on: not on the GPU path");
+    // (a column in no file has nothing to read: k_scan takes it)
+    if (n_general && (rank_min_max(ag) || bool_min_max(ag)) && table->columns[shape_cols[ag.col]].kind != 0xfe)
+      refuse(std::string(ag.fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
+             ") over Utf8 / Boolean needs a flat-store copy of every page the query reads: " + shape->why_general);
+  }
+  if (!refusal.empty() && !agree) throw Error(PQ_ERR_UNSUPPORTED, refusal);
   // k_flat_agg walks a regular expression's DFA per row only in its RX instantiations
   bool rx_bytes = false;
   for (uint32_t l = 0; l < nleaves; l++) rx_bytes |= plan.leaves[l].kind == LK_REGEX && plan.cols[plan.leaves[l].col].has_plain;
   plan.n_items = uint32_t(items.size());
   metrics.bytes_scanned = scanned_bytes;
-  const bool allreduce = (d.flags & PQ_QUERY_ALLREDUCE) != 0;
-  if (allreduce && !comm_active()) throw Error(PQ_ERR_INVALID_ARG, "PQ_QUERY_ALLREDUCE without pq_comm_init_rank");
-  const bool multi = agg_kernel && allreduce && comm_nranks() > 1;
   // an aggregated column whose footers promise null_count == 0 in every row group read: its non-null
   // counter equals the group's row count, so the scan skips that atomic (and the table is 4 cells per group
   // narrower on C4).  Under PQ_QUERY_ALLREDUCE the cells are summed across ranks and every rank must make the same
   // choice: the per-rank footer verdicts are summed over the ranks first (a rank whose row groups were all pruned
   // contributes zeros).  The same tiny all-reduce carries whether every rank still holds the agreed numbering of the
   // GROUP BY key values (kept with the table column, tagged with the communicator's epoch; a rank may have reopened its
-  // table): ONE collective and one round trip per query for both agreements.
+  // table): ONE collective and one round trip per query for both agreements.  Its last two words are the number of ranks
+  // that refuse the query (then every rank refuses) and a mask of the refusing ranks below 63 (bit r for rank r; the bits
+  // are distinct, so their sum is their union), which names one of them.  A COUNT(*)-only query runs it for the refusals
+  // alone: its total's all-reduce comes after the scan.
   bool keys_agreed = true;
-  if (multi) {
-    std::vector<unsigned long long> f(1 + ncols, 0ull);
+  if (agree) {
+    std::vector<unsigned long long> f(3 + ncols, 0ull);
+    if (!refusal.empty()) {
+      f[1 + ncols] = 1;
+      if (comm_rank() < 63) f[2 + ncols] = 1ull << comm_rank();
+    }
     for (uint32_t k = 0; k < d.n_group_by; k++) {
       if (d.group_exprs && d.group_exprs[k].kind == PQ_KEY_DATE_BIN) continue;
       const uint32_t s = uint32_t(slot_of[d.group_by[k]]);
@@ -1762,8 +1847,15 @@ void Query::run(const PqQueryDesc& d) {
     comm_allreduce_u64(df.p, f.size(), 0 /*sum*/, stream);
     PQB_CUDA(cudaMemcpyAsync(f.data(), df.p, f.size() * 8, cudaMemcpyDeviceToHost, stream));
     PQB_CUDA(cudaStreamSynchronize(stream));
-    keys_agreed = f[0] == 0;
-    for (uint32_t s = 0; s < ncols; s++) col_has_nulls[s] = f[1 + s] != 0;
+    if (!refusal.empty()) throw Error(PQ_ERR_UNSUPPORTED, refusal);
+    if (f[1 + ncols])
+      throw Error(PQ_ERR_UNSUPPORTED, "refused on " + (f[2 + ncols] ? "rank " + std::to_string(__builtin_ctzll(f[2 + ncols]))
+                                                                    : std::to_string(f[1 + ncols]) + " ranks") +
+                                          " (its shard holds pages or footers this query cannot take on the GPU path)");
+    if (multi) {
+      keys_agreed = f[0] == 0;
+      for (uint32_t s = 0; s < ncols; s++) col_has_nulls[s] = f[1 + s] != 0;
+    }
   }
   std::vector<uint8_t> nn_is_rows(kMaxAggs, 0);
   {
@@ -1797,7 +1889,6 @@ void Query::run(const PqQueryDesc& d) {
     lf.lut_off = 0;
     if (!value_leaf(lf.kind)) continue;
     const ColSide& cs = table->sides[shape_cols[lf.col]];
-    if (lut_total + cs.total_entries > 0xfffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "leaf LUTs too large");
     lf.lut_off = uint32_t(lut_total);
     lut_total += cs.total_entries;
     any_lut |= cs.total_entries != 0;
@@ -1816,31 +1907,16 @@ void Query::run(const PqQueryDesc& d) {
     const uint8_t kind = plan.cols[key.col].kind;
     if (d.group_exprs && d.group_exprs[k].kind == PQ_KEY_DATE_BIN) {
       // ---- DATE_BIN(width, column, origin) (the counts / histogram API, src/query/mod.rs:623-680): the key is
-      // computed from the value; the bins any scanned row can fall into come from the footer statistics ----
+      // computed from the value; the bins any scanned row can fall into come from the footer statistics (bin_vrange,
+      // read with the refusals above) ----
       const PqKeyExpr& gx = d.group_exprs[k];
       const std::string& cname = table->columns[tcol[d.group_by[k]]].name;
       if (kind != DK_I64) throw Error(PQ_ERR_INVALID_ARG, "DATE_BIN needs a Timestamp / Int64 column, '" + cname + "' is neither");
       if (gx.width_ms <= 0) throw Error(PQ_ERR_INVALID_ARG, "DATE_BIN needs a positive stride");
-      int64_t vmin = INT64_MAX, vmax = INT64_MIN;
-      for (uint32_t g = 0; g < nrg_table; g++) {
-        if (!rg_live[g]) continue;
-        const TableChunk& tc = table->row_groups[g].chunks[shape_cols[key.col]];
-        if (!tc.present) continue;
-        const ColumnStats& st = tc.meta->stats;
-        if (st.null_count >= 0 && uint64_t(st.null_count) == uint64_t(tc.meta->num_values)) continue;   // all NULL: no bins
-        if (!st.has_min || !st.has_max || st.min.size() != 8 || st.max.size() != 8)
-          throw Error(PQ_ERR_UNSUPPORTED, "DATE_BIN over '" + cname + "' needs min / max statistics in the file footers");
-        int64_t mn, mx;
-        std::memcpy(&mn, st.min.data(), 8);
-        std::memcpy(&mx, st.max.data(), 8);
-        vmin = std::min(vmin, mn);
-        vmax = std::max(vmax, mx);
-      }
+      const int64_t vmin = bin_vrange[k].first, vmax = bin_vrange[k].second;
       auto floordiv = [](int64_t a, int64_t b) { int64_t q = a / b; return (a % b != 0 && ((a < 0) != (b < 0))) ? q - 1 : q; };
       int64_t bmin = 0, bmax = 0;
       if (vmin <= vmax) {
-        if (vmin < gx.origin_ms - (int64_t(1) << 52) || vmax > gx.origin_ms + (int64_t(1) << 52))
-          throw Error(PQ_ERR_UNSUPPORTED, "DATE_BIN: values more than 2^52 ms away from the origin");
         bmin = floordiv(vmin - gx.origin_ms, gx.width_ms);
         bmax = floordiv(vmax - gx.origin_ms, gx.width_ms);
       }
@@ -1865,19 +1941,8 @@ void Query::run(const PqQueryDesc& d) {
     }
     key.kind = kind == DK_BOOL ? KK_BOOL : KK_DICT_LUT;
     if (key.kind == KK_BOOL) { qk[k].card = 2; continue; }
-    if (plan.cols[key.col].has_plain || plan.cols[key.col].has_delta) {
-      // Pages without a dictionary (PLAIN fallback of an overflowed dictionary, PLAIN / DELTA numerics): ensure_key interns
-      // their ROWS next to the dictionary entries; the aggregate kernel then stages the pages' ids instead of their values,
-      // so nothing else of this query may read the column's values
-      for (uint32_t l = 0; l < nleaves; l++)
-        if (plan.leaves[l].col == key.col && value_leaf(plan.leaves[l].kind))
-          throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[tcol[d.group_by[k]]].name + "' has pages without a dictionary and is also filtered on: not on the GPU path");
-      for (uint32_t a = 0; a < d.n_aggs; a++)
-        if (((plan.aggs[a].fn >= AG_SUM && plan.aggs[a].fn <= AG_AVG) || plan.aggs[a].fn >= AG_MEDIAN) && plan.aggs[a].col == key.col &&
-            !rank_min_max(plan.aggs[a]))
-          throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[tcol[d.group_by[k]]].name + "' has pages without a dictionary and is also aggregated: not on the GPU path");
-      row_keys[k] = 1;
-    }
+    // pages without a dictionary: ensure_key interns their rows (the uses this rules out were refused above)
+    if (plan.cols[key.col].has_plain || plan.cols[key.col].has_delta) row_keys[k] = 1;
     const int tc_i = shape_cols[key.col];
     table->ensure_key(tc_i, stream);
     const ColSide& cs = table->sides[tc_i];
@@ -1949,12 +2014,7 @@ void Query::run(const PqQueryDesc& d) {
       if (!rank_min_max(ag)) continue;
       const int tc_i = shape_cols[ag.col];
       if (table->columns[tc_i].kind == 0xfe && !multi) continue;   // in no file: every row NULL, nothing to rank
-      const bool row_ids = plan.cols[ag.col].has_plain || plan.cols[ag.col].has_delta;
-      if (row_ids)
-        for (uint32_t l = 0; l < nleaves; l++)
-          if (plan.leaves[l].col == ag.col && value_leaf(plan.leaves[l].kind))
-            throw Error(PQ_ERR_UNSUPPORTED, std::string(ag.fn == AG_MIN ? "MIN(" : "MAX(") + table->columns[tc_i].name +
-                                                "): the column has pages without a dictionary and is also filtered on: not on the GPU path");
+      const bool row_ids = plan.cols[ag.col].has_plain || plan.cols[ag.col].has_delta;   // (a filter on them was refused above)
       table->ensure_key(tc_i, stream);
       if (multi && !keys_agreed && unified.insert(tc_i).second) table->unify_key(tc_i, stream);
       rank_luts[a] = table->ensure_rank_luts(tc_i, multi, stream);
@@ -2093,18 +2153,8 @@ void Query::run(const PqQueryDesc& d) {
   // ---- which kernels run ----
   (void)has_null_const;   // the flat kernels evaluate SQL three-valued logic, NULL literals included
   plan.no_flat = flat_ok ? 0 : 1;
-  const uint32_t n_flat = flat_ok ? shape->n_flat : 0;
-  const uint32_t n_general = flat_ok ? shape->n_general : uint32_t(items.size());
-
-  for (uint32_t k = 0; agg_kernel && k < d.n_group_by; k++)
-    if (plan.keys[k].kind == KK_BIN && n_general)
-      throw Error(PQ_ERR_UNSUPPORTED, "DATE_BIN keys need a flat-store copy of every page the query reads: " + shape->why_general);
-  // k_scan reads a key's dictionary index of every row; the rows of pages without a dictionary have none (their ids are
-  // staged as id pages by k_flat_agg only)
-  for (uint32_t k = 0; agg_kernel && k < d.n_group_by; k++)
-    if (row_keys[k] && n_general)
-      throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY column '" + table->columns[shape_cols[plan.keys[k].col]].name +
-                                      "' has pages without a dictionary, which need a flat-store copy of every page the query reads: " + shape->why_general);
+  // (DATE_BIN keys, keys with pages without a dictionary and MIN / MAX over Utf8 / Boolean were refused above when
+  // some page has no flat-store copy)
   if (agg_kernel && plan.hashed && n_general)
     throw Error(PQ_ERR_UNSUPPORTED, "a hashed GROUP BY needs a flat-store copy of every page the query reads: " + shape->why_general);
   for (uint32_t i = 0; agg_kernel && i < plan.ndist; i++)
@@ -2113,10 +2163,6 @@ void Query::run(const PqQueryDesc& d) {
                                           ") needs a flat-store copy of every page the query reads: " + shape->why_general);
   if (agg_kernel && plan.npct && n_general)
     throw Error(PQ_ERR_UNSUPPORTED, "MEDIAN / PERCENTILE_CONT need a flat-store copy of every page the query reads: " + shape->why_general);
-  for (uint32_t a = 0; agg_kernel && n_general && a < d.n_aggs; a++)   // (a column in no file has nothing to read: k_scan takes it)
-    if ((rank_min_max(plan.aggs[a]) || bool_min_max(plan.aggs[a])) && table->columns[shape_cols[plan.aggs[a].col]].kind != 0xfe)
-      throw Error(PQ_ERR_UNSUPPORTED, std::string(plan.aggs[a].fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
-                                          ") over Utf8 / Boolean needs a flat-store copy of every page the query reads: " + shape->why_general);
   if (row_order && n_general)
     throw Error(PQ_ERR_UNSUPPORTED, "ORDER BY on a scan needs a flat-store copy of every page the query reads: " + shape->why_general);
   // ---- ORDER BY on a scan: a Utf8 term sorts by the bytewise rank of the column's GROUP BY ids (ensure_key, cached with
@@ -3069,7 +3115,7 @@ void Query::run(const PqQueryDesc& d) {
     DevBuf<unsigned long long> d_item_base, d_total, d_ids;
     std::shared_ptr<PinnedBlock> ids_block;   // selected row ordinals land in page-locked memory, batches alias it
     unsigned long long n_ids = 0, total = 0;
-    d_total.alloc(1, stream);
+    d_total.alloc(2, stream);   // the selected rows; under PQ_QUERY_ALLREDUCE also the ranks that met a corrupt page
     d_item_base.alloc(std::max<size_t>(items.size(), 1), stream);
     if (!items.empty()) {
       k_item_prefix<<<1, 1024, 0, stream>>>(d_item_counts.p, uint32_t(items.size()), d_item_base.p, d_total.p);
@@ -3361,14 +3407,23 @@ void Query::run(const PqQueryDesc& d) {
     PQB_CUDA(cudaEventRecord(t_all.b, stream));
     PQB_CUDA(cudaStreamSynchronize(stream));
     mark("results on host");
-    if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
     metrics.rows_selected = total;
+    unsigned long long corrupt_ranks = 0;
+    if (has_aggs && allreduce) {
+      // SELECT COUNT(*) under PQ_QUERY_ALLREDUCE: the total's all-reduce also counts the ranks that met a corrupt page,
+      // so that every rank throws, not only the ones that met it
+      const unsigned long long bad = h_counters[1] ? 1ull : 0ull;
+      PQB_CUDA(cudaMemcpyAsync(d_total.p + 1, &bad, 8, cudaMemcpyHostToDevice, stream));
+      comm_allreduce_u64(d_total.p, 2, 0, stream);
+      unsigned long long w[2];
+      PQB_CUDA(cudaMemcpyAsync(w, d_total.p, 16, cudaMemcpyDeviceToHost, stream));
+      PQB_CUDA(cudaStreamSynchronize(stream));
+      total = w[0];
+      corrupt_ranks = w[1];
+    }
+    if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
+    if (corrupt_ranks) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device of " + std::to_string(corrupt_ranks) + " other rank(s)");
     if (has_aggs) {  // SELECT COUNT(*) [, COUNT(*)...] WHERE ...
-      if (allreduce) {
-        comm_allreduce_u64(d_total.p, 1, 0, stream);
-        PQB_CUDA(cudaMemcpyAsync(&total, d_total.p, 8, cudaMemcpyDeviceToHost, stream));
-        PQB_CUDA(cudaStreamSynchronize(stream));
-      }
       metrics.groups_total = 1;
       // one row, ordered trivially; LIMIT 0 keeps none, and a window keeps it when its rank range holds rn = 1
       const bool win_drops = win && !(win->offset == 0 && win->fetch != 0);

@@ -20,7 +20,7 @@ def main():
     from parseable_b200 import _lib as L
     from parseable_b200.query import StandardTableProvider, col, count_star, sum_, min_, max_, avg, count
     lib = L.load()
-    dev = (C.c_int * 1)(rank)
+    dev = (C.c_int * 1)(int(os.environ.get("PQB_RANK_DEVICE", rank)))   # PQB_RANK_DEVICE: every rank on one device
     assert lib.pq_init(dev, 1) == 0, lib.pq_last_error(None)
     if rank == 0:
         buf = C.create_string_buffer(L.PQ_COMM_ID_BYTES)

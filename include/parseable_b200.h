@@ -247,7 +247,9 @@ typedef struct {
  * order is file order, then row order.  For an aggregate it is ascending group slot, and every rank of an all-reduced
  * query returns the same rows.  Slot order follows the group ids a table numbers when it is opened (a resident table
  * keeps them); under a hashed GROUP BY (a key space wider than 2^26) the slots are hash-table cells and their order, so
- * the order of tied rows, may differ from one query to the next.
+ * the order of tied rows, may differ from one query to the next.  Except under PQ_QUERY_ALLREDUCE: there the ranks'
+ * tables are merged into ascending wide group id (the mixed-radix id of the key tuple in the numbering the ranks agreed
+ * on), so tied rows come out in the same order on every rank, and on every run over the same resident tables.
  * Paths (all stable on that order): <= 4096 rows one CTA sorts them; a key that packs into one 64-bit word with
  * LIMIT <= 4096 takes a radix select of the LIMIT-th key; anything else an LSD radix sort. */
 typedef enum { PQ_ORDER_KEY = 0, PQ_ORDER_AGG = 1, PQ_ORDER_COLUMN = 2 } PqOrderTarget;
@@ -271,7 +273,8 @@ typedef struct {
  * payloads), Utf8 by bytes, a DATE_BIN key by bin.
  * Ranking: row_number rn counts 1, 2, ... within a partition in the order of the order_by terms; ties keep the order
  * the query has without a window (as ORDER BY states above: slot order, or file then row order), and with no order_by
- * terms that order is the ranking.  Under a hashed GROUP BY the order of tied rows may differ from one query to the next.
+ * terms that order is the ranking.  Under a hashed GROUP BY the order of tied rows may differ from one query to the next
+ * (not under PQ_QUERY_ALLREDUCE: see ORDER BY above).
  * Output: the rows with offset < rn <= offset + fetch (fetch < 0: no upper bound), ordered by the partition terms and
  * then the window's order; `limit` (>= 0) then keeps the first `limit` of them (the outer LIMIT), for aggregates too.
  * PQ_WINDOW_ROW_NUMBER appends an Int64 column "row_number", PQ_WINDOW_PARTITION_ROWS an Int64 column "partition_rows"
@@ -363,7 +366,19 @@ typedef struct {
 } PqQueryDesc;
 
 #define PQ_QUERY_COUNT_ONLY 1u    /* filter scan: only rows_selected is wanted, emit no batches */
-#define PQ_QUERY_ALLREDUCE 2u     /* aggregate: all-reduce partial tables over the pq_comm communicator */
+/* PQ_QUERY_ALLREDUCE, aggregate: every rank returns the whole table's groups.  A key space of up to 2^26 group ids:
+ * the ranks all-reduce their dense partial tables.  A wider one (a hashed GROUP BY, at any number of ranks, one
+ * included): every rank lists the groups its hash table holds, the lists are all-gathered and merged on the device in
+ * rank order.  The merge combines the cells as the all-reduce does: wrapping add (the row count, COUNT, non-null
+ * counters, Int64 SUM), f64 add in rank order ((r0 + r1) + r2 ... for Float64 SUM / AVG), signed min / max (MIN / MAX
+ * on their cell encodings); its rows come out in ascending wide group id.  Refused alike by every rank:
+ *   PQ_ERR_UNSUPPORTED  more than 2^26 merged groups, or a rank's hash table ran full (the message names the rank); a
+ *                       rank with pages that have no flat-store copy (named likewise); the hashed table would exceed
+ *                       24 GiB for the rows of every rank
+ *   PQ_ERR_CORRUPT      a rank met a corrupt page (named)
+ *   PQ_ERR_OOM          the exchange and merge buffers exceed half the smallest free HBM of any rank (named)
+ * COUNT(DISTINCT), MEDIAN and PERCENTILE_CONT are refused under this flag. */
+#define PQ_QUERY_ALLREDUCE 2u
 #define PQ_QUERY_EMIT_ROW_IDS 4u  /* filter scan: append a UInt64 `__row_id` column (global row ordinal) */
 
 typedef struct {
@@ -381,7 +396,9 @@ typedef struct {
   uint64_t groups;          /* output groups (aggregate queries) */
   double host_ms;           /* wall time of pq_query_open (planning + uploads + device work + result copy) */
   double upload_ms;         /* of which: footer parse, page walk and H2D of the column chunks (file-list queries) */
-  double allreduce_ms;      /* CUDA-event time of the NCCL all-reduce of the partial tables (PQ_QUERY_ALLREDUCE) */
+  double allreduce_ms;      /* CUDA-event time of the NCCL all-reduce of the partial tables (PQ_QUERY_ALLREDUCE); a
+                               hashed GROUP BY: its exchange, both all-gathers and the merge kernels, without the one
+                               host round trip between them */
   uint64_t groups_total;    /* aggregate queries: groups before the ORDER BY ... LIMIT cut (== groups without ORDER BY) */
   double order_ms;          /* CUDA-event time of the ORDER BY kernels, without the one host round trip between them
                                (0 without ORDER BY) */

@@ -32,6 +32,7 @@
 #include "egress_kernels.cuh"
 #include "order_kernels.cuh"
 #include "percentile_kernels.cuh"
+#include "hash_merge.cuh"
 #include "regex_compile.hpp"
 
 namespace pqb {
@@ -900,6 +901,180 @@ struct OrderBufs {
   }
 };
 
+// LSD radix sort of n rows by 64-bit keys (key[row]), 8-bit digits: per pass tile histograms, one scan of the digit x
+// tile matrix and a stable scatter.  ORDER BY sorts its packed words with it, the merge of a hashed GROUP BY under
+// PQ_QUERY_ALLREDUCE its wide group ids.  Every buffer is allocated by the constructor, so a caller can time sort()
+// as device work only.
+struct RadixSort {
+  uint32_t n, ntiles;
+  DevBuf<uint32_t> hist, ia, ib;
+  DevBuf<unsigned long long> base, total;
+  RadixSort(uint32_t rows, cudaStream_t stream) : n(rows), ntiles(uint32_t((uint64_t(rows) + kRadixTile - 1) / kRadixTile)) {
+    hist.alloc(size_t(256) * ntiles, stream);
+    base.alloc(size_t(256) * ntiles, stream);
+    total.alloc(1, stream);
+    ia.alloc(n, stream);
+    ib.alloc(n, stream);
+  }
+  // one pass per digit of bits [lo, hi) of key[row], the rows taken in the order `cur` (nullptr: 0 .. n - 1).  Stable,
+  // so a sort by a more significant key after this one keeps this order among its ties.  Returns the sorted rows (`cur`
+  // itself when there are no bits)
+  const uint32_t* sort(const unsigned long long* key, const uint32_t* cur, uint32_t lo, uint32_t hi, cudaStream_t stream, uint64_t& launches) {
+    for (uint32_t sh = lo; sh < hi; sh += 8) {
+      uint32_t* out = cur == ia.p ? ib.p : ia.p;
+      k_radix_hist<<<ntiles, kRadixThreads, 0, stream>>>(key, cur, n, sh, hist.p, ntiles);
+      k_item_prefix<<<1, 1024, 0, stream>>>(hist.p, 256 * ntiles, base.p, total.p);
+      k_radix_scatter<<<ntiles, kRadixThreads, 0, stream>>>(key, cur, n, sh, base.p, ntiles, out);
+      launches += 3;
+      cur = out;
+    }
+    return cur;
+  }
+};
+
+// A hashed GROUP BY under PQ_QUERY_ALLREDUCE (hash_merge.cuh): every rank's groups gathered and merged into one table of
+// the layout k_flat_agg leaves, which then replaces acc / hkeys, so the result tail runs on it unchanged.  Its capacity
+// (plan.nslots) is the groups every rank listed; the G merged groups take the first slots in ascending wide id, the slots
+// past them hold count 0.  One host round trip, on the exchange records: any rank's full table or corrupt page, and an
+// exchange above half the smallest free HBM of any rank, are refused by every rank alike before the cells travel.
+struct MergeRun {
+  Timer t_rec, t_merge, t_sort, t_fold;
+  uint64_t listed = 0, e_max = 0, total = 0;
+
+  uint64_t run(DevPlan& plan, uint32_t cells, uint64_t key_space, uint64_t out_cap, DevBuf<unsigned long long>& acc,
+               DevBuf<unsigned long long>& hkeys, const unsigned long long* counters, cudaStream_t stream, PqMetrics& m) {
+    const uint32_t nr = uint32_t(comm_nranks()), me = uint32_t(comm_rank());
+    // ---- this rank's groups (the cells with rows, in slot order) and its exchange record ----
+    const uint32_t ntiles = (plan.nslots + kSlotTile - 1) / kSlotTile;
+    DevBuf<uint32_t> tile_counts, out_slot;
+    DevBuf<unsigned long long> tile_base, d_listed, rec, recs;
+    tile_counts.alloc(ntiles, stream);
+    tile_base.alloc(ntiles, stream);
+    out_slot.alloc(out_cap, stream);
+    d_listed.alloc(1, stream);
+    rec.alloc(kMergeRecWords, stream);
+    recs.alloc(size_t(kMergeRecWords) * nr, stream);
+    size_t free_b = 0, total_b = 0;
+    PQB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    uint64_t budget = free_b / 2;
+    if (const char* e = getenv("PQB_MERGE_BUDGET")) budget = std::min<uint64_t>(budget, strtoull(e, nullptr, 10));   // test switch: bytes
+    PQB_CUDA(cudaEventRecord(t_rec.a, stream));
+    k_slot_tile_counts<<<ntiles, 256, 0, stream>>>(acc.p, plan.nslots, tile_counts.p, nullptr);
+    k_item_prefix<<<1, 1024, 0, stream>>>(tile_counts.p, ntiles, tile_base.p, d_listed.p);
+    k_slot_compact<<<ntiles, 256, 0, stream>>>(acc.p, plan.nslots, tile_base.p, out_slot.p, nullptr);
+    k_merge_record<<<1, 1, 0, stream>>>(rec.p, d_listed.p, counters, budget);
+    PQB_CUDA(cudaGetLastError());
+    comm_allgather_bytes(rec.p, recs.p, kMergeRecWords * 8, stream);
+    PQB_CUDA(cudaEventRecord(t_rec.b, stream));
+    std::vector<unsigned long long> h(size_t(kMergeRecWords) * nr);
+    PQB_CUDA(cudaMemcpyAsync(h.data(), recs.p, h.size() * 8, cudaMemcpyDeviceToHost, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+    m.d2h_bytes += h.size() * 8;
+    // ---- the verdicts: every rank holds the same records ----
+    std::vector<unsigned long long> pre(nr + 1, 0);
+    int full = -1, corrupt = -1;
+    uint32_t low = 0;   // the rank with the smallest budget
+    for (uint32_t r = 0; r < nr; r++) {
+      const unsigned long long* x = &h[size_t(kMergeRecWords) * r];
+      pre[r + 1] = pre[r] + x[kMergeListed];
+      e_max = std::max<uint64_t>(e_max, x[kMergeListed]);
+      if (x[kMergeFull] && full < 0) full = int(r);
+      if (x[kMergeCorrupt] && corrupt < 0) corrupt = int(r);
+      if (x[kMergeBudget] < h[size_t(kMergeRecWords) * low + kMergeBudget]) low = r;
+    }
+    listed = h[size_t(kMergeRecWords) * me + kMergeListed];
+    total = pre[nr];
+    if (full >= 0)
+      throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: more distinct groups than the hashed accumulator table holds (2^26), on rank " + std::to_string(full));
+    if (corrupt >= 0)
+      throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device of rank " + std::to_string(corrupt) + " (code " +
+                                      std::to_string(h[size_t(kMergeRecWords) * corrupt + kMergeCorrupt]) + ")");
+    if (total > 0xffffffffull) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: the ranks' hashed tables list more than 2^32 - 1 groups together");
+    // send and receive blocks, the sort's keys and its buffers, the merged table
+    const uint64_t need = 8 * (1 + uint64_t(cells)) * e_max * (nr + 1) + total * (8 + 8 + 8 * (1 + uint64_t(cells))) +
+                          (total / kRadixTile + 1) * 256 * 12;
+    const uint64_t low_budget = h[size_t(kMergeRecWords) * low + kMergeBudget];
+    if (need > low_budget)
+      throw Error(PQ_ERR_OOM, "GROUP BY: merging the ranks' hashed tables needs " + std::to_string(need >> 20) +
+                                  " MiB of HBM, more than its budget on rank " + std::to_string(low) + ": half the free HBM (" +
+                                  std::to_string(low_budget >> 20) + " MiB)");
+    // ---- the cells travel, then the merge ----
+    const uint32_t n = uint32_t(total), cap = std::max<uint32_t>(n, 1), mt = (n + kSlotTile - 1) / kSlotTile;
+    const uint64_t block = (1 + uint64_t(cells)) * e_max;
+    DevBuf<unsigned long long> send, recv, ids, d_pre, macc, mwide, mbase, groups;
+    DevBuf<uint32_t> mtiles;
+    send.alloc(block, stream);
+    recv.alloc(block * nr, stream);
+    ids.alloc(n, stream);
+    d_pre.upload(pre, stream);
+    m.h2d_bytes += pre.size() * 8;
+    macc.alloc(size_t(cells) * cap, stream);
+    mwide.alloc(cap, stream);
+    mtiles.alloc(mt, stream);
+    mbase.alloc(mt, stream);
+    groups.alloc(1, stream);
+    RadixSort rs(n, stream);
+    PQB_CUDA(cudaMemsetAsync(macc.p, 0, size_t(cap) * 8, stream));   // the count plane: slots past G hold no group
+    uint64_t launches = 4;
+    PQB_CUDA(cudaEventRecord(t_merge.a, stream));
+    if (listed) {
+      k_hash_pack<<<uint32_t(std::min<uint64_t>(2048, (listed + 255) / 256)), 256, 0, stream>>>(acc.p, hkeys.p, plan.nslots, cells, out_slot.p,
+                                                                                             uint32_t(listed), e_max, send.p);
+      launches++;
+    }
+    if (e_max) comm_allgather_bytes(send.p, recv.p, block * 8, stream);   // e_max is the same on every rank
+    HashMergeArgs a{};
+    a.recv = recv.p;
+    a.pre = d_pre.p;
+    a.ids = ids.p;
+    a.acc = macc.p;
+    a.wide = mwide.p;
+    a.e_max = e_max;
+    a.nranks = nr;
+    a.n = n;
+    a.cap = cap;
+    a.cells = cells;
+    a.n_acc = plan.n_acc;
+    std::memcpy(a.acc_init, plan.acc_init, sizeof(a.acc_init));
+    if (n) k_merge_list<<<std::min<uint32_t>(2048, (n + 255) / 256), 256, 0, stream>>>(a, ids.p);
+    PQB_CUDA(cudaEventRecord(t_sort.a, stream));
+    if (n) a.sorted = rs.sort(ids.p, nullptr, 0, 64 - __builtin_clzll(key_space - 1), stream, launches);   // wide ids < key_space
+    PQB_CUDA(cudaEventRecord(t_sort.b, stream));
+    PQB_CUDA(cudaEventRecord(t_fold.a, stream));
+    if (n) {
+      k_merge_heads<<<mt, 256, 0, stream>>>(a, mtiles.p);
+      k_item_prefix<<<1, 1024, 0, stream>>>(mtiles.p, mt, mbase.p, groups.p);
+      a.tile_base = mbase.p;
+      k_merge_fold<<<mt, 256, 0, stream>>>(a);
+      launches += 4;
+    }
+    PQB_CUDA(cudaEventRecord(t_fold.b, stream));
+    PQB_CUDA(cudaEventRecord(t_merge.b, stream));
+    PQB_CUDA(cudaGetLastError());
+    std::swap(acc.p, macc.p);   // the rank's own table is freed with macc
+    std::swap(acc.n, macc.n);
+    std::swap(hkeys.p, mwide.p);
+    std::swap(hkeys.n, mwide.n);
+    plan.nslots = cap;
+    return launches;
+  }
+
+  // after the caller's stream synchronise: allreduce_ms (the exchange, the all-gather and the merge kernels, without the
+  // round trip between them), and with PQB_VERBOSE the sizes and the merge kernels' time
+  void report(bool verbose, uint32_t groups, PqMetrics& m) {
+    float rec_ms = 0, merge_ms = 0, sort_ms = 0, fold_ms = 0;
+    cudaEventElapsedTime(&rec_ms, t_rec.a, t_rec.b);
+    cudaEventElapsedTime(&merge_ms, t_merge.a, t_merge.b);
+    cudaEventElapsedTime(&sort_ms, t_sort.a, t_sort.b);
+    cudaEventElapsedTime(&fold_ms, t_fold.a, t_fold.b);
+    m.allreduce_ms = double(rec_ms) + double(merge_ms);
+    if (verbose)
+      fprintf(stderr, "[pqb] hashed merge: E_r %llu, E_max %llu, listed by all ranks %llu, G %u, exchange %.3f ms, merge %.3f ms "
+              "(sort %.3f ms, fold %.3f ms)\n", (unsigned long long)listed, (unsigned long long)e_max, (unsigned long long)total,
+              groups, rec_ms, merge_ms, sort_ms, fold_ms);
+  }
+};
+
 // ORDER BY [LIMIT] of n encoded rows (groups or selected scan rows), after the caller's encode step.  One round trip: the
 // value ranges the pack plan is sized from.  Then `kept` becomes the first `keep` rows in the query's order, as their
 // entries of `rows` (nullptr: the row indices themselves); it stays empty when every term is one value for every row
@@ -971,30 +1146,14 @@ uint64_t order_sort(const OrderBufs& ob, uint32_t nterms, uint32_t n, const uint
     k_order_cta<<<1, 1024, smem, stream>>>(words.p, n, 1, cand.p, keep, keep, rows, kept.p);
     launches += 4;
   } else {
-    const uint32_t ntiles = uint32_t((uint64_t(n) + kRadixTile - 1) / kRadixTile);
-    DevBuf<uint32_t> hist, ia, ib;
-    DevBuf<unsigned long long> base, total;
-    hist.alloc(size_t(256) * ntiles, stream);
-    base.alloc(size_t(256) * ntiles, stream);
-    total.alloc(1, stream);
-    ia.alloc(n, stream);
-    ib.alloc(n, stream);
+    RadixSort rs(n, stream);
     PQB_CUDA(cudaEventRecord(t_sort.a, stream));
     k_order_pack<<<grid_n, 256, 0, stream>>>(pk, ob.vals.p, ob.nulls.p, n, words.p);
     launches++;
     const uint32_t* cur = nullptr;   // the first pass reads the rows in row order
-    uint32_t* out = ia.p;
     for (int w = int(pk.nwords) - 1; w >= 0; w--) {   // least significant word first
-      const unsigned long long* key = words.p + size_t(w) * n;
       const uint32_t used = std::min<uint32_t>(64, pk.total_bits - 64u * uint32_t(w));   // MSB-first: the low bits of the last word are empty
-      for (uint32_t sh = 64 - used; sh < 64; sh += 8) {
-        k_radix_hist<<<ntiles, kRadixThreads, 0, stream>>>(key, cur, n, sh, hist.p, ntiles);
-        k_item_prefix<<<1, 1024, 0, stream>>>(hist.p, 256 * ntiles, base.p, total.p);
-        k_radix_scatter<<<ntiles, kRadixThreads, 0, stream>>>(key, cur, n, sh, base.p, ntiles, out);
-        launches += 3;
-        cur = out;
-        out = out == ia.p ? ib.p : ia.p;
-      }
+      cur = rs.sort(words.p + size_t(w) * n, cur, 64 - used, 64, stream, launches);
     }
     k_order_gather<<<(keep + 255) / 256, 256, 0, stream>>>(cur, keep, rows, kept.p);
     launches++;
@@ -1821,14 +1980,24 @@ void Query::run(const PqQueryDesc& d) {
   // table): ONE collective and one round trip per query for both agreements.  Its last two words are the number of ranks
   // that refuse the query (then every rank refuses) and a mask of the refusing ranks below 63 (bit r for rank r; the bits
   // are distinct, so their sum is their union), which names one of them.  A COUNT(*)-only query runs it for the refusals
-  // alone: its total's all-reduce comes after the scan.
+  // alone: its total's all-reduce comes after the scan.  Two more words do the same for the ranks with items that have no
+  // flat-store copy, which only a hashed GROUP BY refuses (whether it is hashed is known once the key cards are agreed),
+  // and the last one sums the rows of every rank's live row groups, which bound the hashed table's size alike on every rank.
   bool keys_agreed = true;
+  uint64_t live_rows = 0;
+  for (uint32_t g = 0; g < nrg_table; g++) if (rg_live[g]) live_rows += table->row_groups[g].num_rows;
+  uint64_t rows_all = live_rows, general_ranks = n_general ? 1 : 0, general_mask = 0;
   if (agree) {
-    std::vector<unsigned long long> f(3 + ncols, 0ull);
+    std::vector<unsigned long long> f(6 + ncols, 0ull);
     if (!refusal.empty()) {
       f[1 + ncols] = 1;
       if (comm_rank() < 63) f[2 + ncols] = 1ull << comm_rank();
     }
+    if (n_general) {
+      f[3 + ncols] = 1;
+      if (comm_rank() < 63) f[4 + ncols] = 1ull << comm_rank();
+    }
+    f[5 + ncols] = live_rows;
     for (uint32_t k = 0; k < d.n_group_by; k++) {
       if (d.group_exprs && d.group_exprs[k].kind == PQ_KEY_DATE_BIN) continue;
       const uint32_t s = uint32_t(slot_of[d.group_by[k]]);
@@ -1852,6 +2021,9 @@ void Query::run(const PqQueryDesc& d) {
       throw Error(PQ_ERR_UNSUPPORTED, "refused on " + (f[2 + ncols] ? "rank " + std::to_string(__builtin_ctzll(f[2 + ncols]))
                                                                     : std::to_string(f[1 + ncols]) + " ranks") +
                                           " (its shard holds pages or footers this query cannot take on the GPU path)");
+    general_ranks = f[3 + ncols];
+    general_mask = f[4 + ncols];
+    rows_all = f[5 + ncols];
     if (multi) {
       keys_agreed = f[0] == 0;
       for (uint32_t s = 0; s < ncols; s++) col_has_nulls[s] = f[1 + s] != 0;
@@ -2070,17 +2242,28 @@ void Query::run(const PqQueryDesc& d) {
   // A key space wider than the dense table (2^26 slots): the groups that actually occur are found through a hash
   // table on the wide id (DataFusion's GroupValues hashes the key tuple, SURVEY §8 a12); its capacity is twice the
   // groups that can occur (<= rows scanned, <= combinations), so it never runs full below the 2^27-slot ceiling.
+  // Under PQ_QUERY_ALLREDUCE every rank's table is merged after the scan (hash_merge.cuh), and every refusal here is
+  // decided from what every rank holds: the summed rows, and the ranks with items that have no flat-store copy.
   const uint64_t key_space = nslots64;   // group-id combinations (the dense table, or the groups a hashed table may meet)
   plan.hashed = 0;
   plan.hmask = 0;
   if (nslots64 > (1ull << 26)) {
-    if (allreduce || multi)
-      throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY key space too large for the dense accumulator table the ranks all-reduce (hashed tables are per rank)");
-    uint64_t rows_bound = 0;
-    for (uint32_t g = 0; g < nrg_table; g++) if (rg_live[g]) rows_bound += table->row_groups[g].num_rows;
-    uint64_t cap = 1024;
-    while (cap < 2 * std::min<uint64_t>(nslots64, std::max<uint64_t>(rows_bound, 1)) && cap < (1ull << 27)) cap <<= 1;
-    if (cap * (1 + plan.n_acc + plan.n_nn) * 8 > (24ull << 30)) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: the hashed accumulator table would exceed 24 GiB");
+    auto table_cap = [&](uint64_t rows) {
+      uint64_t cap = 1024;
+      while (cap < 2 * std::min<uint64_t>(nslots64, std::max<uint64_t>(rows, 1)) && cap < (1ull << 27)) cap <<= 1;
+      return cap;
+    };
+    if (table_cap(rows_all) * (1 + plan.n_acc + plan.n_nn) * 8 > (24ull << 30))
+      throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: the hashed accumulator table would exceed 24 GiB");
+    if (agg_kernel && general_ranks) {
+      const std::string why = "a hashed GROUP BY needs a flat-store copy of every page the query reads";
+      if (n_general) throw Error(PQ_ERR_UNSUPPORTED, why + ": " + shape->why_general);
+      throw Error(PQ_ERR_UNSUPPORTED, why + ": refused on " + (general_mask ? "rank " + std::to_string(__builtin_ctzll(general_mask))
+                                                                            : std::to_string(general_ranks) + " ranks"));
+    }
+    uint64_t cap = table_cap(live_rows);
+    if (const char* e = getenv("PQB_HASH_SLOTS"))   // test switch: a smaller table on this rank (a power of two, >= 64)
+      while (cap > 64 && cap > strtoull(e, nullptr, 10)) cap >>= 1;
     plan.hashed = 1;
     plan.hmask = uint32_t(cap - 1);
     nslots64 = cap;
@@ -2153,10 +2336,8 @@ void Query::run(const PqQueryDesc& d) {
   // ---- which kernels run ----
   (void)has_null_const;   // the flat kernels evaluate SQL three-valued logic, NULL literals included
   plan.no_flat = flat_ok ? 0 : 1;
-  // (DATE_BIN keys, keys with pages without a dictionary and MIN / MAX over Utf8 / Boolean were refused above when
-  // some page has no flat-store copy)
-  if (agg_kernel && plan.hashed && n_general)
-    throw Error(PQ_ERR_UNSUPPORTED, "a hashed GROUP BY needs a flat-store copy of every page the query reads: " + shape->why_general);
+  // (DATE_BIN keys, keys with pages without a dictionary, MIN / MAX over Utf8 / Boolean and hashed GROUP BYs were
+  // refused above when some page has no flat-store copy)
   for (uint32_t i = 0; agg_kernel && i < plan.ndist; i++)
     if (n_general)
       throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT " + table->columns[shape_cols[plan.dist[i].col]].name +
@@ -2650,7 +2831,12 @@ void Query::run(const PqQueryDesc& d) {
     // multi-GPU: the partial tables meet in ONE grouped all-reduce (SURVEY §8e): one NCCL launch,
     // per array the reduction its aggregate needs
     Timer t_ar;
-    if (allreduce) {
+    std::unique_ptr<MergeRun> merge;   // a hashed GROUP BY: every rank's listed groups gathered and merged instead
+    if (allreduce && plan.hashed) {
+      merge = std::make_unique<MergeRun>();
+      launches += merge->run(plan, cells, key_space, std::min<uint64_t>(plan.nslots, std::max<uint64_t>(metrics.rows_scanned, 1)),
+                             d_acc, d_hkeys, d_counters.p, stream, metrics);
+    } else if (allreduce) {
       PQB_CUDA(cudaEventRecord(t_ar.a, stream));
       comm_group_begin();
       comm_allreduce_u64(d_acc.p, plan.nslots, 0, stream);
@@ -2896,6 +3082,10 @@ void Query::run(const PqQueryDesc& d) {
       if (plan.npct) std::memcpy(pct_count.data(), small.p + 16 + sizeof(h_counters), plan.npct * 4);
     }
     metrics.d2h_bytes += 16 + sizeof(h_counters) + plan.npct * 4;
+    if (merge) {   // G is the same on every rank, and no collective follows: every rank throws alike
+      merge->report(verbose, uint32_t(totals[0]), metrics);
+      if (totals[0] > (1ull << 26)) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: more distinct groups than the hashed accumulator table holds (2^26)");
+    }
     if (plan.hashed && h_counters[1] == 100) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: more distinct groups than the hashed accumulator table holds (2^26)");
     if (plan.ndist && h_counters[1] == kDistinctFull) throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT): more distinct (group, value) pairs than the pair set holds (2^27)");
     if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
@@ -2906,7 +3096,7 @@ void Query::run(const PqQueryDesc& d) {
       if (shape->groups_hint.size() >= 64 && !shape->groups_hint.count(tail_key)) shape->groups_hint.clear();   // a bound, not an LRU
       shape->groups_hint[tail_key] = n_out;
     }
-    if (allreduce) { float ms = 0; cudaEventElapsedTime(&ms, t_ar.a, t_ar.b); metrics.allreduce_ms = ms; }
+    if (allreduce && !merge) { float ms = 0; cudaEventElapsedTime(&ms, t_ar.a, t_ar.b); metrics.allreduce_ms = ms; }
     static const char* fn_names[] = {"count(*)", "count", "sum", "min", "max", "avg", "count(distinct", "median", "percentile_cont"};
     auto agg_name = [&](uint32_t a) {
       const DevAgg& ag = plan.aggs[a];

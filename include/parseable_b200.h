@@ -232,7 +232,8 @@ typedef struct {
  * and need a LIMIT: limit < 0 returns PQ_ERR_UNSUPPORTED.  The result is the first `limit` rows of the ordered
  * selection (LIMIT 0: no rows); the __row_id column of PQ_QUERY_EMIT_ROW_IDS follows the order, and without a
  * projection the result is the selected __row_ids in order.  rows_selected counts the rows before the cut.  Under
- * row-group or file sharding every shard orders and cuts its own selection; merging the shards' rows is the caller's.
+ * row-group or file sharding every shard orders and cuts its own selection, unless PQ_QUERY_ALLGATHER merges the
+ * shards' rows (row-group sharding of one file list only): then every rank returns the whole table's first rows.
  * A PQ_ORDER_KEY / PQ_ORDER_AGG term on a scan returns PQ_ERR_UNSUPPORTED; ORDER BY with PQ_QUERY_COUNT_ONLY
  * PQ_ERR_INVALID_ARG; more than 2^32 - 1 selected rows, or pages without a flat-store copy, PQ_ERR_UNSUPPORTED.
  * Every query: an out-of-range index or an unknown target returns PQ_ERR_INVALID_ARG, more than 8 terms
@@ -282,7 +283,7 @@ typedef struct {
  * or after a scan's projection and __row_id.  Neither is ever NULL.
  * Scans: a window needs no `limit`; the caps of a scan ORDER BY hold (2^32 - 1 selected rows, 2^31 projected rows, a
  * flat-store copy of every page read).  Under row-group or file sharding every shard ranks and cuts its own selection;
- * merging the shards' rows is the caller's.  Aggregates: the window runs after the all-reduce (every rank of a
+ * merging the shards' rows is the caller's (PQ_QUERY_ALLGATHER refuses a window).  Aggregates: the window runs after the all-reduce (every rank of a
  * PQ_QUERY_ALLREDUCE query returns the same rows), and takes every aggregate ORDER BY takes as a term.
  * rows_selected and groups_total count the rows before any cut; the window's kernels count into order_ms and
  * kernel_launches.  Errors: offset < 0, unknown flags, a bad term index or target, or a window with PQ_QUERY_COUNT_ONLY
@@ -380,6 +381,29 @@ typedef struct {
  * COUNT(DISTINCT), MEDIAN and PERCENTILE_CONT are refused under this flag. */
 #define PQ_QUERY_ALLREDUCE 2u
 #define PQ_QUERY_EMIT_ROW_IDS 4u  /* filter scan: append a UInt64 `__row_id` column (global row ordinal) */
+/* PQ_QUERY_ALLGATHER, a filter / projection scan with ORDER BY (PQ_ORDER_COLUMN terms) and limit >= 0, with or without
+ * a projection and PQ_QUERY_EMIT_ROW_IDS, over a table that every rank opened from the SAME file list and shards by row
+ * group (shard_count = the communicator's ranks, shard_index = the rank; a resident table opened so, or a file-list
+ * query with those shard_* fields): every rank returns the first `limit` rows of the WHOLE table's ordered selection,
+ * bit for bit and in the order one rank returns them for the same query over the unsharded list (ties in global
+ * __row_id order: file order, then row order); rows_selected is the whole table's selected total on every rank.
+ * __row_id is the row's ordinal over the file list the table was opened with: under file sharding (each rank opening
+ * its own files) every rank's ordinals start at 0 and would collide, so the flag refuses that layout.
+ * Each rank orders its own selection and keeps its first `limit` rows; one all-gather hands every rank those rows'
+ * encoded terms and global row ids, every rank orders the union alike, each output row is projected by the rank that
+ * holds it and the ranks' result blocks are summed (every byte is written by one rank only).  Utf8 terms sort by their
+ * rank in the numbering the ranks agree on (as GROUP BY keys under PQ_QUERY_ALLREDUCE).  With one rank the result is
+ * the one without the flag.
+ * Errors: without pq_comm_init_rank, on an aggregate query or with PQ_QUERY_COUNT_ONLY PQ_ERR_INVALID_ARG; without
+ * ORDER BY or with a window PQ_ERR_UNSUPPORTED.  Refused alike by every rank, the message naming the rank:
+ *   PQ_ERR_UNSUPPORTED  a table not sharded by row group over the communicator (shard_count != ranks or
+ *                       shard_index != rank), or ranks whose file lists hold different numbers of rows; a rank's shard
+ *                       holds pages this scan cannot take (found before the scan: pages without a flat-store copy, ...);
+ *                       more than 2^32 - 1 selected rows on a rank; ranks x the most rows any rank keeps past
+ *                       2^32 - 1; more than 2^31 output rows; projected strings above 2 GiB
+ *   PQ_ERR_CORRUPT      a rank met a corrupt page
+ *   PQ_ERR_OOM          a rank's own sort and the exchange and merge buffers exceed half that rank's free HBM */
+#define PQ_QUERY_ALLGATHER 8u
 
 typedef struct {
   uint64_t bytes_scanned;   /* compressed bytes of the column chunks read (plan metric "bytes_scanned") */
@@ -398,7 +422,9 @@ typedef struct {
   double upload_ms;         /* of which: footer parse, page walk and H2D of the column chunks (file-list queries) */
   double allreduce_ms;      /* CUDA-event time of the NCCL all-reduce of the partial tables (PQ_QUERY_ALLREDUCE); a
                                hashed GROUP BY: its exchange, both all-gathers and the merge kernels, without the one
-                               host round trip between them */
+                               host round trip between them.  A scan under PQ_QUERY_ALLGATHER: its exchange record,
+                               the candidates' all-gather, the merge kernels and sort, the projection by owner and
+                               the reductions of the result block, without the host round trips between them */
   uint64_t groups_total;    /* aggregate queries: groups before the ORDER BY ... LIMIT cut (== groups without ORDER BY) */
   double order_ms;          /* CUDA-event time of the ORDER BY kernels, without the one host round trip between them
                                (0 without ORDER BY) */

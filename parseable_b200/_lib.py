@@ -26,7 +26,7 @@ PQ_LIKE_NEGATED, PQ_LIKE_CASE_INSENSITIVE = 1, 2
 PQ_REGEX_NEGATED, PQ_REGEX_CASE_INSENSITIVE = 1, 2
 (PQ_AGG_COUNT_STAR, PQ_AGG_COUNT, PQ_AGG_SUM, PQ_AGG_MIN, PQ_AGG_MAX, PQ_AGG_AVG, PQ_AGG_COUNT_DISTINCT, PQ_AGG_MEDIAN,
  PQ_AGG_PERCENTILE_CONT) = range(9)
-PQ_QUERY_COUNT_ONLY, PQ_QUERY_ALLREDUCE, PQ_QUERY_EMIT_ROW_IDS = 1, 2, 4
+PQ_QUERY_COUNT_ONLY, PQ_QUERY_ALLREDUCE, PQ_QUERY_EMIT_ROW_IDS, PQ_QUERY_ALLGATHER = 1, 2, 4, 8
 PQ_JSON_LINES = 1
 PQ_COMM_ID_BYTES = 128
 

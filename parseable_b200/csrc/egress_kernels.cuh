@@ -437,11 +437,21 @@ __global__ void __launch_bounds__(256) k_project_rows(const __grid_constant__ Pr
   project_row(f, f.items[uint32_t(h >> 32)], uint32_t(h), i);
 }
 
-// string bytes of one projected column: one warp per output row
-__global__ void k_project_bytes(const __grid_constant__ ProjArgs f, uint32_t ci, unsigned long long n_rows) {
+// ORDER BY ... LIMIT on a scan under PQ_QUERY_ALLGATHER: output row i is this rank's row with handle owned[i], or
+// another rank's (~0): its bytes stay zero here, so that the sum of every rank's block is the result
+__global__ void __launch_bounds__(256) k_project_owned(const __grid_constant__ ProjArgs f, const unsigned long long* __restrict__ owned) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= f.n_out) return;
+  const unsigned long long h = owned[i];
+  if (h != ~0ull) project_row(f, f.items[uint32_t(h >> 32)], uint32_t(h), i);
+}
+
+// string bytes of one projected column: one warp per output row (owned != nullptr: the rows k_project_owned projected)
+__global__ void k_project_bytes(const __grid_constant__ ProjArgs f, uint32_t ci, unsigned long long n_rows,
+                                const unsigned long long* __restrict__ owned = nullptr) {
   const unsigned long long i = (blockIdx.x * uint64_t(blockDim.x) + threadIdx.x) >> 5;
   const uint32_t lane = threadIdx.x & 31;
-  if (i >= n_rows) return;
+  if (i >= n_rows || (owned && owned[i] == ~0ull)) return;
   const ProjCol& pc = f.cols[ci];
   const uint32_t n = reinterpret_cast<const uint32_t*>(f.out + pc.len_off)[i];
   const uint8_t* src = f.arena + reinterpret_cast<const unsigned long long*>(f.out + pc.src_off)[i];

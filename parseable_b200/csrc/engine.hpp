@@ -247,6 +247,8 @@ class Table {
   DevPage* d_pages = nullptr;
   uint8_t* d_strmat = nullptr;            // DELTA_BYTE_ARRAY pages rewritten as PLAIN BYTE_ARRAY pages (outside the arena: DevPage.off wraps)
   uint64_t total_rows = 0;
+  uint32_t shard_index = 0, shard_count = 1;   // this process scans row groups g % shard_count == shard_index of the list
+  uint64_t list_rows = 0;                      // rows of every row group of the file list (global_row0 runs over them)
   uint64_t h2d_bytes = 0;
   uint64_t chunk_bytes = 0;
   int find_column(const std::string& name) const;

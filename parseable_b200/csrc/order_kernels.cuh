@@ -395,6 +395,113 @@ __global__ void k_order_gather(const uint32_t* __restrict__ idx, uint32_t keep, 
   if (r < keep) new_slot[r] = out_slot ? out_slot[idx[r]] : idx[r];
 }
 
+// ---- ORDER BY ... LIMIT on a scan under PQ_QUERY_ALLGATHER: every rank's first rows merged alike on every rank.
+// Rank r packs its first keep_r rows (order_sort's, in its order) as records of W = nterms + 2 words: the encoded term
+// values (order_encode, DESC applied), a word of NULL flags (bit t: term t is NULL) and the global row id; its block
+// holds keep_max records, those past keep_r are padding.  One all-gather hands every rank the same blocks in rank
+// order.  The candidates (record j < keep_r of rank r is candidate pre[r] + j) are sorted by global row id (RadixSort),
+// then scattered into order_sort's input in that order: order_sort breaks ties by position, so rows equal on every
+// term come out in global row order, as one rank over the whole table returns them.
+//   k_scan_cand_pack     this rank's send block
+//   k_scan_cand_list     the global row id (the sort's key) and the record index of every candidate
+//   (RadixSort)          the candidates in ascending global row id
+//   k_scan_cand_scatter  the terms and NULL flags in that order, each term's value range, the record of every position
+//   (order_sort)         the first `limit` positions, as record indices
+//   k_scan_owned         the output rows this rank projects: their handles, ~0 for another rank's rows
+struct ScanMergeArgs {
+  const unsigned long long* recv;   // nranks blocks of keep_max records of nterms + 2 words
+  const unsigned long long* pre;    // [nranks + 1]: the first candidate of every rank, and the total
+  uint64_t keep_max;
+  uint32_t nranks, n, nterms;       // n: the candidates of every rank
+};
+
+__device__ __forceinline__ uint64_t scan_cand_record(const ScanMergeArgs& a, uint32_t p) {
+  uint32_t lo = 0, hi = a.nranks - 1;   // the rank r with pre[r] <= p < pre[r + 1] (a rank may have none)
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi + 1) / 2;
+    if (a.pre[mid] <= p) lo = mid;
+    else hi = mid - 1;
+  }
+  return uint64_t(lo) * a.keep_max + (p - a.pre[lo]);
+}
+
+// record j < keep_max: this rank's row at sorted position kept[j] (kept == nullptr: j) of its selection, or padding
+__global__ void k_scan_cand_pack(const unsigned long long* __restrict__ vals, const uint8_t* __restrict__ nulls, uint32_t n_sel,
+                                 uint32_t nterms, const uint32_t* __restrict__ kept, uint32_t keep,
+                                 const unsigned long long* __restrict__ handles, const DevItem* __restrict__ items,
+                                 uint64_t keep_max, unsigned long long* __restrict__ send) {
+  const uint32_t w = nterms + 2;
+  for (uint64_t j = blockIdx.x * uint64_t(blockDim.x) + threadIdx.x; j < keep_max; j += uint64_t(gridDim.x) * blockDim.x) {
+    unsigned long long* rec = send + j * w;
+    if (j >= keep) {
+      for (uint32_t t = 0; t < w; t++) rec[t] = t + 1 < w ? 0ull : ~0ull;
+      continue;
+    }
+    const uint32_t q = kept ? kept[j] : uint32_t(j);
+    unsigned long long flags = 0;
+    for (uint32_t t = 0; t < nterms; t++) {
+      rec[t] = vals[size_t(t) * n_sel + q];
+      flags |= (unsigned long long)(nulls[size_t(t) * n_sel + q] != 0) << t;
+    }
+    rec[nterms] = flags;
+    const unsigned long long h = handles[q];
+    rec[nterms + 1] = items[uint32_t(h >> 32)].global_row0 + uint32_t(h);
+  }
+}
+
+__global__ void k_scan_cand_list(const ScanMergeArgs a, unsigned long long* __restrict__ ids, uint32_t* __restrict__ rec) {
+  for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < a.n; p += gridDim.x * blockDim.x) {
+    const uint64_t r = scan_cand_record(a, p);
+    ids[p] = a.recv[r * (a.nterms + 2) + a.nterms + 1];
+    rec[p] = uint32_t(r);   // nranks x keep_max < 2^32 (checked on the host)
+  }
+}
+
+// one thread per position i of the global row order (candidate sorted[i]), ranges reduced as k_order_encode does
+__global__ void __launch_bounds__(256) k_scan_cand_scatter(const ScanMergeArgs a, const uint32_t* __restrict__ sorted,
+                                                           const uint32_t* __restrict__ rec, unsigned long long* __restrict__ vals,
+                                                           uint8_t* __restrict__ nulls, OrderRange* __restrict__ ranges,
+                                                           uint32_t* __restrict__ rec_at) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool live = i < a.n;
+  const uint64_t r = live ? rec[sorted ? sorted[i] : i] : 0;   // sorted == nullptr: the sort had no bits to sort by
+  const unsigned long long* x = a.recv + r * (a.nterms + 2);
+  const unsigned long long flags = live ? x[a.nterms] : 0ull;
+  if (live) rec_at[i] = uint32_t(r);
+  for (uint32_t t = 0; t < a.nterms; t++) {
+    const bool valid = live && !((flags >> t) & 1ull);
+    const unsigned long long v = live ? x[t] : 0ull;
+    if (live) {
+      vals[size_t(t) * a.n + i] = v;
+      nulls[size_t(t) * a.n + i] = valid ? 0 : 1;
+    }
+    unsigned long long mn = valid ? v : ~0ull, mx = valid ? v : 0ull;
+    for (int s = 16; s > 0; s >>= 1) {
+      mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, s));
+      mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, s));
+    }
+    const bool any_null = __any_sync(0xffffffffu, live && !valid), any_value = __any_sync(0xffffffffu, valid);
+    if ((threadIdx.x & 31) == 0) {
+      if (any_value) {
+        atomicMin(&ranges[t].min, mn);
+        atomicMax(&ranges[t].max, mx);
+        atomicOr(&ranges[t].has_value, 1u);
+      }
+      if (any_null) atomicOr(&ranges[t].has_null, 1u);
+    }
+  }
+}
+
+// output row j is record order[j]: this rank's when it lies in block `me`, then projected through its handle
+__global__ void k_scan_owned(const uint32_t* __restrict__ order, uint32_t keep, uint64_t keep_max, uint32_t me,
+                             const uint32_t* __restrict__ kept, const unsigned long long* __restrict__ handles,
+                             unsigned long long* __restrict__ owned) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= keep) return;
+  const uint64_t r = order[j], k = r % keep_max;
+  owned[j] = r / keep_max == me ? handles[kept ? kept[k] : uint32_t(k)] : ~0ull;
+}
+
 // ---- ROW_NUMBER() OVER (PARTITION BY ...) cut to a rank range, over the n rows order_sort left in (partition terms,
 // order terms) order.  Sorted position p holds row perm[p] (perm == nullptr: row p).  Tiles of kSlotTile positions,
 // 256 threads x 4 consecutive positions, as k_slot_compact:

@@ -1081,7 +1081,8 @@ struct MergeRun {
 // (the row order is the order).  The kernels are timed by `t_sort` (every buffer is allocated before the events, so the
 // span holds device work only); *sort_timed says whether it was recorded.  Returns the kernels it launched.
 uint64_t order_sort(const OrderBufs& ob, uint32_t nterms, uint32_t n, const uint8_t* nulls_first, uint32_t keep, const uint32_t* rows,
-                    DevBuf<uint32_t>& kept, cudaStream_t stream, PqMetrics& m, Timer& t_sort, bool* sort_timed) {
+                    DevBuf<uint32_t>& kept, cudaStream_t stream, PqMetrics& m, Timer& t_sort, bool* sort_timed,
+                    const char** path_name = nullptr) {
   uint64_t launches = 0;
   *sort_timed = false;
   std::vector<OrderRange> hr(nterms);
@@ -1100,6 +1101,7 @@ uint64_t order_sort(const OrderBufs& ob, uint32_t nterms, uint32_t n, const uint
   if (want == "sort") path = P_SORT;
   else if (want == "topk" && topk_ok) path = P_TOPK;
   else if (want == "cta" && cta_ok) path = P_CTA;
+  if (path_name) *path_name = path == P_CTA ? "cta" : path == P_TOPK ? "topk" : "sort";
   const uint32_t grid_n = uint32_t((uint64_t(n) + 255) / 256);
   DevBuf<unsigned long long> words;
   words.alloc(size_t(pk.nwords) * n, stream);
@@ -1183,6 +1185,160 @@ uint64_t order_groups(OrderArgs oa, const uint8_t* nulls_first, uint32_t keep, D
   }
   return launches;
 }
+
+// ORDER BY ... LIMIT on a scan under PQ_QUERY_ALLGATHER (order_kernels.cuh): every rank's first rows gathered and
+// ordered alike on every rank, each output row then projected by the rank that holds it.  exchange(): one all-gather
+// of a record per rank and one host round trip, after which every rank reaches the same verdicts from the same records
+// and throws the same code, naming the rank.  merge(): the candidates' all-gather and their global order.
+enum : uint32_t { kScanRecKeep = 0, kScanRecTotal = 1, kScanRecCorrupt = 2, kScanRecBudget = 3, kScanRecRowEnd = 4, kScanRecWords = 5 };
+struct ScanMerge {
+  uint32_t nr = 0, me = 0, nterms = 0;
+  uint64_t keep_r = 0, keep_max = 0, cand = 0, total = 0, keep = 0, row_end = 0;   // cand: the candidates of every rank
+  std::vector<uint64_t> str_len;            // the longest string of every projected Utf8 column, over every rank
+  std::vector<unsigned long long> pre;      // [nr + 1]: the first candidate of every rank
+  Timer t_rec, t_cand, t_sort, t_out;
+  bool sort_timed = false, out_timed = false;
+  const char* path = "none";                // order_sort's path ("none": every candidate is one key)
+
+  // keep_r / total_r / corrupt: this rank's kept and selected rows and corrupt-page code; row_end_r: one past its
+  // largest global row id; str_len_r: its longest string of every projected Utf8 column; row_bytes: result block bytes
+  // per output row besides the strings.  Throws the agreed verdicts.
+  void exchange(uint32_t terms, uint64_t keep_rank, uint64_t total_r, uint64_t corrupt, uint64_t row_end_r,
+                const std::vector<uint64_t>& str_len_r, uint64_t lim, uint64_t row_bytes, cudaStream_t stream, PqMetrics& m) {
+    nr = uint32_t(comm_nranks());
+    me = uint32_t(comm_rank());
+    nterms = terms;
+    keep_r = keep_rank;
+    const size_t nw = kScanRecWords + str_len_r.size();
+    std::vector<unsigned long long> rec(nw, 0), h(nw * nr);
+    size_t free_b = 0, total_b = 0;
+    PQB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    uint64_t budget = free_b / 2;
+    if (const char* e = getenv("PQB_MERGE_BUDGET")) budget = std::min<uint64_t>(budget, strtoull(e, nullptr, 10));   // test switch: bytes
+    rec[kScanRecKeep] = keep_r;
+    rec[kScanRecTotal] = total_r;
+    rec[kScanRecCorrupt] = corrupt;
+    rec[kScanRecBudget] = budget;
+    rec[kScanRecRowEnd] = row_end_r;
+    for (size_t c = 0; c < str_len_r.size(); c++) rec[kScanRecWords + c] = str_len_r[c];
+    DevBuf<unsigned long long> d_rec, d_recs;
+    d_rec.upload(rec, stream);
+    d_recs.alloc(h.size(), stream);
+    PQB_CUDA(cudaEventRecord(t_rec.a, stream));
+    comm_allgather_bytes(d_rec.p, d_recs.p, nw * 8, stream);
+    PQB_CUDA(cudaEventRecord(t_rec.b, stream));
+    PQB_CUDA(cudaMemcpyAsync(h.data(), d_recs.p, h.size() * 8, cudaMemcpyDeviceToHost, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+    m.h2d_bytes += nw * 8;
+    m.d2h_bytes += h.size() * 8;
+    // ---- the verdicts: every rank holds the same records ----
+    pre.assign(nr + 1, 0);
+    str_len.assign(str_len_r.size(), 0);
+    int corrupt_rank = -1, big_rank = -1;
+    for (uint32_t r = 0; r < nr; r++) {
+      const unsigned long long* x = &h[nw * r];
+      pre[r + 1] = pre[r] + x[kScanRecKeep];
+      keep_max = std::max<uint64_t>(keep_max, x[kScanRecKeep]);
+      total += x[kScanRecTotal];
+      row_end = std::max<uint64_t>(row_end, x[kScanRecRowEnd]);
+      if (x[kScanRecCorrupt] && corrupt_rank < 0) corrupt_rank = int(r);
+      if (x[kScanRecTotal] > 0xffffffffull && big_rank < 0) big_rank = int(r);
+      for (size_t c = 0; c < str_len.size(); c++) str_len[c] = std::max<uint64_t>(str_len[c], x[kScanRecWords + c]);
+    }
+    cand = pre[nr];
+    keep = std::min<uint64_t>(cand, lim);
+    if (corrupt_rank >= 0)
+      throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device of rank " + std::to_string(corrupt_rank) + " (code " +
+                                      std::to_string(h[nw * corrupt_rank + kScanRecCorrupt]) + ")");
+    if (big_rank >= 0)
+      throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY over more than 2^32 - 1 selected rows, on rank " + std::to_string(big_rank));
+    if (uint64_t(nr) * keep_max > 0xffffffffull)
+      throw Error(PQ_ERR_UNSUPPORTED, "ORDER BY ... LIMIT across ranks: the ranks' kept rows exceed 2^32 - 1 records: lower the LIMIT");
+    if (keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
+    uint64_t str_bytes = 0;
+    for (uint64_t len : str_len) {
+      if (keep * len > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "projected strings of one result exceed 2 GiB: add a LIMIT");
+      str_bytes += keep * len;
+    }
+    // send and receive blocks; the candidates' ids, records and row-id sort; their terms, the global sort's packed words
+    // and its radix sort; the kept order, the owners' handles and the result block
+    const uint64_t w = nterms + 2;
+    const uint64_t need = 8 * w * keep_max * (nr + 1) + cand * (8 + 4 + 8 + 4 + 9 * uint64_t(nterms) + 8 * (nterms + 1ull) + 8) +
+                          2 * (cand / kRadixTile + 1) * 256 * 12 + keep * (4 + 8 + row_bytes) + str_bytes;
+    // and on every rank its own sort, which comes first: its selected rows' terms (9 bytes per term), handles, packed words
+    // (<= 8 x (nterms + 1)) and radix sort, its kept positions
+    for (uint32_t r = 0; r < nr; r++) {
+      const uint64_t t = h[nw * r + kScanRecTotal], budget_r = h[nw * r + kScanRecBudget];
+      const uint64_t need_r = need + t * (9 * uint64_t(nterms) + 8 + 8 * (nterms + 1ull) + 8 + 4) + (t / kRadixTile + 1) * 256 * 12;
+      if (need_r > budget_r)
+        throw Error(PQ_ERR_OOM, "ORDER BY ... LIMIT across ranks: the rank's sort and the merge of the ranks' first rows need " +
+                                    std::to_string(need_r >> 20) + " MiB of HBM, more than their budget on rank " + std::to_string(r) +
+                                    ": half the free HBM (" + std::to_string(budget_r >> 20) + " MiB)");
+    }
+  }
+
+  // This rank's first keep_r rows (its encoded terms vals / nulls over its n_sel selected rows, kept: their positions,
+  // nullptr: 0 .. keep_r - 1) go out, every rank's come back, and owned[j] becomes the handle of output row j when this
+  // rank holds it (~0 otherwise).  Returns the kernels it launched.
+  uint64_t merge(const unsigned long long* vals, const uint8_t* nulls, uint32_t n_sel, const uint32_t* kept,
+                 const unsigned long long* handles, const DevItem* items, const uint8_t* nulls_first,
+                 DevBuf<unsigned long long>& owned, cudaStream_t stream, PqMetrics& m) {
+    const uint64_t w = nterms + 2;
+    const uint32_t n = uint32_t(cand);
+    DevBuf<unsigned long long> send, recv, ids, d_pre;
+    DevBuf<uint32_t> rec, rec_at, order;
+    send.alloc(keep_max * w, stream);
+    recv.alloc(nr * keep_max * w, stream);
+    ids.alloc(n, stream);
+    rec.alloc(n, stream);
+    rec_at.alloc(n, stream);
+    d_pre.upload(pre, stream);
+    m.h2d_bytes += pre.size() * 8;
+    owned.alloc(keep, stream);
+    RadixSort rs(n, stream);
+    OrderBufs ob(nterms, n, stream, m);
+    uint64_t launches = 0;
+    PQB_CUDA(cudaEventRecord(t_cand.a, stream));
+    if (keep_max) {   // the same on every rank
+      k_scan_cand_pack<<<uint32_t(std::min<uint64_t>(2048, (keep_max + 255) / 256)), 256, 0, stream>>>(
+          vals, nulls, n_sel, nterms, kept, uint32_t(keep_r), handles, items, keep_max, send.p);
+      comm_allgather_bytes(send.p, recv.p, keep_max * w * 8, stream);
+      launches++;
+    }
+    ScanMergeArgs a{recv.p, d_pre.p, keep_max, nr, n, nterms};
+    if (n) {
+      k_scan_cand_list<<<std::min<uint32_t>(2048, (n + 255) / 256), 256, 0, stream>>>(a, ids.p, rec.p);
+      const uint32_t bits = row_end > 1 ? 64 - __builtin_clzll(row_end - 1) : 0;   // global row ids < row_end
+      const uint32_t* sorted = rs.sort(ids.p, nullptr, 0, bits, stream, launches);
+      k_scan_cand_scatter<<<(n + 255) / 256, 256, 0, stream>>>(a, sorted, rec.p, ob.vals.p, ob.nulls.p, ob.ranges.p, rec_at.p);
+      launches += 2;
+    }
+    PQB_CUDA(cudaEventRecord(t_cand.b, stream));
+    PQB_CUDA(cudaGetLastError());
+    if (keep) {
+      launches += order_sort(ob, nterms, n, nulls_first, uint32_t(keep), rec_at.p, order, stream, m, t_sort, &sort_timed, &path);
+      k_scan_owned<<<uint32_t((keep + 255) / 256), 256, 0, stream>>>(order.p ? order.p : rec_at.p, uint32_t(keep), keep_max, me, kept,
+                                                                     handles, owned.p);
+      launches++;
+      PQB_CUDA(cudaGetLastError());
+    }
+    return launches;
+  }
+
+  // after the caller's stream synchronise: allreduce_ms, and with PQB_VERBOSE the sizes, the sort path and the times
+  void report(bool verbose, PqMetrics& m) {
+    float rec_ms = 0, cand_ms = 0, sort_ms = 0, out_ms = 0;
+    cudaEventElapsedTime(&rec_ms, t_rec.a, t_rec.b);
+    cudaEventElapsedTime(&cand_ms, t_cand.a, t_cand.b);
+    if (sort_timed) cudaEventElapsedTime(&sort_ms, t_sort.a, t_sort.b);
+    if (out_timed) cudaEventElapsedTime(&out_ms, t_out.a, t_out.b);
+    m.allreduce_ms = double(rec_ms) + double(cand_ms) + double(sort_ms) + double(out_ms);
+    if (verbose)
+      fprintf(stderr, "[pqb] scan merge: keep_r %llu, keep_max %llu, candidates %llu, kept %llu, sort path %s, exchange %.3f ms, "
+              "candidates %.3f ms, sort %.3f ms, projection and reductions %.3f ms\n", (unsigned long long)keep_r,
+              (unsigned long long)keep_max, (unsigned long long)cand, (unsigned long long)keep, path, rec_ms, cand_ms, sort_ms, out_ms);
+  }
+};
 
 // ROW_NUMBER() OVER (PARTITION BY ... ORDER BY ...) cut to a rank range, over n rows whose partition terms and then
 // order terms the caller encoded into `ob`.  count() sorts and counts the kept rows; the caller sizes its result from
@@ -1376,6 +1532,16 @@ void Query::run(const PqQueryDesc& d) {
     if (row_order && (d.flags & PQ_QUERY_COUNT_ONLY)) throw Error(PQ_ERR_INVALID_ARG, "ORDER BY with PQ_QUERY_COUNT_ONLY: a count has no rows to order");
     if (row_order && d.limit < 0 && !win) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY needs a LIMIT (limit >= 0)");
   }
+  // PQ_QUERY_ALLGATHER: the ranks' first rows of an ordered scan merged into the whole table's (checked alike on every rank)
+  if (d.flags & PQ_QUERY_ALLGATHER) {
+    if (!comm_active()) throw Error(PQ_ERR_INVALID_ARG, "PQ_QUERY_ALLGATHER without pq_comm_init_rank");
+    if (d.n_aggs) throw Error(PQ_ERR_INVALID_ARG, "PQ_QUERY_ALLGATHER on an aggregate query: PQ_QUERY_ALLREDUCE merges aggregates");
+    if (d.flags & PQ_QUERY_COUNT_ONLY) throw Error(PQ_ERR_INVALID_ARG, "PQ_QUERY_ALLGATHER with PQ_QUERY_COUNT_ONLY: a count has no rows to merge");
+    if (win) throw Error(PQ_ERR_UNSUPPORTED, "PQ_QUERY_ALLGATHER with a window: windows are not merged across ranks");
+    if (!row_order) throw Error(PQ_ERR_UNSUPPORTED, "PQ_QUERY_ALLGATHER needs ORDER BY ... LIMIT: an unordered scan is not merged across ranks");
+  }
+  // every rank's first rows are gathered and merged (with one rank they already are the table's)
+  const bool merge_rows = (d.flags & PQ_QUERY_ALLGATHER) && comm_nranks() > 1;
 
   cudaStream_t stream = ctx.stream_acquire();
   struct StreamGuard { cudaStream_t s; int dev; ~StreamGuard() { Context::get().stream_release(s, dev); } } sg{stream, ctx.device()};
@@ -1877,8 +2043,9 @@ void Query::run(const PqQueryDesc& d) {
   const bool allreduce = (d.flags & PQ_QUERY_ALLREDUCE) != 0;
   if (allreduce && !comm_active()) throw Error(PQ_ERR_INVALID_ARG, "PQ_QUERY_ALLREDUCE without pq_comm_init_rank");
   const bool multi = agg_kernel && allreduce && comm_nranks() > 1;
-  // every query that meets the other ranks in a collective (an aggregate table, or COUNT(*)'s total) agrees on refusals
-  const bool agree = has_aggs && allreduce && comm_nranks() > 1;
+  // every query that meets the other ranks in a collective (an aggregate table, COUNT(*)'s total, or a scan's merged
+  // first rows) agrees on refusals
+  const bool agree = (has_aggs && allreduce && comm_nranks() > 1) || merge_rows;
   const uint32_t n_flat = flat_ok ? shape->n_flat : 0;
   const uint32_t n_general = flat_ok ? shape->n_general : uint32_t(items.size());
   // ---- refusals that depend on what this rank's shard holds (its pages, footers and flat-store copies).  Under a
@@ -1965,6 +2132,14 @@ void Query::run(const PqQueryDesc& d) {
       refuse(std::string(ag.fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
              ") over Utf8 / Boolean needs a flat-store copy of every page the query reads: " + shape->why_general);
   }
+  if (merge_rows && n_general)   // (without other ranks: thrown with the other scan refusals below)
+    refuse("ORDER BY on a scan needs a flat-store copy of every page the query reads: " + shape->why_general);
+  // the merge breaks ties by __row_id, which is global only when every rank opened the same file list and scans its row
+  // groups g % N == rank (under file sharding each rank numbers its own files from 0)
+  if (merge_rows && (table->shard_count != uint32_t(comm_nranks()) || table->shard_index != uint32_t(comm_rank())))
+    refuse("PQ_QUERY_ALLGATHER needs the table sharded by row group over the communicator (shard_count " +
+           std::to_string(table->shard_count) + ", shard_index " + std::to_string(table->shard_index) + " on rank " +
+           std::to_string(comm_rank()) + " of " + std::to_string(comm_nranks()) + "): only then is __row_id global");
   if (!refusal.empty() && !agree) throw Error(PQ_ERR_UNSUPPORTED, refusal);
   // k_flat_agg walks a regular expression's DFA per row only in its RX instantiations
   bool rx_bytes = false;
@@ -1988,7 +2163,14 @@ void Query::run(const PqQueryDesc& d) {
   for (uint32_t g = 0; g < nrg_table; g++) if (rg_live[g]) live_rows += table->row_groups[g].num_rows;
   uint64_t rows_all = live_rows, general_ranks = n_general ? 1 : 0, general_mask = 0;
   if (agree) {
-    std::vector<unsigned long long> f(6 + ncols, 0ull);
+    // a merged scan adds two words: the sum and the sum of squares of every rank's file-list rows (mod 2^20), which are
+    // equal on every rank when nr x (sum of squares) == sum^2: one file list for every rank
+    std::vector<unsigned long long> f(6 + ncols + (merge_rows ? 2 : 0), 0ull);
+    if (merge_rows) {
+      const unsigned long long x = table->list_rows & 0xfffffull;
+      f[6 + ncols] = x;
+      f[7 + ncols] = x * x;
+    }
     if (!refusal.empty()) {
       f[1 + ncols] = 1;
       if (comm_rank() < 63) f[2 + ncols] = 1ull << comm_rank();
@@ -2010,6 +2192,12 @@ void Query::run(const PqQueryDesc& d) {
       const ColSide& cs = table->sides[shape_cols[plan.aggs[a].col]];
       if (!cs.glob_ready || cs.glob_epoch != comm_epoch()) f[0] = 1;
     }
+    for (uint32_t t = 0; merge_rows && t < d.n_order_by; t++) {   // so do the Utf8 terms of a merged scan
+      const uint32_t s = uint32_t(slot_of[d.order_by[t].index]);
+      if (plan.cols[s].kind != DK_STR) continue;
+      const ColSide& cs = table->sides[shape_cols[s]];
+      if (!cs.glob_ready || cs.glob_epoch != comm_epoch()) f[0] = 1;
+    }
     for (uint32_t s = 0; s < ncols; s++) f[1 + s] = col_has_nulls[s] ? 1ull : 0ull;
     DevBuf<unsigned long long> df;
     df.upload(f, stream);
@@ -2021,13 +2209,15 @@ void Query::run(const PqQueryDesc& d) {
       throw Error(PQ_ERR_UNSUPPORTED, "refused on " + (f[2 + ncols] ? "rank " + std::to_string(__builtin_ctzll(f[2 + ncols]))
                                                                     : std::to_string(f[1 + ncols]) + " ranks") +
                                           " (its shard holds pages or footers this query cannot take on the GPU path)");
+    if (merge_rows && (unsigned __int128)f[7 + ncols] * comm_nranks() != (unsigned __int128)f[6 + ncols] * f[6 + ncols])
+      throw Error(PQ_ERR_UNSUPPORTED, "PQ_QUERY_ALLGATHER: the ranks opened file lists of different sizes; every rank must open the same "
+                                      "list, sharded by row group");
     general_ranks = f[3 + ncols];
     general_mask = f[4 + ncols];
     rows_all = f[5 + ncols];
-    if (multi) {
-      keys_agreed = f[0] == 0;
+    if (multi || merge_rows) keys_agreed = f[0] == 0;
+    if (multi)
       for (uint32_t s = 0; s < ncols; s++) col_has_nulls[s] = f[1 + s] != 0;
-    }
   }
   std::vector<uint8_t> nn_is_rows(kMaxAggs, 0);
   {
@@ -2348,13 +2538,16 @@ void Query::run(const PqQueryDesc& d) {
     throw Error(PQ_ERR_UNSUPPORTED, "ORDER BY on a scan needs a flat-store copy of every page the query reads: " + shape->why_general);
   // ---- ORDER BY on a scan: a Utf8 term sorts by the bytewise rank of the column's GROUP BY ids (ensure_key, cached with
   // the table); its pages without a dictionary are read as their id pages, through this query's copy of the flat page
-  // table that only the encode kernel sees ----
+  // table that only the encode kernel sees.  When the ranks' rows are merged, the ids and ranks are those of the
+  // numbering every rank agreed on (unify_key, a collective: every rank joins it for the same columns, also a rank whose
+  // files lack the column), so that every rank encodes a value alike ----
   RowOrderArgs roa{};
   uint8_t row_nulls_first[kMaxOrder] = {};
   std::vector<std::shared_ptr<const uint32_t>> row_rank_hold;   // a query keeps the ranks it sorts with alive
   DevBuf<FlatPageRec> d_opages;
   if (row_order) {
-    std::vector<int> id_cols;   // table columns whose pages without a dictionary are read as id pages
+    std::vector<std::pair<int, const uint32_t*>> id_cols;   // table columns whose pages without a dictionary are read as id pages
+    std::set<int> unified;
     roa.nterms = n_part + d.n_order_by;   // a window sorts by its partition terms first
     for (uint32_t t = 0; t < roa.nterms; t++) {
       const PqOrderBy& ob = t < n_part ? win->partition_by[t] : d.order_by[t - n_part];
@@ -2365,25 +2558,31 @@ void Query::run(const PqQueryDesc& d) {
       row_nulls_first[t] = (ob.flags & PQ_ORDER_NULLS_FIRST) ? 1 : 0;
       ot.enc = ot.kind == DK_F64 ? OE_F64 : ot.kind == DK_I64 ? OE_I64 : OE_RAW;   // Boolean: 0 / 1; Utf8: the rank
       const int tc_i = shape_cols[ot.slot];
-      if (ot.kind != DK_STR || table->columns[tc_i].kind == 0xfe) continue;   // in no file: every row NULL, nothing to rank
+      const bool absent = table->columns[tc_i].kind == 0xfe;   // in no file: every row NULL, nothing to rank
+      if (ot.kind != DK_STR || (absent && !merge_rows)) continue;
       table->ensure_key(tc_i, stream);
-      row_rank_hold.push_back(table->ensure_kd_rank(tc_i, false, stream));
-      ot.gid = table->sides[tc_i].d_gid;
+      if (merge_rows && !keys_agreed && unified.insert(tc_i).second) {
+        if (verbose) fprintf(stderr, "[pqb] scan merge: the ranks agree on a numbering of '%s'\n", table->columns[tc_i].name.c_str());
+        table->unify_key(tc_i, stream);
+      }
+      if (absent) continue;
+      row_rank_hold.push_back(table->ensure_kd_rank(tc_i, merge_rows, stream));
+      ot.gid = merge_rows ? table->sides[tc_i].d_glob_gid : table->sides[tc_i].d_gid;
       ot.rank = row_rank_hold.back().get();
-      if (!table->sides[tc_i].key_row_pages.empty()) id_cols.push_back(tc_i);
+      if (!table->sides[tc_i].key_row_pages.empty()) id_cols.push_back({tc_i, ot.gid});
     }
     if (!id_cols.empty()) {
       std::vector<FlatPageRec> fp;
       {
         std::lock_guard<std::mutex> lk(table->side_mu);
         fp = table->flat_pages;
-        for (int tc_i : id_cols) {
+        for (const auto& [tc_i, gid] : id_cols) {
           const ColSide& cs = table->sides[tc_i];
           for (const ColSide::KeyRowPage& rp : cs.key_row_pages) {
             FlatPageRec& r = fp[rp.page];
             r.fkind = FK_IDS;
             r.bw = 32;
-            r.off = uint64_t(cs.d_gid) + 4ull * (uint64_t(cs.n_dict_pad) + rp.ebase) - uint64_t(table->d_flat);   // as for key columns
+            r.off = uint64_t(gid) + 4ull * (uint64_t(cs.n_dict_pad) + rp.ebase) - uint64_t(table->d_flat);   // as for key columns
           }
         }
       }
@@ -3329,6 +3528,14 @@ void Query::run(const PqQueryDesc& d) {
       // an ordered scan without a projection returns its selected row ordinals in order
       if ((d.flags & PQ_QUERY_EMIT_ROW_IDS) || !projecting) pcs.push_back({0, 0xffffffffu, DK_I64, "__row_id", PQ_T_I64});
       const uint32_t npc = uint32_t(pcs.size());
+      // the longest string of every projected Utf8 column sizes its bytes (the ranks' merged rows: over every rank)
+      std::vector<uint64_t> str_len(npc, 0);
+      for (uint32_t c = 0; c < npc; c++)
+        if (pcs[c].kind == DK_STR) {
+          const ColSide& cs = table->sides[shape_cols[pcs[c].slot]];
+          str_len[c] = std::max(cs.max_ent_len, cs.max_plain_len);
+        }
+      std::unique_ptr<ScanMerge> smerge;   // PQ_QUERY_ALLGATHER with other ranks
       std::shared_ptr<PinnedBlock> block;
       ProjArgs pj{};
       uint64_t nulls_off = 0, copy_bytes = 0;
@@ -3343,8 +3550,11 @@ void Query::run(const PqQueryDesc& d) {
       if (win && (win->flags & PQ_WINDOW_PARTITION_ROWS)) win_names.push_back("partition_rows");
       uint64_t win_off[2] = {0, 0};
       std::function<void(long long*, long long*)> win_fill;
-      // the first `cap` selected rows, or with `handles` the rows at positions kept[0, cap) (ORDER BY ... LIMIT)
-      auto gather = [&](unsigned long long cap, const unsigned long long* handles, const uint32_t* kept) {
+      // the first `cap` selected rows, or with `handles` the rows at positions kept[0, cap) (ORDER BY ... LIMIT), or with
+      // `owned` the output rows this rank holds of the ranks' merged rows: every byte of the block is then written by one
+      // rank and zero on the others, and the ranks' blocks are summed (their u64 words: disjoint bytes never carry).
+      // String offsets, which every rank computes alike, are computed after the lengths are summed and never summed.
+      auto gather = [&](unsigned long long cap, const unsigned long long* handles, const uint32_t* kept, const unsigned long long* owned) {
         nbatches = uint32_t((cap + batch_rows - 1) / batch_rows);
         uint64_t off = 0;
         auto take = [&](uint64_t bytes) { uint64_t o = off; off = (off + bytes + 63) & ~63ull; return o; };
@@ -3359,15 +3569,16 @@ void Query::run(const PqQueryDesc& d) {
           else if (pc.kind == DK_STR) pc.val_off = take((cap + 1) * 4);
           else pc.val_off = take(cap * 8);
         }
+        uint64_t data_lo = off;   // the string bytes of every column: [data_lo, data_hi)
         for (uint32_t c = 0; c < npc; c++) {
           ProjCol& pc = pj.cols[c];
           if (pc.kind != DK_STR) continue;
-          const ColSide& cs = table->sides[shape_cols[pc.slot]];
-          pc.ent = cs.d_ent_off;
-          const uint64_t bound = cap * uint64_t(std::max(cs.max_ent_len, cs.max_plain_len));
+          pc.ent = table->sides[shape_cols[pc.slot]].d_ent_off;
+          const uint64_t bound = cap * str_len[c];
           if (bound > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "projected strings of one result exceed 2 GiB: add a LIMIT");
           pc.data_off = take(bound);
         }
+        const uint64_t data_hi = off;
         for (size_t w = 0; w < win_names.size(); w++) win_off[w] = take(cap * 8);
         copy_bytes = off;
         for (uint32_t c = 0; c < npc; c++)
@@ -3397,7 +3608,13 @@ void Query::run(const PqQueryDesc& d) {
           win_fill(cols[0], cols[1]);
           launches++;
         }
-        if (handles) {
+        if (owned) {
+          PQB_CUDA(cudaEventRecord(smerge->t_out.a, stream));
+          k_project_owned<<<uint32_t((cap + 255) / 256), 256, 0, stream>>>(pj, owned);
+          // everything but the string bytes (summed once they are written); the string offsets are still zero
+          comm_allreduce_u64(d_block.p, data_lo / 8, 0 /*sum*/, stream);
+          if (off > data_hi) comm_allreduce_u64(d_block.p + data_hi, (off - data_hi) / 8, 0 /*sum*/, stream);   // the lengths
+        } else if (handles) {
           k_project_rows<<<uint32_t((cap + 255) / 256), 256, 0, stream>>>(pj, handles, kept);
         } else {
           const uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
@@ -3409,8 +3626,13 @@ void Query::run(const PqQueryDesc& d) {
           // rows beyond the selected total have length 0: the scan over `cap` rows is exact
           k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + pj.cols[c].len_off), uint32_t(cap), nullptr,
                                                  reinterpret_cast<int32_t*>(d_block.p + pj.cols[c].val_off));
-          k_project_bytes<<<uint32_t((cap * 32 + 255) / 256), 256, 0, stream>>>(pj, c, cap);
+          k_project_bytes<<<uint32_t((cap * 32 + 255) / 256), 256, 0, stream>>>(pj, c, cap, owned);
           launches += 2;
+        }
+        if (owned) {
+          if (data_hi > data_lo) comm_allreduce_u64(d_block.p + data_lo, (data_hi - data_lo) / 8, 0 /*sum*/, stream);
+          PQB_CUDA(cudaEventRecord(smerge->t_out.b, stream));
+          smerge->out_timed = true;
         }
         PQB_CUDA(cudaGetLastError());
         block = std::make_shared<PinnedBlock>();
@@ -3418,19 +3640,32 @@ void Query::run(const PqQueryDesc& d) {
         block->bytes = copy_bytes;
         PQB_CUDA(cudaMemcpyAsync(block->p, d_block.p, copy_bytes, cudaMemcpyDeviceToHost, stream));
       };
-      if (row_order && !items.empty()) {
+      if (row_order && (!items.empty() || merge_rows)) {
         // ---- ORDER BY ... LIMIT: every selected row's terms and handle (k_order_rows_encode), the positions of the first
-        // `keep` rows in order (order_sort), then their projection.  Per shard: the merge of the shards' rows is above.
+        // `keep` rows in order (order_sort), then their projection.  Under PQ_QUERY_ALLGATHER with other ranks, those
+        // first rows of every rank are merged (ScanMerge) and each rank projects the merged rows it holds; without the
+        // flag every shard orders and cuts its own selection.
         PQB_CUDA(cudaStreamSynchronize(stream));   // the selected-row total sizes the sort
-        if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
-        if (total > 0xffffffffull) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY over more than 2^32 - 1 selected rows");
         unsigned long long keep = std::min(total, lim);   // a window: the kept rows, known after its sort
-        if (!win && keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
+        if (merge_rows) {   // the checks below, agreed by every rank
+          uint64_t row_end = 0, row_bytes = 0;
+          for (const DevItem& it : items) row_end = std::max<uint64_t>(row_end, it.global_row0 + it.nrows);
+          for (const PC& pc : pcs) row_bytes += 1 + (pc.kind == DK_STR ? 16 : pc.kind == DK_BOOL ? 1 : 8);   // validity, values / offsets and scratch
+          smerge = std::make_unique<ScanMerge>();
+          smerge->exchange(roa.nterms, keep, total, h_counters[1], row_end, str_len, lim, row_bytes, stream, metrics);
+          str_len = smerge->str_len;
+        } else {
+          if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
+          if (total > 0xffffffffull) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY over more than 2^32 - 1 selected rows");
+          if (!win && keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
+        }
+        const uint32_t n = uint32_t(total);
+        std::unique_ptr<OrderBufs> obuf;   // (the merge reads this rank's encoded rows)
+        DevBuf<unsigned long long> handles;
+        DevBuf<uint32_t> kept;
         if (win ? total > 0 : keep > 0) {
-          const uint32_t n = uint32_t(total);
-          OrderBufs ob(roa.nterms, n, stream, metrics);
-          DevBuf<unsigned long long> handles;
-          DevBuf<uint32_t> kept;
+          obuf = std::make_unique<OrderBufs>(roa.nterms, n, stream, metrics);
+          OrderBufs& ob = *obuf;
           handles.alloc(n, stream);
           roa.arena = table->d_arena;
           roa.flat = table->d_flat;
@@ -3464,28 +3699,43 @@ void Query::run(const PqQueryDesc& d) {
             if (keep) {
               kept.alloc(keep, stream);
               win_fill = [&](long long* rn, long long* prows) { wrun->fill(nullptr, keep, kept.p, rn, prows, stream); };
-              gather(keep, handles.p, kept.p);
+              gather(keep, handles.p, kept.p, nullptr);
             }
           } else {
             launches += 1 + order_sort(ob, roa.nterms, n, row_nulls_first, uint32_t(keep), nullptr, kept, stream, metrics, t_sort, &sort_timed);
-            gather(keep, handles.p, kept.p);
+            if (!smerge) gather(keep, handles.p, kept.p, nullptr);
           }
           PQB_CUDA(cudaStreamSynchronize(stream));
-          if (keep) metrics.d2h_bytes += copy_bytes;
+          if (keep && !smerge) metrics.d2h_bytes += copy_bytes;
           float ms = 0, ms2 = 0;
           cudaEventElapsedTime(&ms, t_enc.a, t_enc.b);
           if (sort_timed) cudaEventElapsedTime(&ms2, t_sort.a, t_sort.b);
           metrics.order_ms = double(ms) + double(ms2) + (wrun ? wrun->ms() : 0.0);
         }
-        n_rows = keep;
         shape->last_total.store(total);
+        if (smerge) {
+          // every rank's first rows: the same candidates and the same order on every rank, each output row projected by
+          // the rank that holds it and the ranks' blocks summed
+          DevBuf<unsigned long long> owned;
+          launches += smerge->merge(obuf ? obuf->vals.p : nullptr, obuf ? obuf->nulls.p : nullptr, n, kept.p, handles.p, shape->d_items,
+                                    row_nulls_first, owned, stream, metrics);
+          keep = smerge->keep;
+          if (keep) {
+            gather(keep, nullptr, nullptr, owned.p);
+            metrics.d2h_bytes += copy_bytes;
+          }
+          PQB_CUDA(cudaStreamSynchronize(stream));
+          smerge->report(verbose, metrics);
+          total = smerge->total;
+        }
+        n_rows = keep;
       } else if (!items.empty()) {
         const unsigned long long hint = shape->last_total.load();
         bool done = false;
         if (hint != ~0ull) {
           const unsigned long long cap = std::max<unsigned long long>(1, std::min(lim, hint + hint / 8 + 1024));
           if (cap > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
-          gather(cap, nullptr, nullptr);
+          gather(cap, nullptr, nullptr, nullptr);
           PQB_CUDA(cudaStreamSynchronize(stream));
           if (std::min(total, lim) <= cap) { done = true; n_rows = std::min(total, lim); metrics.d2h_bytes += copy_bytes; }
           else block.reset();
@@ -3496,7 +3746,7 @@ void Query::run(const PqQueryDesc& d) {
           const unsigned long long keep = std::min(total, lim);
           if (keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
           if (keep) {
-            gather(keep, nullptr, nullptr);
+            gather(keep, nullptr, nullptr, nullptr);
             PQB_CUDA(cudaStreamSynchronize(stream));
             metrics.d2h_bytes += copy_bytes;
           }

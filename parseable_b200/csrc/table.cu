@@ -323,6 +323,8 @@ void Table::open(const PqFile* in_files, uint32_t n_files, const std::vector<std
   };
   if (shard_count == 0) shard_count = 1;
   if (shard_index >= shard_count) throw Error(PQ_ERR_INVALID_ARG, "shard_index >= shard_count");
+  this->shard_index = shard_index;
+  this->shard_count = shard_count;
   // footers are parsed on a few host threads (one Parquet file per ingest minute: many small footers)
   files.resize(n_files);
   {
@@ -502,6 +504,7 @@ void Table::open(const PqFile* in_files, uint32_t n_files, const std::vector<std
       const RowGroupMeta& g = hf.meta.row_groups[gi];
       uint64_t row0 = global_row;
       global_row += uint64_t(g.num_rows);
+      list_rows = global_row;
       if (global_rg % shard_count != shard_index) continue;
       if (g.num_rows == 0) continue;
       TableRowGroup trg;

@@ -99,7 +99,19 @@ typedef enum {
   PQ_T_I64 = 2,   /* Int64 */
   PQ_T_F64 = 3,   /* Float64 */
   PQ_T_UTF8 = 4,  /* Utf8 */
-  PQ_T_TS_MS = 5  /* Timestamp(Millisecond, None) */
+  PQ_T_TS_MS = 5, /* Timestamp(Millisecond, None) */
+  /* Date32: days since 1970-01-01 (6 is PQ_T_TS_NS, planning only).  A Parquet INT32 leaf with the DATE logical or
+   * converted type; every other INT32 leaf and FLOAT leaves stay PQ_ERR_UNSUPPORTED at open.  The flat store keeps the
+   * values sign-extended to 8 bytes; results hand them out as Arrow Date32 ("tdD", 4-byte values) and JSON egress writes
+   * a quoted "YYYY-MM-DD" (the date part of the Timestamp(ms) text of d * 86400000).  A literal carries the days in
+   * PqLiteral.i64 (outside int32: PQ_ERR_INVALID_ARG).  PQ_OP_CMP compares a Date32 column with a Date32 literal only,
+   * signed; either side against any other type returns PQ_ERR_UNSUPPORTED, and LIKE / REGEX are refused as on Int64.
+   * Footer min / max (4 bytes) prune row groups.  GROUP BY keys, MIN / MAX (output Date32), COUNT, COUNT(DISTINCT) (by
+   * value), ORDER BY / PARTITION BY terms and projections take it, in signed order; SUM, AVG, MEDIAN, PERCENTILE_CONT
+   * and DATE_BIN over it return PQ_ERR_UNSUPPORTED, and so does a query that reads a Date32 column while some page of a
+   * column it reads has no flat-store copy (PQB_FLAT_SCAN=0 included).  A Date32 column declared PQ_T_I64 or PQ_T_TS_MS
+   * in columns[] returns PQ_ERR_INVALID_ARG. */
+  PQ_T_DATE32 = 7
 } PqType;
 
 /* ---- predicate: flat postfix program (SURVEY §8a "Predicate vocabulary") ---- */
@@ -166,7 +178,8 @@ typedef enum {
   PQ_AGG_COUNT_STAR = 0,
   PQ_AGG_COUNT = 1,
   PQ_AGG_SUM = 2,
-  /* MIN / MAX (DataFusion's min / max, restated, not checked): Int64, Timestamp(ms), Float64 (totalOrder), and:
+  /* MIN / MAX (DataFusion's min / max, restated, not checked): Int64, Timestamp(ms), Date32 (output Date32),
+   * Float64 (totalOrder), and:
    *   Utf8: bytewise order, a prefix before any longer string (the order ORDER BY uses); output Utf8 with int32 offsets
    *     (the shim casts it to Utf8View, as for Utf8 keys), named "min(<col>)" / "max(<col>)".  Dictionary pages,
    *     PLAIN-fallback pages and DELTA_BYTE_ARRAY / DELTA_LENGTH_BYTE_ARRAY pages.
@@ -182,12 +195,12 @@ typedef enum {
   /* COUNT(DISTINCT col) (the alerts' CountDistinct, src/alerts/mod.rs:245-251): Int64, never NULL, named
    * "count(distinct <col>)".  NULL inputs do not count; a group whose inputs are all NULL gets 0.  Values are
    * distinct as GROUP BY keys are: strings by bytes, integers / timestamps / booleans by value, Float64 by bit
-   * pattern (-0.0 and 0.0 differ, as do NaNs with different payloads).  Utf8, Int64, Timestamp(ms), Float64 and
+   * pattern (-0.0 and 0.0 differ, as do NaNs with different payloads).  Utf8, Int64, Timestamp(ms), Date32, Float64 and
    * Boolean columns; refused (PQ_ERR_UNSUPPORTED) under PQ_QUERY_ALLREDUCE. */
   PQ_AGG_COUNT_DISTINCT = 6,
   /* Exact order statistics (DataFusion's median / percentile_cont, restated from DataFusion 53; its crates are not
    * vendored here, so the rules are restated, not checked).  Int64 and Float64 inputs (dictionary or PLAIN pages); Utf8,
-   * Boolean and Timestamp inputs return PQ_ERR_UNSUPPORTED.  NULL inputs are ignored and a column missing from a file
+   * Boolean, Timestamp and Date32 inputs return PQ_ERR_UNSUPPORTED.  NULL inputs are ignored and a column missing from a file
    * reads as NULL; a group with no non-NULL input gets NULL (a global aggregate over zero rows: one row holding NULL).
    * Values are sorted as ORDER BY sorts them: Int64 signed, Float64 by IEEE totalOrder (-NaN < -inf < ... < -0.0 < +0.0
    * < ... < +inf < +NaN).
@@ -213,7 +226,7 @@ typedef struct {
 } PqAgg;
 
 /* ---- computed GROUP BY keys: the counts / histogram API groups by DATE_BIN(<width>, p_timestamp, origin)
- *      (src/query/mod.rs:623-680) ---- */
+ *      (src/query/mod.rs:623-680); DATE_BIN over a Date32 column returns PQ_ERR_UNSUPPORTED ---- */
 typedef enum { PQ_KEY_COLUMN = 0, PQ_KEY_DATE_BIN = 1 } PqKeyKind;
 typedef struct {
   int32_t kind;       /* PqKeyKind */

@@ -20,6 +20,7 @@ ERR_NAMES = {-1: "PQ_ERR_INVALID_ARG", -2: "PQ_ERR_UNSUPPORTED", -3: "PQ_ERR_IO"
              -5: "PQ_ERR_CUDA", -6: "PQ_ERR_OOM"}
 
 PQ_T_NULL, PQ_T_BOOL, PQ_T_I64, PQ_T_F64, PQ_T_UTF8, PQ_T_TS_MS = range(6)
+PQ_T_DATE32 = 7   # Date32: days since 1970-01-01 in PqLiteral.i64 (6 is PQ_T_TS_NS, planning only)
 PQ_OP_CMP, PQ_OP_IS_NULL, PQ_OP_IS_NOT_NULL, PQ_OP_LIKE, PQ_OP_AND, PQ_OP_OR, PQ_OP_NOT, PQ_OP_CONST, PQ_OP_REGEX = range(1, 10)
 PQ_EQ, PQ_NE, PQ_LT, PQ_LE, PQ_GT, PQ_GE = range(6)
 PQ_LIKE_NEGATED, PQ_LIKE_CASE_INSENSITIVE = 1, 2

@@ -54,6 +54,7 @@ const char* format_of(int type) {
     case PQ_T_F64: return "g";
     case PQ_T_UTF8: return "u";
     case PQ_T_TS_MS: return "tsm:";
+    case PQ_T_DATE32: return "tdD";
     default: return "n";
   }
 }

@@ -67,7 +67,7 @@ struct FinishKey {
   uint64_t data_off;           // strings: bytes
   uint32_t stride, card;
   uint64_t wstride;            // stride in 64 bits (hashed group-by decodes the wide id)
-  uint32_t kind;               // DevKind
+  uint32_t kind;               // DevKind (DK_I32: a Date32 key, 4-byte values)
   uint32_t is_bin;             // DATE_BIN key: value = bin_base + group id * bin_width
   int64_t bin_base, bin_width;
 };
@@ -95,7 +95,7 @@ struct FinishArgs {
   uint8_t nn_is_rows[kMaxAggs];
   // the output layout of each aggregate: DK_STR (MIN / MAX over Utf8: int32 offsets at val_off, bytes at astr.data_off),
   // DK_BOOL (MIN / MAX over Boolean: bit-packed values per batch at val_off), anything else 8-byte values
-  uint8_t out_kind[kMaxAggs];
+  uint8_t out_kind[kMaxAggs];   // (DK_I32: MIN / MAX over Date32, 4-byte values)
   uint64_t val_off[kMaxAggs], valid_off[kMaxAggs];
   FinishAggStr astr[kMaxAggs];
   FinishKey keys[kMaxKeys];
@@ -155,6 +155,8 @@ __global__ void k_agg_finish(const __grid_constant__ FinishArgs f) {
       reinterpret_cast<uint32_t*>(f.out + s.len_off)[i] = valid ? s.kd_offs[g + 1] - s.kd_offs[g] : 0u;
     } else if (f.out_kind[a] == DK_BOOL) {
       if (valid && v) atomicOr(reinterpret_cast<uint32_t*>(f.out + f.val_off[a]) + word, bit);
+    } else if (f.out_kind[a] == DK_I32) {   // MIN / MAX over Date32: the low word of the sign-extended cell
+      reinterpret_cast<uint32_t*>(f.out + f.val_off[a])[i] = valid ? uint32_t(v) : 0u;
     } else {
       reinterpret_cast<unsigned long long*>(f.out + f.val_off[a])[i] = valid ? v : 0ull;
     }
@@ -178,7 +180,8 @@ __global__ void k_agg_finish(const __grid_constant__ FinishArgs f) {
         const uint8_t* p = key.kd_bytes + key.kd_offs[gid];
         for (int b = 0; b < 8; b++) v |= (unsigned long long)p[b] << (8 * b);
       }
-      reinterpret_cast<unsigned long long*>(f.out + key.val_off)[i] = v;
+      if (key.kind == DK_I32) reinterpret_cast<uint32_t*>(f.out + key.val_off)[i] = uint32_t(v);   // Date32
+      else reinterpret_cast<unsigned long long*>(f.out + key.val_off)[i] = v;
     }
   }
 }
@@ -272,7 +275,7 @@ struct ProjCol {
   uint64_t len_off;      // strings: u32 length per output row (device-only scratch)
   uint64_t data_off;     // strings: bytes
   uint32_t slot;         // column slot of the plan (chunk table, item.page, item.poff); 0xffffffff: the __row_id column
-  uint32_t kind;         // DevKind
+  uint32_t kind;         // DevKind (DK_I32: a Date32 column, 4-byte values)
 };
 struct ProjArgs {
   const uint8_t* arena;
@@ -413,6 +416,8 @@ __device__ __forceinline__ void project_row(const ProjArgs& f, const DevItem& it
       reinterpret_cast<uint32_t*>(f.out + pc.len_off)[pos] = len;
     } else if (pc.kind == DK_BOOL) {
       if (v) atomicOr(reinterpret_cast<uint32_t*>(f.out + pc.val_off) + vword, vbit);
+    } else if (pc.kind == DK_I32) {   // Date32: the low word of the sign-extended value
+      reinterpret_cast<uint32_t*>(f.out + pc.val_off)[pos] = uint32_t(v);
     } else {
       reinterpret_cast<unsigned long long*>(f.out + pc.val_off)[pos] = v;
     }

@@ -106,6 +106,7 @@ struct TableColumn {
   std::string name;
   uint8_t kind = 0;      // DevKind
   bool is_ts = false;
+  bool is_date = false;  // Date32: INT32 leaves, kind DK_I64 with sign-extended 8-byte values in the flat store
   uint8_t max_def = 0;
 };
 

@@ -96,13 +96,15 @@ __device__ inline bool def_levels_all_valid(const uint8_t* __restrict__ p, uint3
   return true;
 }
 
-enum FlatJobKind : uint32_t { FJ_HYBRID = 1, FJ_COPY8 = 2, FJ_BITS = 3, FJ_DICT8 = 4, FJ_VALID = 5, FJ_BYTES = 6 };
+enum FlatJobKind : uint32_t { FJ_HYBRID = 1, FJ_COPY8 = 2, FJ_BITS = 3, FJ_DICT8 = 4, FJ_VALID = 5, FJ_BYTES = 6, FJ_DICT4 = 7, FJ_WIDEN4 = 8 };
 // FJ_HYBRID: RLE / bit-packed hybrid stream -> flat bits       (page)
 // FJ_COPY8 : PLAIN 8-byte values -> aligned copy               (page)
 // FJ_BITS  : PLAIN boolean bits -> aligned copy                (page)
 // FJ_DICT8 : numeric dictionary (8-byte entries) -> aligned copy (src = arena offset, rows = entries)
 // FJ_VALID : validity bitmap only (a DELTA page with NULLs: its values follow on demand, ensure_plain8)
 // FJ_BYTES : PLAIN BYTE_ARRAY page (dictionary fallback, streams.rs:584-631) -> u32 start of every row's bytes
+// FJ_DICT4 : Date32 dictionary (4-byte INT32 entries) -> sign-extended 8-byte copy, as FJ_DICT8 writes it
+// FJ_WIDEN4: PLAIN Date32 page (4-byte INT32 values) -> sign-extended 8-byte values, as FJ_COPY8 writes them (FK_PLAIN8)
 // A page with NULLs (vdst != ~0) also gets its validity bitmap (1 bit per ROW, from the definition
 // levels) and its values EXPANDED to one slot per row (NULL rows hold 0), so that row r of the page
 // is slot r whatever the NULLs: the scan needs no rank / prefix popcount.
@@ -256,9 +258,12 @@ __global__ void __launch_bounds__(128) k_flat_store(const uint8_t* __restrict__ 
   const uint32_t ji = blockIdx.x * 4 + warp;
   if (ji >= n_jobs) return;
   const FlatStoreJob job = jobs[ji];
-  if (job.kind == FJ_DICT8) {
+  if (job.kind == FJ_DICT8 || job.kind == FJ_DICT4) {
     uint64_t* d = reinterpret_cast<uint64_t*>(flat + job.dst);
-    for (uint32_t i = lane; i < job.rows; i += 32) d[i] = load_u64_unaligned(arena + job.src + uint64_t(i) * 8);
+    if (job.kind == FJ_DICT8)
+      for (uint32_t i = lane; i < job.rows; i += 32) d[i] = load_u64_unaligned(arena + job.src + uint64_t(i) * 8);
+    else
+      for (uint32_t i = lane; i < job.rows; i += 32) d[i] = uint64_t(int64_t(int32_t(load_u32_unaligned(arena + job.src + uint64_t(i) * 4))));
     if (lane == 0) ok_out[ji] = 1;
     return;
   }
@@ -324,6 +329,18 @@ __global__ void __launch_bounds__(128) k_flat_store(const uint8_t* __restrict__ 
     } else {
       expand_rows(valid, rows, [&](uint32_t k) { return load_u64_unaligned(vals + uint64_t(k) * 8); },
                   [&](uint32_t r, bool, uint64_t v, uint32_t) { if (r < rows) d[r] = v; });
+    }
+    if (lane == 0) ok_out[ji] = 1;
+    return;
+  }
+  if (job.kind == FJ_WIDEN4) {
+    if (uint64_t(pg.val_off) + uint64_t(nn) * 4 > pg.len) { if (lane == 0) ok_out[ji] = 0; return; }
+    uint64_t* d = reinterpret_cast<uint64_t*>(flat + job.dst);
+    auto at = [&](uint32_t k) { return uint64_t(int64_t(int32_t(load_u32_unaligned(vals + uint64_t(k) * 4)))); };
+    if (!has_nulls) {
+      for (uint32_t i = lane; i < rows; i += 32) d[i] = at(i);
+    } else {
+      expand_rows(valid, rows, at, [&](uint32_t r, bool, uint64_t v, uint32_t) { if (r < rows) d[r] = v; });
     }
     if (lane == 0) ok_out[ji] = 1;
     return;
@@ -585,7 +602,7 @@ __global__ void __launch_bounds__(128) k_tuple_pack(uint8_t* __restrict__ flat, 
 // the column is then never read.  One warp per page: lane 0 walks the block headers (zigzag varints,
 // one bit width per miniblock), the warp unpacks a miniblock's deltas in parallel and turns them into
 // values with a shuffle scan carried across miniblocks.
-struct DeltaJob { uint32_t page; uint32_t _pad; uint64_t dst; uint64_t vsrc /* validity bitmap of a page with NULLs (flat-base relative), or ~0 */; uint64_t tmp /* scratch for its dense values */; };
+struct DeltaJob { uint32_t page; uint32_t sext32 /* 1: an INT32 (Date32) stream, the low word sign-extended */; uint64_t dst; uint64_t vsrc /* validity bitmap of a page with NULLs (flat-base relative), or ~0 */; uint64_t tmp /* scratch for its dense values */; };
 
 __device__ __forceinline__ bool rd_varint(const uint8_t* __restrict__ p, uint64_t& pos, uint64_t end, uint64_t& out) {
   uint64_t v = 0;
@@ -686,7 +703,8 @@ __global__ void __launch_bounds__(128) k_delta_to_plain8(const uint8_t* __restri
   int64_t* final_out = reinterpret_cast<int64_t*>(flat_base + job.dst);
   int64_t* out = has_nulls ? reinterpret_cast<int64_t*>(flat_base + job.tmp) : final_out;
   uint32_t total = 0;
-  const bool ok = dbp_decode_warp(p, pos, uint64_t(pg.len), nvals, nvals, total, [&](uint32_t i, int64_t v) { out[i] = v; });
+  const bool ok = dbp_decode_warp(p, pos, uint64_t(pg.len), nvals, nvals, total,
+                                  [&](uint32_t i, int64_t v) { out[i] = job.sext32 ? int64_t(int32_t(uint32_t(v))) : v; });
   if (has_nulls && ok) {
     __syncwarp();
     __threadfence_block();

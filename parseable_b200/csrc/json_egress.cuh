@@ -47,18 +47,26 @@ PQB_JF void jf_civil(int64_t z, int64_t& y, uint32_t& m, uint32_t& d) {
   m = mp < 10 ? mp + 3 : mp - 9;
   y += m <= 2;
 }
-// Timestamp(Millisecond, None) without the quotes; at most 32 bytes
-PQB_JF uint32_t jf_ts_ms(int64_t ms, char* out) {
-  int64_t days = ms / 86400000, rem = ms % 86400000;
-  if (rem < 0) { rem += 86400000; days -= 1; }
+// Date32 (days since 1970-01-01) without the quotes: YYYY-MM-DD, a '-' before negative years and a '+' before years above
+// 9999 (chrono prints years beyond 9999 with a sign); at most 20 bytes
+PQB_JF uint32_t jf_date32(int64_t days, char* out) {
   int64_t y; uint32_t mo, d;
   jf_civil(days, y, mo, d);
   uint32_t n = 0;
   if (y < 0) { out[n++] = '-'; y = -y; }
-  if (y > 9999) { out[n++] = '+'; n += jf_i64(y, out + n); }   // chrono prints years beyond 9999 with a sign
+  if (y > 9999) { out[n++] = '+'; n += jf_i64(y, out + n); }
   else { out[n++] = char('0' + y / 1000); out[n++] = char('0' + y / 100 % 10); out[n++] = char('0' + y / 10 % 10); out[n++] = char('0' + y % 10); }
   auto two = [&](uint32_t v) { out[n++] = char('0' + v / 10); out[n++] = char('0' + v % 10); };
-  out[n++] = '-'; two(mo); out[n++] = '-'; two(d); out[n++] = 'T';
+  out[n++] = '-'; two(mo); out[n++] = '-'; two(d);
+  return n;
+}
+// Timestamp(Millisecond, None) without the quotes: the date of jf_date32, 'T', the time; at most 32 bytes
+PQB_JF uint32_t jf_ts_ms(int64_t ms, char* out) {
+  int64_t days = ms / 86400000, rem = ms % 86400000;
+  if (rem < 0) { rem += 86400000; days -= 1; }
+  uint32_t n = jf_date32(days, out);
+  auto two = [&](uint32_t v) { out[n++] = char('0' + v / 10); out[n++] = char('0' + v % 10); };
+  out[n++] = 'T';
   const uint32_t msod = uint32_t(rem), s = msod / 1000, f = msod % 1000;
   two(s / 3600); out[n++] = ':'; two(s / 60 % 60); out[n++] = ':'; two(s % 60);
   if (f) { out[n++] = '.'; out[n++] = char('0' + f / 100); out[n++] = char('0' + f / 10 % 10); out[n++] = char('0' + f % 10); }
@@ -99,9 +107,9 @@ PQB_JF uint32_t jf_escape(const uint8_t* s, uint32_t len, char* out) {
 }
 
 constexpr int kJsonMaxCols = 64;
-enum JsonType : uint32_t { JT_I64 = 0, JT_F64 = 1, JT_BOOL = 2, JT_UTF8 = 3, JT_TS_MS = 4, JT_U64 = 5 };
+enum JsonType : uint32_t { JT_I64 = 0, JT_F64 = 1, JT_BOOL = 2, JT_UTF8 = 3, JT_TS_MS = 4, JT_U64 = 5, JT_DATE32 = 6 };
 struct JsonCol {
-  const uint8_t* values;     // 8-byte values | bit-packed booleans (words per batch) | string bytes
+  const uint8_t* values;     // 8-byte values | 4-byte values (Date32) | bit-packed booleans (words per batch) | string bytes
   const uint32_t* validity;  // bit-packed, words per batch; nullptr: no NULLs
   const int32_t* offsets;    // strings: n_rows + 1 offsets into `values`
   uint32_t type;             // JsonType
@@ -152,6 +160,12 @@ __device__ __forceinline__ uint32_t json_value(const JsonArgs& a, const JsonCol&
     case JT_TS_MS: {
       o[0] = '"';
       const uint32_t n = jf_ts_ms(reinterpret_cast<const long long*>(c.values)[i], o + 1);
+      o[n + 1] = '"';
+      return n + 2;
+    }
+    case JT_DATE32: {
+      o[0] = '"';
+      const uint32_t n = jf_date32(reinterpret_cast<const int*>(c.values)[i], o + 1);
       o[n + 1] = '"';
       return n + 2;
     }

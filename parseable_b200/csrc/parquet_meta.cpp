@@ -17,6 +17,7 @@ struct SchemaElem {
   int32_t converted = -1;
   bool logical_string = false;
   int32_t ts_unit = -1;  // 0 ms 1 us 2 ns
+  bool logical_date = false;
 };
 
 void parse_time_unit(ThriftReader& r, int32_t& unit) {
@@ -31,6 +32,7 @@ void parse_logical_type(ThriftReader& r, SchemaElem& e) {
   int16_t last = 0, id; uint8_t t;
   while (r.field(last, id, t)) {
     if (id == 1 && t == T_STRUCT) { e.logical_string = true; r.skip_struct(); }
+    else if (id == 6 && t == T_STRUCT) { e.logical_date = true; r.skip_struct(); }   // DATE
     else if (id == 8 && t == T_STRUCT) {  // TIMESTAMP
       int16_t l2 = 0, id2; uint8_t t2;
       while (r.field(l2, id2, t2)) {
@@ -167,6 +169,7 @@ void build_leaves(const std::vector<SchemaElem>& el, size_t& pos, int def, int r
     if (e.ts_unit == 0 || (e.ts_unit < 0 && e.converted == 9)) l.is_timestamp_ms = true;
     else if (e.ts_unit > 0 || e.converted == 10) l.is_timestamp_other = true;
   }
+  if (e.type == PT_INT32) l.is_date = e.logical_date || e.converted == 6;
   out.push_back(std::move(l));
 }
 

@@ -61,6 +61,7 @@ struct LeafColumn {
   bool is_string = false;        // converted UTF8 / logical STRING (or plain BYTE_ARRAY with binary_as_string)
   bool is_timestamp_ms = false;  // logical TIMESTAMP(MILLIS) / converted TIMESTAMP_MILLIS
   bool is_timestamp_other = false;
+  bool is_date = false;          // logical DATE / converted DATE (INT32 days since 1970-01-01: Arrow Date32)
 };
 
 struct FileMeta {

@@ -86,7 +86,7 @@ int satisfy(const PqLiteral& lit, int32_t cmp, const PqColumnStat& st) {
       if (st.kind != PQ_STAT_BOOL) return -1;
       vs_min = (lit.i64 != 0) - (st.min_i != 0); vs_max = (lit.i64 != 0) - (st.max_i != 0);
       break;
-    case PQ_T_I64: case PQ_T_TS_MS:   // TimestampMillisecond casts to Int (stream_schema_provider.rs:1002-1015)
+    case PQ_T_I64: case PQ_T_TS_MS: case PQ_T_DATE32:   // TimestampMillisecond and Date32 cast to Int (stream_schema_provider.rs:1002-1015)
       if (st.kind != PQ_STAT_INT) return -1;
       vs_min = lit.i64 < st.min_i ? -1 : (lit.i64 > st.min_i ? 1 : 0);
       vs_max = lit.i64 < st.max_i ? -1 : (lit.i64 > st.max_i ? 1 : 0);

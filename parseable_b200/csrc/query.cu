@@ -156,10 +156,19 @@ Tri leaf_from_stats(const HostLeaf& lf, uint8_t kind, const TableChunk& ch, uint
   if (lf.d.kind != LK_CMP || !st.has_min || !st.has_max) return TRI_MAYBE;
   int lo_c, hi_c;  // sign of compare(min, lit), compare(max, lit)
   if (kind == DK_I64) {
-    if (st.min.size() != 8 || st.max.size() != 8) return TRI_MAYBE;
     int64_t mn, mx;
-    std::memcpy(&mn, st.min.data(), 8);
-    std::memcpy(&mx, st.max.data(), 8);
+    if (st.min.size() == 8 && st.max.size() == 8) {
+      std::memcpy(&mn, st.min.data(), 8);
+      std::memcpy(&mx, st.max.data(), 8);
+    } else if (st.min.size() == 4 && st.max.size() == 4) {   // an INT32 (Date32) leaf: sign-extended like its values
+      int32_t a, b;
+      std::memcpy(&a, st.min.data(), 4);
+      std::memcpy(&b, st.max.data(), 4);
+      mn = a;
+      mx = b;
+    } else {
+      return TRI_MAYBE;
+    }
     lo_c = mn < lf.d.lit_i64 ? -1 : (mn > lf.d.lit_i64 ? 1 : 0);
     hi_c = mx < lf.d.lit_i64 ? -1 : (mx > lf.d.lit_i64 ? 1 : 0);
   } else if (kind == DK_F64) {
@@ -215,7 +224,7 @@ Tri tri_not(Tri a) { (void)a; return TRI_MAYBE; }
 
 const char* type_name(int t) {
   switch (t) { case PQ_T_BOOL: return "Boolean"; case PQ_T_I64: return "Int64"; case PQ_T_F64: return "Float64";
-    case PQ_T_UTF8: return "Utf8"; case PQ_T_TS_MS: return "Timestamp(ms)"; default: return "Null"; }
+    case PQ_T_UTF8: return "Utf8"; case PQ_T_TS_MS: return "Timestamp(ms)"; case PQ_T_DATE32: return "Date32"; default: return "Null"; }
 }
 
 uint32_t align_up(uint32_t v, uint32_t a) { return (v + a - 1) & ~(a - 1); }
@@ -1575,11 +1584,11 @@ void Query::run(const PqQueryDesc& d) {
     if (kind == 0xfe) {  // in no file: all NULL, take the plan's type
       kind = want == PQ_T_F64 ? DK_F64 : want == PQ_T_UTF8 ? DK_STR : want == PQ_T_BOOL ? DK_BOOL : DK_I64;
     } else {
-      bool ok = (want == PQ_T_I64 && kind == DK_I64 && !tc.is_ts) || (want == PQ_T_TS_MS && kind == DK_I64 && tc.is_ts) ||
+      bool ok = (want == PQ_T_I64 && kind == DK_I64 && !tc.is_ts && !tc.is_date) || (want == PQ_T_TS_MS && kind == DK_I64 && tc.is_ts) ||
                 (want == PQ_T_F64 && kind == DK_F64) || (want == PQ_T_UTF8 && kind == DK_STR) ||
-                (want == PQ_T_BOOL && kind == DK_BOOL) || want == PQ_T_NULL;
-      // Int64 plan type also accepts a timestamp column and vice versa (same physical values)
-      if (!ok && kind == DK_I64 && (want == PQ_T_I64 || want == PQ_T_TS_MS)) ok = true;
+                (want == PQ_T_BOOL && kind == DK_BOOL) || (want == PQ_T_DATE32 && kind == DK_I64 && tc.is_date) || want == PQ_T_NULL;
+      // Int64 plan type also accepts a timestamp column and vice versa (same physical values); a Date32 column is neither
+      if (!ok && kind == DK_I64 && !tc.is_date && (want == PQ_T_I64 || want == PQ_T_TS_MS)) ok = true;
       if (!ok) throw Error(PQ_ERR_INVALID_ARG, std::string("column '") + tc.name + "' is not " + type_name(want) + " in the Parquet files");
     }
     plan.cols[c].kind = kind;
@@ -1589,8 +1598,11 @@ void Query::run(const PqQueryDesc& d) {
     const TableColumn& tc = table->columns[tcol[c]];
     if (d.columns[c].type != PQ_T_NULL) return d.columns[c].type;
     switch (plan.cols[c].kind) { case DK_F64: return PQ_T_F64; case DK_STR: return PQ_T_UTF8; case DK_BOOL: return PQ_T_BOOL;
-      default: return tc.is_ts ? PQ_T_TS_MS : PQ_T_I64; }
+      default: return tc.is_date ? PQ_T_DATE32 : tc.is_ts ? PQ_T_TS_MS : PQ_T_I64; }
   };
+  // Date32 columns (by the plan's type, or the files' when the plan leaves it NULL): Int64 values in every kernel, 4-byte
+  // values in the results
+  auto is_date = [&](uint32_t c) { return out_type_of(c) == PQ_T_DATE32; };
 
   // ---- predicate compile ----
   std::vector<HostLeaf> leaves;
@@ -1640,10 +1652,16 @@ void Query::run(const PqQueryDesc& d) {
             lf.d.kind = LK_CMP;
             if (op.cmp < PQ_EQ || op.cmp > PQ_GE) throw Error(PQ_ERR_INVALID_ARG, "bad comparison operator");
             lf.d.cmp = uint8_t(op.cmp);
+            // Date32 compares with Date32 only (DataFusion rejects the other pairs or casts both sides to Timestamp)
+            if (is_date(uint32_t(op.col)) != (op.lit.type == PQ_T_DATE32))
+              throw Error(PQ_ERR_UNSUPPORTED, std::string("comparison of the ") + type_name(out_type_of(uint32_t(op.col))) + " column '" +
+                                                  d.columns[op.col].name + "' with a " + type_name(op.lit.type) + " literal is not on the GPU path");
+            if (op.lit.type == PQ_T_DATE32 && (op.lit.i64 < INT32_MIN || op.lit.i64 > INT32_MAX))
+              throw Error(PQ_ERR_INVALID_ARG, "Date32 literal outside int32 days");
             // literal coercion as DataFusion's type coercion does for column-vs-literal (SURVEY §8 a11)
             switch (kind) {
               case DK_I64:
-                if (op.lit.type == PQ_T_I64 || op.lit.type == PQ_T_TS_MS) lf.d.lit_i64 = op.lit.i64;
+                if (op.lit.type == PQ_T_I64 || op.lit.type == PQ_T_TS_MS || op.lit.type == PQ_T_DATE32) lf.d.lit_i64 = op.lit.i64;
                 else if (op.lit.type == PQ_T_F64 && std::nearbyint(op.lit.f64) == op.lit.f64 && op.lit.f64 >= -9223372036854775808.0 && op.lit.f64 < 9223372036854775808.0)
                   lf.d.lit_i64 = int64_t(op.lit.f64);
                 else if (op.lit.type == PQ_T_F64) {
@@ -1998,7 +2016,7 @@ void Query::run(const PqQueryDesc& d) {
         agg_out_type[a] = out_type_of(qc);
         continue;
       }
-      if (ag.fn != AG_COUNT && ag.kind != DK_I64 && ag.kind != DK_F64)
+      if (ag.fn != AG_COUNT && ((ag.kind != DK_I64 && ag.kind != DK_F64) || ((ag.fn == AG_SUM || ag.fn == AG_AVG) && is_date(qc))))
         throw Error(PQ_ERR_UNSUPPORTED, std::string("SUM/AVG over ") + type_name(out_type_of(qc)) + " is not on the GPU path");
       if (ag.fn == AG_COUNT) { agg_out_type[a] = PQ_T_I64; continue; }
       ag.acc_slot = uint8_t(n_acc);
@@ -2020,6 +2038,9 @@ void Query::run(const PqQueryDesc& d) {
       throw Error(PQ_ERR_UNSUPPORTED, "MEDIAN / PERCENTILE_CONT together with COUNT(DISTINCT) in one query is not on the GPU path");
   }
 
+  for (uint32_t k = 0; k < d.n_group_by; k++)
+    if (d.group_exprs && d.group_exprs[k].kind == PQ_KEY_DATE_BIN && is_date(uint32_t(d.group_by[k])))
+      throw Error(PQ_ERR_UNSUPPORTED, std::string("DATE_BIN over the Date32 column '") + d.columns[d.group_by[k]].name + "' is not on the GPU path");
   mark("plan compiled");
   // ---- what this query reads: bytes, NULL presence, encodings the kernels cannot take ----
   std::vector<uint8_t> col_needs_ent(ncols, 0);  // entry offsets (string leaf)
@@ -2064,6 +2085,12 @@ void Query::run(const PqQueryDesc& d) {
       refuse("column '" + cname + "': DELTA_BINARY_PACKED is decoded for INT64 columns only");
     if (shape->has_plain[s] && plan.cols[s].kind == DK_STR && shape->n_uncopied)
       refuse("column '" + cname + "': PLAIN (dictionary-fallback) string pages without a flat-store copy are not decoded on the GPU");
+    // k_scan reads a page's raw values at 8 bytes: a Date32 column the query reads (slot s) is read from its widened
+    // flat-store copy only.  An item without a flat-store copy of any of its columns goes to k_scan whole, so one such
+    // item among the query's columns refuses a query that reads a Date32 column
+    if (table->columns[shape_cols[s]].is_date && n_general)
+      refuse("Date32 column '" + cname + "' needs a flat-store copy of every page the query reads" +
+             (shape->why_general.empty() ? std::string(" (the flat kernels are switched off)") : ": " + shape->why_general));
   }
   auto filtered_on = [&](uint32_t s) {
     for (uint32_t l = 0; l < nleaves; l++)
@@ -3095,14 +3122,14 @@ void Query::run(const PqQueryDesc& d) {
       for (uint32_t k = 0; k < d.n_group_by; k++) {
         FinishKey& fk = fa.keys[k];
         const uint8_t kind = plan.cols[plan.keys[k].col].kind;
-        fk.kind = kind;
+        fk.kind = (!qk[k].is_bin && is_date(uint32_t(d.group_by[k]))) ? uint8_t(DK_I32) : kind;   // Date32: 4-byte values
         fk.stride = plan.keys[k].stride;
         fk.wstride = plan.keys[k].wstride;
         fk.card = qk[k].card;
         fk.valid_off = take(uint64_t(nbatches) * wpb * 4);
         if (kind == DK_BOOL) fk.val_off = take(uint64_t(nbatches) * wpb * 4);
         else if (kind == DK_STR) fk.val_off = take((uint64_t(n_out) + 1) * 4);
-        else fk.val_off = take(uint64_t(n_out) * 8);
+        else fk.val_off = take(uint64_t(n_out) * (fk.kind == DK_I32 ? 4 : 8));
         if (qk[k].is_bin) {
           fk.is_bin = 1;
           fk.bin_base = plan.keys[k].bin_base;
@@ -3122,10 +3149,11 @@ void Query::run(const PqQueryDesc& d) {
         fa.aggs[a] = plan.aggs[a];
         fa.nn_is_rows[a] = nn_is_rows[a];
         fa.valid_off[a] = take(uint64_t(nbatches) * wpb * 4);
-        fa.out_kind[a] = rank_min_max(plan.aggs[a]) ? DK_STR : bool_min_max(plan.aggs[a]) ? DK_BOOL : DK_I64;   // the layouts of the keys
+        fa.out_kind[a] = rank_min_max(plan.aggs[a]) ? DK_STR : bool_min_max(plan.aggs[a]) ? DK_BOOL
+                       : agg_out_type[a] == PQ_T_DATE32 ? DK_I32 : DK_I64;   // the layouts of the keys
         if (fa.out_kind[a] == DK_BOOL) fa.val_off[a] = take(uint64_t(nbatches) * wpb * 4);
         else if (fa.out_kind[a] == DK_STR) fa.val_off[a] = take((uint64_t(n_out) + 1) * 4);
-        else fa.val_off[a] = take(uint64_t(n_out) * 8);
+        else fa.val_off[a] = take(uint64_t(n_out) * (fa.out_kind[a] == DK_I32 ? 4 : 8));
       }
       // MIN / MAX over Utf8: the winning values' bytes, bounded by rows x the longest value of the numbering (any group may
       // hold the longest one)
@@ -3470,7 +3498,7 @@ void Query::run(const PqQueryDesc& d) {
             oc.ext_validity_off = fk.valid_off + uint64_t(b) * wpb * 4;
             if (fk.kind == DK_STR) { oc.ext_offsets_off = fk.val_off + uint64_t(r0) * 4; oc.ext_off = fk.data_off; }
             else if (fk.kind == DK_BOOL) oc.ext_off = fk.val_off + uint64_t(b) * wpb * 4;
-            else oc.ext_off = fk.val_off + uint64_t(r0) * 8;
+            else oc.ext_off = fk.val_off + uint64_t(r0) * (fk.kind == DK_I32 ? 4 : 8);
           } else if (c >= d.n_group_by + d.n_aggs) {   // row_number / partition_rows
             const uint32_t w = c - d.n_group_by - d.n_aggs;
             oc.name = win_names[w];
@@ -3483,7 +3511,7 @@ void Query::run(const PqQueryDesc& d) {
             oc.ext_validity_off = fa.valid_off[a] + uint64_t(b) * wpb * 4;
             if (fa.out_kind[a] == DK_STR) { oc.ext_offsets_off = fa.val_off[a] + uint64_t(r0) * 4; oc.ext_off = fa.astr[a].data_off; }
             else if (fa.out_kind[a] == DK_BOOL) oc.ext_off = fa.val_off[a] + uint64_t(b) * wpb * 4;
-            else oc.ext_off = fa.val_off[a] + uint64_t(r0) * 8;
+            else oc.ext_off = fa.val_off[a] + uint64_t(r0) * (fa.out_kind[a] == DK_I32 ? 4 : 8);
           }
           ob.cols.push_back(std::move(oc));
         }
@@ -3522,7 +3550,8 @@ void Query::run(const PqQueryDesc& d) {
       std::vector<PC> pcs;
       for (uint32_t i = 0; i < d.n_projection; i++) {
         const uint32_t qc = uint32_t(d.projection[i]);
-        pcs.push_back({qc, uint32_t(slot_of[qc]), plan.cols[slot_of[qc]].kind, d.columns[qc].name, out_type_of(qc)});
+        // a Date32 column is projected as 4-byte values (DK_I32: the output layout only, read like Int64)
+        pcs.push_back({qc, uint32_t(slot_of[qc]), is_date(qc) ? uint8_t(DK_I32) : plan.cols[slot_of[qc]].kind, d.columns[qc].name, out_type_of(qc)});
         if (pcs.back().kind == DK_STR) table->ensure_ent_off(shape_cols[slot_of[qc]], stream);
       }
       // an ordered scan without a projection returns its selected row ordinals in order
@@ -3567,7 +3596,7 @@ void Query::run(const PqQueryDesc& d) {
           pc.valid_off = take(uint64_t(nbatches) * wpb * 4);
           if (pc.kind == DK_BOOL) pc.val_off = take(uint64_t(nbatches) * wpb * 4);
           else if (pc.kind == DK_STR) pc.val_off = take((cap + 1) * 4);
-          else pc.val_off = take(cap * 8);
+          else pc.val_off = take(cap * (pc.kind == DK_I32 ? 4 : 8));
         }
         uint64_t data_lo = off;   // the string bytes of every column: [data_lo, data_hi)
         for (uint32_t c = 0; c < npc; c++) {
@@ -3777,7 +3806,7 @@ void Query::run(const PqQueryDesc& d) {
             oc.ext_validity_off = pc.valid_off + uint64_t(b) * wpb * 4;
             if (pc.kind == DK_STR) { oc.ext_offsets_off = pc.val_off + r0 * 4; oc.ext_off = pc.data_off; }
             else if (pc.kind == DK_BOOL) oc.ext_off = pc.val_off + uint64_t(b) * wpb * 4;
-            else oc.ext_off = pc.val_off + r0 * 8;
+            else oc.ext_off = pc.val_off + r0 * (pc.kind == DK_I32 ? 4 : 8);
           } else if (oc.type == PQ_T_UTF8) oc.offsets.assign(1, 0);
           ob.cols.push_back(std::move(oc));
         }
@@ -3955,7 +3984,8 @@ void Query::json(uint32_t flags, const char** out, uint64_t* len) {
   for (size_t c = 0; c < ncols; c++) {
     const OutColumn& oc = first->cols[c];
     JsonCol& jc = ja.cols[c];
-    jc.type = oc.type == PQ_T_F64 ? JT_F64 : oc.type == PQ_T_BOOL ? JT_BOOL : oc.type == PQ_T_UTF8 ? JT_UTF8 : oc.type == PQ_T_TS_MS ? JT_TS_MS : JT_I64;
+    jc.type = oc.type == PQ_T_F64 ? JT_F64 : oc.type == PQ_T_BOOL ? JT_BOOL : oc.type == PQ_T_UTF8 ? JT_UTF8 : oc.type == PQ_T_TS_MS ? JT_TS_MS
+            : oc.type == PQ_T_DATE32 ? JT_DATE32 : JT_I64;
     // "name": with the name escaped like any string
     jc.key_off = uint32_t(keys.size());
     keys.push_back('"');

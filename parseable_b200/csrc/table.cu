@@ -198,7 +198,8 @@ std::string describe_file(const PqFile& f) {
     o += "{\"name\":";
     js_str(o, l.name);
     o += ",\"phys_type\":" + std::to_string(l.phys_type) + ",\"max_def\":" + std::to_string(l.max_def) +
-         ",\"max_rep\":" + std::to_string(l.max_rep) + ",\"is_timestamp_ms\":" + (l.is_timestamp_ms ? "true" : "false") + "}";
+         ",\"max_rep\":" + std::to_string(l.max_rep) + ",\"is_timestamp_ms\":" + (l.is_timestamp_ms ? "true" : "false") +
+         ",\"is_date\":" + (l.is_date ? "true" : "false") + "}";
   }
   o += "],\"row_groups\":[";
   for (size_t g = 0; g < hf->meta.row_groups.size(); g++) {
@@ -214,7 +215,17 @@ std::string describe_file(const PqFile& f) {
            ",\"total_compressed_size\":" + std::to_string(cm.total_compressed_size) +
            ",\"data_page_offset\":" + std::to_string(cm.data_page_offset) +
            ",\"dictionary_page_offset\":" + std::to_string(cm.dictionary_page_offset) +
-           ",\"null_count\":" + std::to_string(cm.stats.null_count) + ",\"encodings\":[";
+           ",\"null_count\":" + std::to_string(cm.stats.null_count);
+      // PLAIN-encoded min / max statistics as hex (INT32: 4 bytes, INT64 / DOUBLE: 8)
+      auto hex = [](const std::string& b) {
+        static const char* d = "0123456789abcdef";
+        std::string h;
+        for (unsigned char c : b) { h.push_back(d[c >> 4]); h.push_back(d[c & 15]); }
+        return h;
+      };
+      if (cm.stats.has_min) o += ",\"stats_min\":\"" + hex(cm.stats.min) + "\"";
+      if (cm.stats.has_max) o += ",\"stats_max\":\"" + hex(cm.stats.max) + "\"";
+      o += ",\"encodings\":[";
       for (size_t e = 0; e < cm.encodings.size(); e++) o += (e ? "," : "") + std::to_string(cm.encodings[e]);
       o += "],\"pages\":[";
       if (uint64_t(cm.start()) + uint64_t(cm.total_compressed_size) > hf->size) throw Error(PQ_ERR_CORRUPT, "column chunk outside the file");
@@ -437,7 +448,7 @@ void Table::open(const PqFile* in_files, uint32_t n_files, const std::vector<std
               tc.max_bw = std::max<uint32_t>(tc.max_bw, 1);
               break;
             case ENC_DELTA_BINARY_PACKED:
-              if (leaf.phys_type != PT_INT64) throw Error(PQ_ERR_UNSUPPORTED, "column '" + colname + "': DELTA_BINARY_PACKED on a non-INT64 column");
+              if (leaf.phys_type != PT_INT64 && !leaf.is_date) throw Error(PQ_ERR_UNSUPPORTED, "column '" + colname + "': DELTA_BINARY_PACKED on a non-INT64 column");
               dp.enc = DE_DELTA;
               tc.has_delta_pages = true;
               break;
@@ -487,12 +498,16 @@ void Table::open(const PqFile* in_files, uint32_t n_files, const std::vector<std
       if (l.max_rep != 0 || l.depth != 1 || l.max_def > 1)
         throw Error(PQ_ERR_UNSUPPORTED, "column '" + col_names[c] + "' is nested; only flat columns are on the GPU path");
       uint8_t k = kind_of_leaf(l);
-      if (k == 0xff || k == DK_I32 || k == DK_F32)
+      if (k == 0xff || (k == DK_I32 && !l.is_date) || k == DK_F32)
         throw Error(PQ_ERR_UNSUPPORTED, "column '" + col_names[c] + "': physical type " + std::to_string(l.phys_type) + " not supported");
+      // Date32: INT32 days, widened to the flat store's sign-extended 8-byte values when the table is opened
+      // (build_flat_store, ensure_plain8), so that every kernel past the flat store sees an Int64 column
+      if (k == DK_I32) k = DK_I64;
       if (columns[c].kind == 0xff) {
         columns[c].kind = k;
         columns[c].is_ts = l.is_timestamp_ms;
-      } else if (columns[c].kind != k) {
+        columns[c].is_date = l.is_date;
+      } else if (columns[c].kind != k || columns[c].is_date != l.is_date) {
         throw Error(PQ_ERR_UNSUPPORTED, "column '" + col_names[c] + "' changes physical type across files");
       }
       if (l.is_timestamp_other)
@@ -562,7 +577,7 @@ void Table::open(const PqFile* in_files, uint32_t n_files, const std::vector<std
                 case ENC_PLAIN: dp.enc = DE_PLAIN; tc.has_plain_pages = true; break;
                 case ENC_RLE_DICTIONARY: case ENC_PLAIN_DICTIONARY: dp.enc = DE_DICT; tc.has_dict_pages = true; break;
                 case ENC_DELTA_BINARY_PACKED:
-                  if (leaf.phys_type != PT_INT64) throw Error(PQ_ERR_UNSUPPORTED, "column '" + col_names[c] + "': DELTA_BINARY_PACKED on a non-INT64 column");
+                  if (leaf.phys_type != PT_INT64 && !leaf.is_date) throw Error(PQ_ERR_UNSUPPORTED, "column '" + col_names[c] + "': DELTA_BINARY_PACKED on a non-INT64 column");
                   dp.enc = DE_DELTA; tc.has_delta_pages = true; break;
                 case ENC_DELTA_BYTE_ARRAY: case ENC_DELTA_LENGTH_BYTE_ARRAY:
                   if (leaf.phys_type != PT_BYTE_ARRAY) throw Error(PQ_ERR_UNSUPPORTED, "column '" + col_names[c] + "': DELTA_BYTE_ARRAY on a non-BYTE_ARRAY column");
@@ -972,10 +987,11 @@ void Table::build_flat_store(cudaStream_t stream) {
       TableChunk& tc = rg.chunks[c];
       if (!tc.present) continue;
       const uint8_t kind = columns[c].kind;
+      const bool wide4 = columns[c].is_date;   // INT32 values: widened (sign-extended) to 8 bytes
       if (tc.dict_n && (kind == DK_I64 || kind == DK_F64)) {
-        if (uint64_t(tc.dict_n) * 8 > tc.dict_len)
+        if (uint64_t(tc.dict_n) * (wide4 ? 4 : 8) > tc.dict_len)
           throw Error(PQ_ERR_CORRUPT, "column '" + columns[c].name + "': dictionary page shorter than its entry count");
-        js.push_back({tc.dict_off, take(1, uint64_t(tc.dict_n) * 8), kNone, kNone, 0u, 4u /*FJ_DICT8*/, tc.dict_n, 1u});
+        js.push_back({tc.dict_off, take(1, uint64_t(tc.dict_n) * 8), kNone, kNone, 0u, wide4 ? 7u /*FJ_DICT4*/ : 4u /*FJ_DICT8*/, tc.dict_n, 1u});
         tc.dict8_off = js.size() - 1;   // job index for now, resolved below
       }
       for (uint32_t k = 0; k < tc.pages.n_pages; k++) {
@@ -995,7 +1011,7 @@ void Table::build_flat_store(cudaStream_t stream) {
         } else if (pg.enc == DE_PLAIN && (kind == DK_I64 || kind == DK_F64)) {
           fr.fkind = FK_PLAIN8;
           fr.bw = 64;
-          J j{0, take(1, uint64_t(pg.num_rows) * 8), kNone, kNone, pi, 2u /*FJ_COPY8*/, pg.num_rows, 1u};
+          J j{0, take(1, uint64_t(pg.num_rows) * 8), kNone, kNone, pi, wide4 ? 8u /*FJ_WIDEN4*/ : 2u /*FJ_COPY8*/, pg.num_rows, 1u};
           if (nul) j.voff = take(0, vbytes);
           js.push_back(j);
         } else if (pg.enc == DE_PLAIN && kind == DK_BOOL) {
@@ -1032,14 +1048,23 @@ void Table::build_flat_store(cudaStream_t stream) {
   for (size_t i = 0; i < js.size(); i++) {
     const uint64_t dst = js[i].zone ? zone1 + js[i].off : js[i].off;
     dj[i] = {js[i].src, dst, js[i].voff, js[i].toff == kNone ? kNone : zone2 + js[i].toff, js[i].page, js[i].kind, js[i].rows, 0u};
-    if (js[i].kind == 4u) continue;
+    if (js[i].kind == 4u || js[i].kind == 7u) continue;
     FlatPageRec& fr = flat_pages[js[i].page];
     fr.voff = js[i].voff;
     if (js[i].kind != 5u) fr.off = dst;
   }
   for (TableRowGroup& rg : row_groups)
-    for (TableChunk& tc : rg.chunks)
-      if (tc.present && tc.dict8_off != ~0ull) tc.dict8_off = dj[tc.dict8_off].dst;
+    for (size_t c = 0; c < rg.chunks.size(); c++) {
+      TableChunk& tc = rg.chunks[c];
+      if (!tc.present || tc.dict8_off == ~0ull) continue;
+      tc.dict8_off = dj[tc.dict8_off].dst;
+      if (columns[c].is_date) {
+        // the readers of raw dictionary entries (entry offsets for key interning, the leaf LUTs) take 8-byte entries:
+        // a Date32 chunk's dictionary is its widened copy from here on (an arena offset that wraps, like d_strmat's pages)
+        tc.dict_off = uint64_t(reinterpret_cast<uintptr_t>(d_flat) + tc.dict8_off - reinterpret_cast<uintptr_t>(d_arena));
+        tc.dict_len = tc.dict_n * 8;
+      }
+    }
   void* d_jobs = nullptr;
   uint8_t* d_ok = nullptr;
   uint32_t* d_maxlen = nullptr;
@@ -1070,7 +1095,7 @@ void Table::build_flat_store(cudaStream_t stream) {
     }
   size_t n_ok = 0, n_nul = 0;
   for (size_t i = 0; i < dj.size(); i++) {
-    if (dj[i].kind == 4u) continue;
+    if (dj[i].kind == 4u || dj[i].kind == 7u) continue;
     if (ok[i]) { n_ok += dj[i].kind != 5u; n_nul += dj[i].vdst != kNone; }
     else {
       // a run header past the page, a length prefix past the page, a stream that stops early: the reference's reader fails such a file
@@ -1273,7 +1298,7 @@ void Table::ensure_plain8(int tcol, cudaStream_t stream) const {
   std::lock_guard<std::mutex> lk(side_mu);
   ColSide& cs = sides[tcol];
   if (cs.delta_ready || !cs.has_delta) return;
-  struct Job { uint32_t page, pad; uint64_t dst, vsrc, tmp; };   // == DeltaJob; offsets relative to d_flat
+  struct Job { uint32_t page, sext32; uint64_t dst, vsrc, tmp; };   // == DeltaJob; offsets relative to d_flat
   std::vector<Job> jobs;
   uint64_t off = 0;
   FlatPageRec blank{};
@@ -1286,7 +1311,7 @@ void Table::ensure_plain8(int tcol, cudaStream_t stream) const {
     for (uint32_t k = 0; k < tc.pages.n_pages; k++) {
       const uint32_t pi = tc.pages.first_page + k;
       if (pages[pi].enc != DE_DELTA || flat_pages[pi].fkind != FK_NONE) continue;
-      Job j{pi, 0u, take(uint64_t(pages[pi].num_rows) * 8), flat_pages[pi].voff, ~0ull};
+      Job j{pi, columns[tcol].is_date ? 1u : 0u, take(uint64_t(pages[pi].num_rows) * 8), flat_pages[pi].voff, ~0ull};
       if (j.vsrc != ~0ull) j.tmp = take(uint64_t(pages[pi].num_rows) * 8);
       jobs.push_back(j);
     }

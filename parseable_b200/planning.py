@@ -192,6 +192,8 @@ def _cast_or_none(v):
         return "bool", v
     if isinstance(v, Timestamp):
         return "int", v.ms
+    if isinstance(v, _dt.date) and not isinstance(v, _dt.datetime):   # Date32 casts to Int (days): :1011
+        return "int", (v - _dt.date(1970, 1, 1)).days
     if isinstance(v, int):
         return "int", v
     if isinstance(v, float):

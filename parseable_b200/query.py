@@ -15,6 +15,7 @@ into pyarrow.  There is no CPU execution path in this module.
 from __future__ import annotations
 
 import ctypes as C
+import datetime as _dt
 import re
 from dataclasses import dataclass, field
 from typing import Any, Iterable, Sequence
@@ -24,6 +25,8 @@ import pyarrow as pa
 from . import _lib as L
 
 DEFAULT_TIMESTAMP_KEY = "p_timestamp"  # src/event/mod.rs DEFAULT_TIMESTAMP_KEY
+_EPOCH_DAY = _dt.date(1970, 1, 1)   # day 0 of a Date32 literal
+_DATE_LITERAL = re.compile(r"\d{4}-\d{2}-\d{2}")   # DATE 'YYYY-MM-DD'
 
 
 class QueryError(RuntimeError):
@@ -196,6 +199,8 @@ class _Desc:
             out.type, out.i64 = L.PQ_T_BOOL, int(v)
         elif isinstance(v, Timestamp):
             out.type, out.i64 = L.PQ_T_TS_MS, int(v.ms)
+        elif isinstance(v, _dt.date) and not isinstance(v, _dt.datetime):
+            out.type, out.i64 = L.PQ_T_DATE32, (v - _EPOCH_DAY).days
         elif isinstance(v, int):
             out.type, out.i64 = L.PQ_T_I64, v
         elif isinstance(v, float):
@@ -315,6 +320,8 @@ def _pq_type(t: pa.DataType | None) -> int:
         t = t.value_type
     if pa.types.is_timestamp(t):
         return L.PQ_T_TS_MS
+    if pa.types.is_date32(t):
+        return L.PQ_T_DATE32
     return _ARROW_TO_PQ.get(t, L.PQ_T_NULL)
 
 
@@ -937,6 +944,14 @@ class Query:
             return lit(float(t[1]) if any(c in t[1] for c in ".eE") else int(t[1]))
         if t[0] == "str":
             return lit(t[1])
+        if t[0] == "id" and t[1].upper() == "DATE" and self._peek()[0] == "str":   # DATE 'YYYY-MM-DD': a Date32 literal
+            s = self._next("str")[1]
+            try:   # fromisoformat alone also takes 20200102 and ISO week dates
+                if not _DATE_LITERAL.fullmatch(s):
+                    raise ValueError
+                return lit(_dt.date.fromisoformat(s))
+            except ValueError:
+                raise QueryError(L.PQ_ERR_INVALID_ARG, f"DATE {s!r} is not a YYYY-MM-DD date") from None
         if t[0] == "id":
             return col(t[1])
         if t == ("kw", "TRUE"):

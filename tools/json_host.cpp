@@ -14,6 +14,7 @@ void jh_format_f64_many(const double* v, uint64_t n, char* out /* 32 bytes each,
 }
 uint32_t jh_format_i64(int64_t v, char* out) { return pqb::jf_i64(v, out); }
 uint32_t jh_format_ts_ms(int64_t v, char* out) { return pqb::jf_ts_ms(v, out); }
+uint32_t jh_format_date32(int32_t v, char* out) { return pqb::jf_date32(v, out); }
 uint32_t jh_escape(const uint8_t* s, uint32_t n, char* out) {
   const uint32_t want = pqb::jf_escaped_len(s, n), got = pqb::jf_escape(s, n, out);
   return want == got ? got : 0xffffffffu;

@@ -30,7 +30,6 @@ void release_schema(ArrowSchema* s) {
 
 struct ArrayPriv {
   std::shared_ptr<PinnedBlock> keep;
-  std::vector<std::vector<uint8_t>> owned;
   std::vector<const void*> buffers;
   std::vector<ArrowArray> children;
   std::vector<ArrowArray*> child_ptrs;
@@ -94,39 +93,12 @@ void export_batch(const OutBatch& b, ArrowArray* out, ArrowSchema* schema) {
     std::memset(&a, 0, sizeof(a));
     a.length = b.rows;
     a.null_count = c.null_count;
-    if (c.ext_all) {
-      // device-assembled column: validity, [offsets], data all alias the page-locked block
-      p->keep = c.ext;
-      const uint8_t* base = c.ext->p;
-      p->buffers.push_back(c.null_count ? static_cast<const void*>(base + c.ext_validity_off) : nullptr);
-      if (c.type == PQ_T_UTF8) p->buffers.push_back(base + c.ext_offsets_off);
-      p->buffers.push_back(base + c.ext_off);
-      a.n_buffers = int64_t(p->buffers.size());
-      a.buffers = p->buffers.data();
-      a.release = release_array;
-      a.private_data = p;
-      top->child_ptrs.push_back(&a);
-      continue;
-    }
-    // buffers: validity, [offsets], data
-    if (c.null_count) { p->owned.push_back(c.validity); } else { p->owned.emplace_back(); }
-    if (c.type == PQ_T_UTF8) {
-      std::vector<uint8_t> offs(c.offsets.size() * 4);
-      if (!offs.empty()) std::memcpy(offs.data(), c.offsets.data(), offs.size());
-      else { offs.assign(4, 0); }
-      p->owned.push_back(std::move(offs));
-    }
-    if (c.ext) { p->keep = c.ext; p->owned.emplace_back(); }
-    else {
-      p->owned.push_back(c.values);
-      if (p->owned.back().empty()) p->owned.back().assign(8, 0);  // never hand out a NULL data pointer
-    }
-    for (size_t k = 0; k < p->owned.size(); k++) {
-      const void* ptr = static_cast<const void*>(p->owned[k].data());
-      if (k == 0 && !c.null_count) ptr = nullptr;
-      if (c.ext && k + 1 == p->owned.size()) ptr = c.ext->p + c.ext_off;
-      p->buffers.push_back(ptr);
-    }
+    // validity, [offsets], data: every buffer aliases the column's block
+    p->keep = c.block;
+    const uint8_t* base = c.block->p;
+    p->buffers.push_back(c.null_count ? static_cast<const void*>(base + c.validity_off) : nullptr);
+    if (c.type == PQ_T_UTF8) p->buffers.push_back(base + c.offsets_off);
+    p->buffers.push_back(base + c.values_off);
     a.n_buffers = int64_t(p->buffers.size());
     a.buffers = p->buffers.data();
     a.release = release_array;

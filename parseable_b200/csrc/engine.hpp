@@ -318,28 +318,26 @@ void build_key_side(const Table& t, int tcol, ColSide& side, cudaStream_t stream
 void unify_key_side(const Table& t, int tcol, ColSide& side, cudaStream_t stream);
 void build_rank_luts(const ColSide& side, bool agreed, const uint32_t* rank, RankLuts& luts, cudaStream_t stream);
 
-// page-locked host block that result batches can alias (zero copy); returns to the pool when
-// the last batch that references it is released by the consumer
+// host block that result batches alias (zero copy): page-locked from the context's pool, or (one-row and empty results)
+// ordinary heap memory, so that a small result does not hold a pool block of 1 MB or more while the consumer keeps it.
+// A pool block returns to the pool when the last batch that references it is released by the consumer
 struct PinnedBlock {
   uint8_t* p = nullptr;
   size_t bytes = 0;
-  uint8_t* dev = nullptr;   // the device block this one was copied from, while the query keeps it (JSON egress reads it there)
+  uint8_t* dev = nullptr;        // the device block this one was copied from, while the query keeps it (JSON egress reads it there)
+  std::vector<uint64_t> heap;    // a heap block: p points into it
   ~PinnedBlock();
 };
 
+// one column of one batch: a slice of a result block (laid out by query.cu's BlockLayout)
 struct OutColumn {
   std::string name;
   int type = PQ_T_I64;               // PqType
-  std::vector<uint8_t> values;       // 8-byte values, bit-packed bools, or utf8 bytes
-  std::shared_ptr<PinnedBlock> ext;  // when set, the values are ext->p + ext_off (not `values`)
-  size_t ext_off = 0;
-  std::vector<int32_t> offsets;      // utf8
-  std::vector<uint8_t> validity;     // empty when null_count == 0
+  std::shared_ptr<PinnedBlock> block;
+  size_t values_off = 0;             // 8-byte values (4-byte Date32), bit-packed bools, or utf8 bytes
+  size_t validity_off = 0;           // validity bitmap (used when null_count != 0)
+  size_t offsets_off = 0;            // utf8: int32 offsets of this batch's first row (n + 1 entries follow)
   int64_t null_count = 0;
-  // device-assembled results: every buffer of the column lives in `ext`
-  bool ext_all = false;
-  size_t ext_validity_off = 0;       // validity bitmap (used when null_count != 0)
-  size_t ext_offsets_off = 0;        // utf8: int32 offsets of this batch's first row (n + 1 entries follow)
 };
 
 struct OutBatch {

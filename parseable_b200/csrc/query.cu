@@ -1490,15 +1490,142 @@ uint64_t pct_finish(DevBuf<uint32_t>& slots, DevBuf<unsigned long long>& keys, u
   return launches;
 }
 
+// ---- the result tail: what the queued scan leaves on the device, turned into result batches ----
+// A GROUP BY key of the query
+struct QKey { const KeyDict* kd = nullptr; uint32_t card = 0; bool is_bin = false; };
+
+// a window's extra columns: Int64, never NULL, after the other columns of the result
+std::vector<std::string> window_columns(const PqWindow* win) {
+  std::vector<std::string> names;
+  if (win && (win->flags & PQ_WINDOW_ROW_NUMBER)) names.push_back("row_number");
+  if (win && (win->flags & PQ_WINDOW_PARTITION_ROWS)) names.push_back("partition_rows");
+  return names;
+}
+
+// A result block holds every buffer of every batch of a result, in 64-byte aligned regions taken in order: first the NULL
+// counts (u32 per column and batch), then per column its validity (words per batch) and its values: 8 bytes per row (4
+// for Date32), int32 offsets (rows + 1) for strings, bit-packed words per batch for booleans.  String bytes, window
+// columns and the device-only scratch behind the copied part are taken where each result places them.
+struct BlockCol {
+  std::string name;
+  int type = PQ_T_I64;      // PqType
+  uint8_t kind = DK_I64;    // DevKind of the layout (DK_I32: a Date32 column, 4-byte values)
+  uint64_t valid_off = 0, val_off = 0, data_off = 0;   // data_off: a string column's bytes
+};
+struct BlockLayout {
+  uint64_t rows = 0;        // the rows the block has room for
+  uint32_t batch_rows = 1, nbatches = 0, wpb = 0;
+  uint32_t ncolumns = 0;    // the columns of the NULL-count table
+  uint64_t off = 0, nulls_off = 0;
+  uint64_t copy_bytes = 0;  // the part that is copied back
+  BlockLayout() = default;
+  BlockLayout(uint64_t n, uint32_t br, uint32_t ncol)
+      : rows(n), batch_rows(br), nbatches(uint32_t((n + br - 1) / br)), wpb((br + 31) / 32), ncolumns(ncol) {
+    nulls_off = take(uint64_t(ncol) * nbatches * 4);
+  }
+  uint64_t take(uint64_t bytes) { const uint64_t o = off; off = (off + bytes + 63) & ~63ull; return o; }
+  uint64_t per_row(uint64_t bytes) { return take(rows * bytes); }
+  void column(BlockCol& c) {   // its validity, then its values
+    const uint64_t bitmap = uint64_t(nbatches) * wpb * 4;
+    c.valid_off = take(bitmap);
+    c.val_off = c.kind == DK_BOOL ? take(bitmap) : c.kind == DK_STR ? take((rows + 1) * 4) : per_row(c.kind == DK_I32 ? 4 : 8);
+  }
+};
+
+// a zeroed block in ordinary memory, for a result laid out on the host (one row, or an empty batch)
+std::shared_ptr<PinnedBlock> heap_block(uint64_t bytes) {
+  auto b = std::make_shared<PinnedBlock>();
+  b->heap.assign(std::max<uint64_t>(bytes / 8, 1), 0);
+  b->p = reinterpret_cast<uint8_t*>(b->heap.data());
+  b->bytes = b->heap.size() * 8;
+  return b;
+}
+
+void host_mark(bool verbose, std::chrono::steady_clock::time_point t_begin, const char* what) {   // PQB_VERBOSE: host timeline of a query
+  if (verbose)
+    fprintf(stderr, "[pqb] +%.3f ms %s\n", std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(), what);
+}
+
+// What the result tail reads of the planned query and its queued scan (Query::run fills it), and the tail: one function
+// per result shape (groups: an aggregate table; rows: a projection or an ordered scan; selection: selected row ids or
+// a COUNT(*) row), then finish() for the timings
+struct ResultTail {
+  const PqQueryDesc& d;
+  const Table* table;
+  Shape& shape;
+  DevPlan& plan;
+  const std::vector<DevItem>& items;
+  const std::vector<int>& out_type;     // query column -> its result type (PqType)
+  const std::vector<int>& slot_of;      // query column -> column slot
+  const std::vector<int>& shape_cols;   // column slot -> table column
+  const std::vector<QKey>& qk;
+  const std::vector<uint8_t>& nn_is_rows;
+  const std::vector<int>& agg_out_type;
+  const std::vector<double>& pct_p;
+  const std::vector<std::shared_ptr<const RankLuts>>& rank_luts;
+  const std::vector<uint8_t>& lit_pool;
+  const std::shared_ptr<const TuplePages>& tuple;
+  DevBuf<unsigned long long>& d_acc;
+  DevBuf<unsigned long long>& d_hkeys;
+  DevBuf<unsigned long long>& d_counters;
+  DevBuf<uint32_t>& d_bitmap;
+  DevBuf<uint32_t>& d_item_counts;
+  DevBuf<unsigned int>& d_pct_count;
+  std::vector<DevBuf<uint32_t>>& d_pct_slots;
+  std::vector<DevBuf<unsigned long long>>& d_pct_keys;
+  RowOrderArgs& roa;
+  const uint8_t* row_nulls_first;
+  DevBuf<FlatPageRec>& d_opages;
+  Timer& t_all;
+  Timer& t_scan;
+  const uint32_t cells, ncols, nrg;
+  const uint64_t key_space;
+  const bool allreduce, multi, merge_rows;
+  uint64_t launches;
+  cudaStream_t stream;
+  const bool verbose;
+  const std::chrono::steady_clock::time_point t_begin;
+  PqMetrics& metrics;
+  std::vector<OutBatch>& batches;
+  std::vector<std::shared_ptr<PinnedBlock>>& dev_blocks;   // result blocks whose device copy is kept until the query closes
+  // from the query
+  const PqWindow* const win = d.window;
+  const uint32_t n_part = win ? win->n_partition_by : 0;
+  const bool ordered = d.n_order_by > 0 || win;
+  const bool row_order = ordered && !d.n_aggs;
+  const bool want_rows = d.n_aggs == 0 && !(d.flags & PQ_QUERY_COUNT_ONLY);
+  const uint32_t batch_rows = d.batch_size ? d.batch_size : 20000;
+  const unsigned long long lim = d.limit >= 0 ? (unsigned long long)d.limit : ~0ull;
+  const std::vector<std::string> win_names = window_columns(win);
+  Context& ctx = Context::get();
+  // the scan's counters and the rows it selected
+  unsigned long long h_counters[4] = {0, 0, 0, 0};
+  unsigned long long total = 0;
+  DevBuf<unsigned long long> d_item_base, d_total;
+
+  void groups();
+  void rows();
+  void selection();
+  void finish();
+
+  void mark(const char* what) const { host_mark(verbose, t_begin, what); }
+  void count_selected();
+  void check_corrupt() const;
+  std::string agg_name(uint32_t a) const;
+  uint8_t agg_kind(uint32_t a) const;
+  void keep_device(const std::shared_ptr<PinnedBlock>& block, DevBuf<uint8_t>& d_block, uint64_t bytes);
+  template <class Fill>
+  unsigned long long sized_pass(unsigned long long min_cap, std::shared_ptr<PinnedBlock>& block, Fill fill, const char* then);
+  void one_row(std::vector<BlockCol> cols, const std::vector<bool>& null, unsigned long long value);
+  void slice(const BlockLayout& L, const std::vector<BlockCol>& cols, const std::shared_ptr<PinnedBlock>& block, uint64_t n);
+};
+
 }  // namespace
 
 void Query::run(const PqQueryDesc& d) {
   const auto t_begin = std::chrono::steady_clock::now();
   const char* vb = getenv("PQB_VERBOSE"); const bool verbose = vb && vb[0] && vb[0] != '0';
-  auto mark = [&](const char* what) {   // PQB_VERBOSE: host timeline of this query
-    if (verbose)
-      fprintf(stderr, "[pqb] +%.3f ms %s\n", std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(), what);
-  };
+  auto mark = [&](const char* what) { host_mark(verbose, t_begin, what); };
   struct HostTimer {
     std::chrono::steady_clock::time_point t0;
     PqMetrics* m;
@@ -2285,7 +2412,6 @@ void Query::run(const PqQueryDesc& d) {
   }
 
   // ---- GROUP BY keys: interned per table column (cached with the table) ----
-  struct QKey { const KeyDict* kd = nullptr; uint32_t card = 0; bool is_bin = false; };
   std::vector<QKey> qk(d.n_group_by);
   std::vector<uint8_t> row_keys(d.n_group_by, 0);   // the key column has pages without a dictionary: per-row ids (FK_IDS pages)
   plan.nkeys = d.n_group_by;
@@ -3050,893 +3176,819 @@ void Query::run(const PqQueryDesc& d) {
   mark("scan queued");
 
   // ---- results ----
-  const uint32_t batch_rows = d.batch_size ? d.batch_size : 20000;
-  batch_rows_ = batch_rows;
-  unsigned long long h_counters[4] = {0, 0, 0, 0};
-  if (agg_kernel) {
-    // multi-GPU: the partial tables meet in ONE grouped all-reduce (SURVEY §8e): one NCCL launch,
-    // per array the reduction its aggregate needs
-    Timer t_ar;
-    std::unique_ptr<MergeRun> merge;   // a hashed GROUP BY: every rank's listed groups gathered and merged instead
-    if (allreduce && plan.hashed) {
-      merge = std::make_unique<MergeRun>();
-      launches += merge->run(plan, cells, key_space, std::min<uint64_t>(plan.nslots, std::max<uint64_t>(metrics.rows_scanned, 1)),
-                             d_acc, d_hkeys, d_counters.p, stream, metrics);
-    } else if (allreduce) {
-      PQB_CUDA(cudaEventRecord(t_ar.a, stream));
-      comm_group_begin();
-      comm_allreduce_u64(d_acc.p, plan.nslots, 0, stream);
-      for (uint32_t a = 0; a < plan.n_acc; a++) {
-        uint8_t how = plan.acc_init[a];
-        comm_allreduce_u64(d_acc.p + size_t(1 + a) * plan.nslots, plan.nslots, how == 0 ? 0 : how == 1 ? 3 : how == 2 ? 1 : 2, stream);
-      }
-      if (plan.n_nn) comm_allreduce_u64(d_acc.p + size_t(1 + plan.n_acc) * plan.nslots, size_t(plan.n_nn) * plan.nslots, 0, stream);
-      comm_group_end();
-      PQB_CUDA(cudaEventRecord(t_ar.b, stream));
+  batch_rows_ = d.batch_size ? d.batch_size : 20000;
+  std::vector<int> out_type(d.n_columns);
+  for (uint32_t c = 0; c < d.n_columns; c++) out_type[c] = out_type_of(c);
+  ResultTail tail{d, table, *shape, plan, items, out_type, slot_of, shape_cols, qk, nn_is_rows, agg_out_type, pct_p, rank_luts,
+                  lit_pool, tuple, d_acc, d_hkeys, d_counters, d_bitmap, d_item_counts, d_pct_count, d_pct_slots, d_pct_keys,
+                  roa, row_nulls_first, d_opages, t_all, t_scan, cells, ncols, nrg, key_space, allreduce, multi, merge_rows,
+                  launches, stream, verbose, t_begin, metrics, batches_, dev_blocks_};
+  if (agg_kernel) tail.groups();
+  else if (projecting || row_order) tail.rows();
+  else tail.selection();
+  tail.finish();
+}
+
+// ---- the result tail ----
+void ResultTail::check_corrupt() const {
+  if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
+}
+
+std::string ResultTail::agg_name(uint32_t a) const {
+  static const char* fn_names[] = {"count(*)", "count", "sum", "min", "max", "avg", "count(distinct", "median", "percentile_cont"};
+  const DevAgg& ag = plan.aggs[a];
+  if (ag.fn == AG_PERCENTILE_CONT) {   // p in shortest round-trip form: percentile_cont(latency_ms, 0.99)
+    char buf[32];
+    const auto r = std::to_chars(buf, buf + sizeof(buf), pct_p[a]);
+    return std::string("percentile_cont(") + d.columns[d.aggs[a].col].name + ", " + std::string(buf, r.ptr) + ")";
+  }
+  return ag.fn == AG_COUNT_STAR ? std::string("count(*)")
+                                : std::string(fn_names[ag.fn]) + (ag.fn == AG_COUNT_DISTINCT ? " " : "(") + d.columns[d.aggs[a].col].name + ")";
+}
+
+// an aggregate's output layout: MIN / MAX over Utf8 or Boolean, or (MIN / MAX over Date32) 4-byte values, like the keys'
+uint8_t ResultTail::agg_kind(uint32_t a) const {
+  return rank_min_max(plan.aggs[a]) ? DK_STR : bool_min_max(plan.aggs[a]) ? DK_BOOL : agg_out_type[a] == PQ_T_DATE32 ? DK_I32 : DK_I64;
+}
+
+// a result block up to kKeepDeviceResult stays on the device until the query closes: JSON egress formats it where it is
+void ResultTail::keep_device(const std::shared_ptr<PinnedBlock>& block, DevBuf<uint8_t>& d_block, uint64_t bytes) {
+  if (!block || !d_block.p || bytes > kKeepDeviceResult) return;
+  block->dev = d_block.p;
+  d_block.p = nullptr;
+  dev_blocks.push_back(block);
+}
+
+// The batches of the first n rows of a block laid out by L, which may have room for more (an empty result: one batch
+// of no rows).  The NULL counts are indexed by the batches of the layout, not by the batches the rows fill.
+void ResultTail::slice(const BlockLayout& L, const std::vector<BlockCol>& cols, const std::shared_ptr<PinnedBlock>& block, uint64_t n) {
+  const uint32_t* nulls = reinterpret_cast<const uint32_t*>(block->p + L.nulls_off);
+  for (uint64_t b = 0, r0 = 0; r0 < n || b == 0; b++, r0 += L.batch_rows) {
+    OutBatch ob;
+    ob.rows = int64_t(std::min<uint64_t>(L.batch_rows, n - r0));
+    for (size_t c = 0; c < cols.size(); c++) {
+      const BlockCol& bc = cols[c];
+      OutColumn oc;
+      oc.name = bc.name;
+      oc.type = bc.type;
+      oc.block = block;
+      oc.null_count = ob.rows && c < L.ncolumns ? nulls[c * L.nbatches + b] : 0;
+      oc.validity_off = bc.valid_off + b * L.wpb * 4;
+      if (bc.kind == DK_STR) { oc.offsets_off = bc.val_off + r0 * 4; oc.values_off = bc.data_off; }
+      else if (bc.kind == DK_BOOL) oc.values_off = bc.val_off + b * L.wpb * 4;
+      else oc.values_off = bc.val_off + r0 * (bc.kind == DK_I32 ? 4 : 8);
+      ob.cols.push_back(std::move(oc));
     }
-    // ---- non-empty groups in ascending slot order (deterministic: the mixed radix of the group ids) ----
-    const uint32_t ntiles = (plan.nslots + kSlotTile - 1) / kSlotTile;
-    const uint64_t out_cap = std::min<uint64_t>(plan.nslots, std::max<uint64_t>(allreduce ? plan.nslots : metrics.rows_scanned, 1));
-    DevBuf<uint32_t> d_tile_counts, d_out_slot;
-    DevBuf<unsigned long long> d_tile_base, d_totals;
-    d_tile_counts.alloc(ntiles, stream);
-    d_tile_base.alloc(ntiles, stream);
-    d_totals.alloc(2, stream);
-    d_out_slot.alloc(out_cap, stream);
-    const uint32_t* order = tuple ? tuple->d_order : nullptr;   // tuple slots: listed in the order of their mixed-radix ids
-    k_slot_tile_counts<<<ntiles, 256, 0, stream>>>(d_acc.p, plan.nslots, d_tile_counts.p, order);
-    k_item_prefix<<<1, 1024, 0, stream>>>(d_tile_counts.p, ntiles, d_tile_base.p, d_totals.p);
-    k_slot_compact<<<ntiles, 256, 0, stream>>>(d_acc.p, plan.nslots, d_tile_base.p, d_out_slot.p, order);
-    // rows this rank selected (its own items)
-    DevBuf<unsigned long long> d_item_base;
-    d_item_base.alloc(std::max<size_t>(items.size(), 1), stream);
-    if (!items.empty()) k_item_prefix<<<1, 1024, 0, stream>>>(d_item_counts.p, uint32_t(items.size()), d_item_base.p, d_totals.p + 1);
-    else PQB_CUDA(cudaMemsetAsync(d_totals.p + 1, 0, 8, stream));
-    launches += 4;
-    // a window's extra columns: Int64, never NULL, after the keys and aggregates
-    std::vector<std::string> win_names;
-    if (win && (win->flags & PQ_WINDOW_ROW_NUMBER)) win_names.push_back("row_number");
-    if (win && (win->flags & PQ_WINDOW_PARTITION_ROWS)) win_names.push_back("partition_rows");
-    std::unique_ptr<WindowRun> wrun;       // only for a query with a window over at least one group
-    // ---- the result block: every buffer of every batch for n_out groups, assembled on the device and copied to page-locked
-    // memory (no synchronise).  n_dev != nullptr: n_out is a capacity, the kernels read the group count on the device.
-    // cut: ORDER BY ... LIMIT keeps a subset of the groups ----
-    struct Assembled {
-      uint32_t rows = 0;   // the groups the block has room for (0: none assembled)
-      FinishArgs fa{};
-      uint32_t nbatches = 0, wpb = 0, ncolumns = 0;
-      uint64_t nulls_off = 0, copy_bytes = 0, win_off[2] = {0, 0};
-      std::unique_ptr<DevBuf<uint8_t>> d_block;
-      std::shared_ptr<PinnedBlock> block;
-    };
-    auto assemble = [&](uint32_t n_out, const unsigned long long* n_dev) -> Assembled {
-      Assembled r;
-      r.rows = n_out;
-      FinishArgs& fa = r.fa;
-      const uint32_t nbatches = (n_out + batch_rows - 1) / batch_rows;
-      const uint32_t wpb = (batch_rows + 31) / 32;
-      const uint32_t ncolumns = d.n_group_by + d.n_aggs + uint32_t(win_names.size());
-      uint64_t off = 0;
-      auto take = [&](uint64_t bytes) { uint64_t o = off; off = (off + bytes + 63) & ~63ull; return o; };
-      const uint64_t nulls_off = take(uint64_t(ncolumns) * nbatches * 4);
-      for (uint32_t k = 0; k < d.n_group_by; k++) {
-        FinishKey& fk = fa.keys[k];
-        const uint8_t kind = plan.cols[plan.keys[k].col].kind;
-        fk.kind = (!qk[k].is_bin && is_date(uint32_t(d.group_by[k]))) ? uint8_t(DK_I32) : kind;   // Date32: 4-byte values
-        fk.stride = plan.keys[k].stride;
-        fk.wstride = plan.keys[k].wstride;
-        fk.card = qk[k].card;
-        fk.valid_off = take(uint64_t(nbatches) * wpb * 4);
-        if (kind == DK_BOOL) fk.val_off = take(uint64_t(nbatches) * wpb * 4);
-        else if (kind == DK_STR) fk.val_off = take((uint64_t(n_out) + 1) * 4);
-        else fk.val_off = take(uint64_t(n_out) * (fk.kind == DK_I32 ? 4 : 8));
-        if (qk[k].is_bin) {
-          fk.is_bin = 1;
-          fk.bin_base = plan.keys[k].bin_base;
-          fk.bin_width = plan.keys[k].bin_width;
-        } else if (kind != DK_BOOL) {
-          const ColSide& cs = table->sides[shape_cols[plan.keys[k].col]];
-          if (multi) {   // the dictionary every rank agreed on
-            fk.kd_offs = cs.d_glob_kd_offs;
-            fk.kd_bytes = cs.d_glob_kd_bytes;
-          } else {
-            fk.kd_offs = cs.d_kd_offs;
-            fk.kd_bytes = cs.d_kd_bytes;
-          }
-        }
-      }
-      for (uint32_t a = 0; a < d.n_aggs; a++) {
-        fa.aggs[a] = plan.aggs[a];
-        fa.nn_is_rows[a] = nn_is_rows[a];
-        fa.valid_off[a] = take(uint64_t(nbatches) * wpb * 4);
-        fa.out_kind[a] = rank_min_max(plan.aggs[a]) ? DK_STR : bool_min_max(plan.aggs[a]) ? DK_BOOL
-                       : agg_out_type[a] == PQ_T_DATE32 ? DK_I32 : DK_I64;   // the layouts of the keys
-        if (fa.out_kind[a] == DK_BOOL) fa.val_off[a] = take(uint64_t(nbatches) * wpb * 4);
-        else if (fa.out_kind[a] == DK_STR) fa.val_off[a] = take((uint64_t(n_out) + 1) * 4);
-        else fa.val_off[a] = take(uint64_t(n_out) * (fa.out_kind[a] == DK_I32 ? 4 : 8));
-      }
-      // MIN / MAX over Utf8: the winning values' bytes, bounded by rows x the longest value of the numbering (any group may
-      // hold the longest one)
-      for (uint32_t a = 0; a < d.n_aggs; a++) {
-        if (fa.out_kind[a] != DK_STR) continue;
-        FinishAggStr& s = fa.astr[a];
-        const ColSide& cs = table->sides[shape_cols[plan.aggs[a].col]];
-        s.kd_offs = multi ? cs.d_glob_kd_offs : cs.d_kd_offs;
-        s.kd_bytes = multi ? cs.d_glob_kd_bytes : cs.d_kd_bytes;
-        s.inv = rank_luts[a] ? rank_luts[a]->inv : nullptr;   // nullptr: a column in no file, every group NULL
-        const uint64_t bound = rank_luts[a] ? uint64_t(n_out) * (multi ? cs.glob_max_len : cs.kd_max_len) : 0;
-        if (bound > 0x7fffffffull)
-          throw Error(PQ_ERR_UNSUPPORTED, std::string(plan.aggs[a].fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
-                                              "): the strings of one result may exceed 2 GiB");
-        s.data_off = take(bound);
-      }
-      uint64_t win_off[2] = {0, 0};
-      for (size_t w = 0; w < win_names.size(); w++) win_off[w] = take(uint64_t(n_out) * 8);
-      // string key bytes: an upper bound keeps the copy to one round trip.  Rows x the longest distinct value; or, as one
-      // value of key k sits in at most prod_{j != k}(card_j + 1) groups, that many copies of all its distinct values.
-      // Both hold for any subset of the groups (a result cut by ORDER BY ... LIMIT).  Where that bound is large, the
-      // exact bytes of the output rows are counted on the device first (one more round trip)
-      for (uint32_t k = 0; k < d.n_group_by; k++) {
-        FinishKey& fk = fa.keys[k];
-        if (fk.kind != DK_STR) continue;
-        uint64_t max_len = 0;
-        const KeyDict* kd = qk[k].kd;
-        max_len = multi ? table->sides[shape_cols[plan.keys[k].col]].glob_max_len : table->sides[shape_cols[plan.keys[k].col]].kd_max_len;
-        uint64_t copies = 1;
-        for (uint32_t j = 0; j < d.n_group_by; j++)
-          if (j != k) copies = std::min<uint64_t>(uint64_t(n_out), copies * (uint64_t(qk[j].card) + 1));
-        uint64_t bound = std::min<uint64_t>(uint64_t(n_out) * max_len, copies * kd->bytes.size());
-        if (bound > kExactKeyBytes && !wrun) {
-          fa.wide = plan.hashed ? d_hkeys.p : tuple ? tuple->d_wide : nullptr;
-          fa.out_slot = d_out_slot.p;
-          fa.n_out = n_out;
-          fa.n_dev = n_dev;
-          DevBuf<unsigned long long> total;
-          total.alloc(1, stream);
-          total.zero();
-          k_key_bytes_total<<<std::min<uint32_t>(1024, (n_out + 255) / 256), 256, 0, stream>>>(fa, k, total.p);
-          launches++;
-          PQB_CUDA(cudaGetLastError());
-          unsigned long long exact = 0;
-          PQB_CUDA(cudaMemcpyAsync(&exact, total.p, 8, cudaMemcpyDeviceToHost, stream));
-          PQB_CUDA(cudaStreamSynchronize(stream));
-          bound = exact;
-        }
-        if (bound > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "group key strings of one result exceed 2 GiB");
-        fk.data_off = take(bound);
-      }
-      const uint64_t copy_bytes = off;
-      for (uint32_t k = 0; k < d.n_group_by; k++)
-        if (fa.keys[k].kind == DK_STR) fa.keys[k].len_off = take(uint64_t(n_out) * 4);   // device-only scratch behind the copied part
-      for (uint32_t a = 0; a < d.n_aggs; a++)
-        if (fa.out_kind[a] == DK_STR) fa.astr[a].len_off = take(uint64_t(n_out) * 4);
-      r.d_block = std::make_unique<DevBuf<uint8_t>>();
-      DevBuf<uint8_t>& d_block = *r.d_block;
-      d_block.alloc(off, stream);
-      PQB_CUDA(cudaMemsetAsync(d_block.p, 0, copy_bytes, stream));
-      if (wrun) {   // the kept groups' slots in output order, their row_number / partition_rows into the block
-        DevBuf<uint32_t> slots;
-        slots.alloc(n_out, stream);
-        auto col = [&](uint32_t flag) -> long long* {
-          if (!(win->flags & flag)) return nullptr;
-          const size_t w = (flag == PQ_WINDOW_PARTITION_ROWS && (win->flags & PQ_WINDOW_ROW_NUMBER)) ? 1 : 0;
-          return reinterpret_cast<long long*>(d_block.p + win_off[w]);
-        };
-        wrun->fill(d_out_slot.p, n_out, slots.p, col(PQ_WINDOW_ROW_NUMBER), col(PQ_WINDOW_PARTITION_ROWS), stream);
-        launches++;
-        std::swap(d_out_slot.p, slots.p);   // the old list is freed with `slots`
-        std::swap(d_out_slot.n, slots.n);
-      }
-      fa.acc = d_acc.p;
-      fa.wide = plan.hashed ? d_hkeys.p : tuple ? tuple->d_wide : nullptr;
-      fa.out_slot = d_out_slot.p;
-      fa.out = d_block.p;
-      fa.nulls = reinterpret_cast<uint32_t*>(d_block.p + nulls_off);
-      fa.n_out = n_out;
-      fa.n_dev = n_dev;
-      fa.nslots = plan.nslots;
-      fa.n_acc = plan.n_acc;
-      fa.naggs = d.n_aggs;
-      fa.nkeys = d.n_group_by;
-      fa.batch_rows = batch_rows;
-      fa.words_per_batch = wpb;
-      fa.nbatches = nbatches;
-      k_agg_finish<<<(n_out + 255) / 256, 256, 0, stream>>>(fa);
-      launches++;
-      for (uint32_t k = 0; k < d.n_group_by; k++) {
-        if (fa.keys[k].kind != DK_STR) continue;
-        k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.keys[k].len_off), n_out, n_dev,
-                                               reinterpret_cast<int32_t*>(d_block.p + fa.keys[k].val_off));
-        k_key_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, k);
-        launches += 2;
-      }
-      for (uint32_t a = 0; a < d.n_aggs; a++) {
-        if (fa.out_kind[a] != DK_STR) continue;
-        k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.astr[a].len_off), n_out, n_dev,
-                                               reinterpret_cast<int32_t*>(d_block.p + fa.val_off[a]));
-        k_agg_str_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, a);
-        launches += 2;
-      }
-      PQB_CUDA(cudaGetLastError());
-      r.block = std::make_shared<PinnedBlock>();
-      r.block->p = ctx.pinned_acquire(copy_bytes);
-      r.block->bytes = copy_bytes;
-      PQB_CUDA(cudaMemcpyAsync(r.block->p, d_block.p, copy_bytes, cudaMemcpyDeviceToHost, stream));
-      PQB_CUDA(cudaEventRecord(t_all.b, stream));
-      metrics.d2h_bytes += copy_bytes;
-      r.nbatches = nbatches;
-      r.wpb = wpb;
-      r.ncolumns = ncolumns;
-      r.nulls_off = nulls_off;
-      r.copy_bytes = copy_bytes;
-      r.win_off[0] = win_off[0];
-      r.win_off[1] = win_off[1];
-      return r;
-    };
-    // ---- one round trip: an unordered GROUP BY whose plan this shape has answered before lays its result block out for
-    // that many groups now, and the block comes back with the group count.  Should the count have grown (other ranks'
-    // tables under PQ_QUERY_ALLREDUCE), the block is laid out again after the round trip.  ORDER BY / windows (the count
-    // sizes their sort), MEDIAN / PERCENTILE_CONT (their pick runs on the groups) and global aggregates keep two ----
-    Assembled pre;
-    const bool tail_hint = d.n_group_by && !ordered && !plan.npct;
-    uint64_t tail_key = 0;
-    if (tail_hint) {
-      tail_key = plan_hash(plan, lit_pool, batch_rows) ^ (tuple ? 0x9e3779b97f4a7c15ull : 0ull);   // a tuple plan is not its per-key plan
-      uint32_t cap = 0;
-      {
-        std::lock_guard<std::mutex> lk(shape->hint_mu);
-        auto it = shape->groups_hint.find(tail_key);
-        if (it != shape->groups_hint.end()) cap = it->second;
-      }
-      if (const char* e = getenv("PQB_TAIL_CAP")) cap = uint32_t(atoi(e));   // test switch: the block's room in groups
-      cap = uint32_t(std::min<uint64_t>(cap, out_cap));
-      if (verbose) fprintf(stderr, "[pqb] result tail: %s\n", cap ? ("one round trip, block for " + std::to_string(cap) + " groups").c_str()
-                                                                     : "no earlier answer of this plan: two round trips");
-      if (cap) pre = assemble(cap, d_totals.p);
-    }
-    unsigned long long totals[2] = {0, 0};
-    std::vector<unsigned int> pct_count(plan.npct, 0u);
-    {   // into page-locked memory: a copy to pageable memory holds the host until it is done, and the next copy waits for
-        // that.  pinned_acquire hands out any free block of the context's pool that is large enough (1 MB at least)
-      PinnedBlock small;
-      small.p = ctx.pinned_acquire(16 + sizeof(h_counters) + plan.npct * 4);
-      PQB_CUDA(cudaMemcpyAsync(small.p, d_totals.p, 16, cudaMemcpyDeviceToHost, stream));
-      PQB_CUDA(cudaMemcpyAsync(small.p + 16, d_counters.p, sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
-      if (plan.npct) PQB_CUDA(cudaMemcpyAsync(small.p + 16 + sizeof(h_counters), d_pct_count.p, plan.npct * 4, cudaMemcpyDeviceToHost, stream));
-      PQB_CUDA(cudaStreamSynchronize(stream));
-      std::memcpy(totals, small.p, 16);
-      std::memcpy(h_counters, small.p + 16, sizeof(h_counters));
-      if (plan.npct) std::memcpy(pct_count.data(), small.p + 16 + sizeof(h_counters), plan.npct * 4);
-    }
-    metrics.d2h_bytes += 16 + sizeof(h_counters) + plan.npct * 4;
-    if (merge) {   // G is the same on every rank, and no collective follows: every rank throws alike
-      merge->report(verbose, uint32_t(totals[0]), metrics);
-      if (totals[0] > (1ull << 26)) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: more distinct groups than the hashed accumulator table holds (2^26)");
-    }
-    if (plan.hashed && h_counters[1] == 100) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: more distinct groups than the hashed accumulator table holds (2^26)");
-    if (plan.ndist && h_counters[1] == kDistinctFull) throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT): more distinct (group, value) pairs than the pair set holds (2^27)");
-    if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
-    uint32_t n_out = uint32_t(totals[0]);
-    metrics.rows_selected = totals[1];
-    if (tail_hint && n_out) {
-      std::lock_guard<std::mutex> lk(shape->hint_mu);
-      if (shape->groups_hint.size() >= 64 && !shape->groups_hint.count(tail_key)) shape->groups_hint.clear();   // a bound, not an LRU
-      shape->groups_hint[tail_key] = n_out;
-    }
-    if (allreduce && !merge) { float ms = 0; cudaEventElapsedTime(&ms, t_ar.a, t_ar.b); metrics.allreduce_ms = ms; }
-    static const char* fn_names[] = {"count(*)", "count", "sum", "min", "max", "avg", "count(distinct", "median", "percentile_cont"};
-    auto agg_name = [&](uint32_t a) {
-      const DevAgg& ag = plan.aggs[a];
-      if (ag.fn == AG_PERCENTILE_CONT) {   // p in shortest round-trip form: percentile_cont(latency_ms, 0.99)
-        char buf[32];
-        const auto r = std::to_chars(buf, buf + sizeof(buf), pct_p[a]);
-        return std::string("percentile_cont(") + d.columns[d.aggs[a].col].name + ", " + std::string(buf, r.ptr) + ")";
-      }
-      return ag.fn == AG_COUNT_STAR ? std::string("count(*)")
-                                    : std::string(fn_names[ag.fn]) + (ag.fn == AG_COUNT_DISTINCT ? " " : "(") + d.columns[d.aggs[a].col].name + ")";
-    };
-    // ---- MEDIAN / PERCENTILE_CONT: sort each column's pairs, pick every group's results into the aggregates' cells ----
-    if (plan.npct && n_out) {
-      double pct_ms = 0.0;
-      for (uint32_t i = 0; i < plan.npct; i++) {
-        PctPickArgs pk{};
-        for (uint32_t a = 0; a < d.n_aggs; a++) {
-          const DevAgg& ag = plan.aggs[a];
-          if ((ag.fn != AG_MEDIAN && ag.fn != AG_PERCENTILE_CONT) || ag.dset != i) continue;
-          pk.a[pk.naggs].p = pct_p[a];
-          pk.a[pk.naggs].median = ag.fn == AG_MEDIAN ? 1 : 0;
-          pk.a[pk.naggs].acc_slot = ag.acc_slot;
-          pk.naggs++;
-        }
-        const uint32_t n = pct_count[i];
-        if (verbose) fprintf(stderr, "[pqb] percentile column %u: %u pairs, %u aggregates\n", i, n, pk.naggs);
-        if (n == 0) continue;   // every input NULL: the non-NULL counts make every result NULL
-        launches += pct_finish(d_pct_slots[i], d_pct_keys[i], n, pk, d_out_slot.p, n_out, d_acc.p, plan.nslots,
-                               plan.pct[i].enc == OE_F64, stream, metrics, pct_ms);
-      }
-      metrics.percentile_ms = pct_ms;
-    }
-    // ---- ORDER BY [LIMIT]: permute and cut out_slot; after the all-reduce, so every rank orders identical tables ----
-    const uint64_t n_total = (d.n_group_by == 0 && n_out == 0) ? 1 : n_out;   // a global aggregate over zero rows is one row
-    uint64_t keep = n_total;
-    metrics.groups_total = n_total;
-    std::unique_ptr<Timer> t_enc, t_sort;   // only for a query with ORDER BY
-    bool sort_timed = false;
-    std::unique_ptr<OrderBufs> wbufs;
-    if (ordered) {
-      if (d.limit >= 0) keep = std::min<uint64_t>(keep, uint64_t(d.limit));
-      if (win ? n_out > 0 : keep && n_out > 1) {
-        OrderArgs oa{};
-        uint8_t nulls_first[kMaxOrder];
-        oa.acc = d_acc.p;
-        oa.wide = plan.hashed ? d_hkeys.p : tuple ? tuple->d_wide : nullptr;
-        oa.out_slot = d_out_slot.p;
-        oa.n = n_out;
-        oa.nslots = plan.nslots;
-        oa.n_acc = plan.n_acc;
-        oa.nterms = n_part + d.n_order_by;   // a window sorts by its partition terms first
-        std::vector<std::shared_ptr<const uint32_t>> rank_hold;   // a concurrent unify_key may replace the column's ranks
-        for (uint32_t t = 0; t < oa.nterms; t++) {
-          const PqOrderBy& ob = t < n_part ? win->partition_by[t] : d.order_by[t - n_part];
-          OrderTerm& ot = oa.t[t];
-          ot.target = uint8_t(ob.target);
-          ot.desc = (ob.flags & PQ_ORDER_DESC) ? 1 : 0;
-          nulls_first[t] = (ob.flags & PQ_ORDER_NULLS_FIRST) ? 1 : 0;
-          if (ob.target == PQ_ORDER_AGG) {
-            const DevAgg& ag = plan.aggs[ob.index];
-            ot.agg = ag;
-            ot.nn_is_rows = nn_is_rows[ob.index];
-            ot.enc = (ag.fn == AG_AVG || ag.fn == AG_PERCENTILE_CONT ||
-                      ((ag.fn == AG_SUM || ag.fn == AG_MIN || ag.fn == AG_MAX || ag.fn == AG_MEDIAN) && ag.kind == DK_F64)) ? OE_F64 : OE_I64;
-            continue;
-          }
-          const DevKey& key = plan.keys[ob.index];
-          const uint8_t kind = plan.cols[key.col].kind;
-          ot.card = qk[ob.index].card;
-          ot.wstride = key.wstride;
-          if (qk[ob.index].is_bin || kind == DK_BOOL) { ot.enc = OE_RAW; ot.source = OS_GID; continue; }   // bins ascend with their start
-          const ColSide& cs = table->sides[shape_cols[key.col]];
-          ot.kd_offs = multi ? cs.d_glob_kd_offs : cs.d_kd_offs;
-          ot.kd_bytes = multi ? cs.d_glob_kd_bytes : cs.d_kd_bytes;
-          if (kind == DK_STR) {
-            ot.enc = OE_RAW;
-            ot.source = OS_RANK;
-            rank_hold.push_back(table->ensure_kd_rank(shape_cols[key.col], multi, stream));
-            ot.rank = rank_hold.back().get();
-          } else {
-            ot.enc = kind == DK_F64 ? OE_F64 : OE_I64;
-            ot.source = OS_VALUE;
-          }
-        }
-        t_enc = std::make_unique<Timer>();
-        t_sort = std::make_unique<Timer>();
-        if (win) {
-          // the window: encode, then sort and count (WindowRun); the kept groups' slots are written once the result
-          // block is allocated
-          wbufs = std::make_unique<OrderBufs>(oa.nterms, oa.n, stream, metrics);
-          oa.vals = wbufs->vals.p;
-          oa.nulls = wbufs->nulls.p;
-          oa.ranges = wbufs->ranges.p;
-          PQB_CUDA(cudaEventRecord(t_enc->a, stream));
-          k_order_encode<<<(oa.n + 255) / 256, 256, 0, stream>>>(oa);
-          PQB_CUDA(cudaEventRecord(t_enc->b, stream));
-          wrun = std::make_unique<WindowRun>(*win, n_out, n_part);
-          const unsigned long long kept = wrun->count(*wbufs, nulls_first, d_out_slot.p, stream, metrics);
-          launches += 1 + wrun->launches;
-          keep = d.limit >= 0 ? std::min<uint64_t>(kept, uint64_t(d.limit)) : kept;
-        } else {
-          launches += order_groups(oa, nulls_first, uint32_t(keep), d_out_slot, stream, metrics, *t_enc, *t_sort, &sort_timed);
-        }
-        n_out = uint32_t(keep);
-      } else if (win) {   // a global aggregate over zero rows: its one row has rn = 1
-        if (!(win->offset == 0 && win->fetch != 0)) keep = 0;
-      }
-    }
-    if (keep == 0) {   // ORDER BY ... LIMIT 0
-      metrics.groups = 0;
-      PQB_CUDA(cudaEventRecord(t_all.b, stream));
-      PQB_CUDA(cudaStreamSynchronize(stream));
-    } else if (d.n_group_by == 0 && n_out == 0) {
-      // SQL: a global aggregate over zero rows still yields one row: COUNT = 0, everything else NULL
-      OutBatch ob;
-      ob.rows = 1;
-      for (uint32_t a = 0; a < d.n_aggs; a++) {
-        OutColumn oc;
-        oc.name = agg_name(a);
-        oc.type = agg_out_type[a];
-        oc.values.assign(8, 0);
-        const bool is_count = plan.aggs[a].fn == AG_COUNT_STAR || plan.aggs[a].fn == AG_COUNT || plan.aggs[a].fn == AG_COUNT_DISTINCT;
-        if (!is_count) { oc.validity.assign(1, 0); oc.null_count = 1; }
-        if (oc.type == PQ_T_UTF8) oc.offsets.assign(2, 0);   // MIN / MAX over Utf8: one NULL row, no bytes
-        ob.cols.push_back(std::move(oc));
-      }
-      for (const std::string& name : win_names) {   // the one row of the one partition: rn = 1, partition_rows = 1
-        OutColumn oc;
-        oc.name = name;
-        oc.type = PQ_T_I64;
-        oc.values.assign(8, 0);
-        oc.values[0] = 1;
-        ob.cols.push_back(std::move(oc));
-      }
-      metrics.groups = 1;
-      batches_.push_back(std::move(ob));
-      PQB_CUDA(cudaEventRecord(t_all.b, stream));
-      PQB_CUDA(cudaStreamSynchronize(stream));
-    } else if (n_out == 0) {
-      metrics.groups = 0;
-      PQB_CUDA(cudaEventRecord(t_all.b, stream));
-      PQB_CUDA(cudaStreamSynchronize(stream));
-    } else {
-      if (pre.rows < n_out) {   // no block yet, or one too small for the groups: lay it out for n_out
-        if (pre.rows && verbose) fprintf(stderr, "[pqb] result tail: %u groups, the block had room for %u: second copy\n", n_out, pre.rows);
-        pre = assemble(n_out, nullptr);
-        PQB_CUDA(cudaStreamSynchronize(stream));
-      }
-      Assembled& r = pre;
-      if (r.copy_bytes <= kKeepDeviceResult) { r.block->dev = r.d_block->p; r.d_block->p = nullptr; dev_blocks_.push_back(r.block); }   // JSON egress formats it where it is
-      metrics.groups = n_out;
-      const FinishArgs& fa = r.fa;
-      const std::shared_ptr<PinnedBlock>& block = r.block;
-      const uint32_t wpb = r.wpb, ncolumns = r.ncolumns;
-      const uint64_t* win_off = r.win_off;
-      const uint32_t nbatches = (n_out + batch_rows - 1) / batch_rows;   // r.nbatches: the batches the block has room for
-      const uint32_t* nulls = reinterpret_cast<const uint32_t*>(block->p + r.nulls_off);
-      for (uint32_t b = 0; b < nbatches; b++) {
-        const uint32_t r0 = b * batch_rows, nb = std::min(batch_rows, n_out - r0);
-        OutBatch ob;
-        ob.rows = nb;
-        for (uint32_t c = 0; c < ncolumns; c++) {
-          OutColumn oc;
-          oc.ext = block;
-          oc.ext_all = true;
-          oc.null_count = nulls[c * r.nbatches + b];
-          if (c < d.n_group_by) {
-            const FinishKey& fk = fa.keys[c];
-            const uint32_t qc = uint32_t(d.group_by[c]);
-            oc.name = fk.is_bin ? std::string("date_bin(") + d.columns[qc].name + ")" : std::string(d.columns[qc].name);
-            oc.type = fk.is_bin ? PQ_T_TS_MS : out_type_of(qc);
-            oc.ext_validity_off = fk.valid_off + uint64_t(b) * wpb * 4;
-            if (fk.kind == DK_STR) { oc.ext_offsets_off = fk.val_off + uint64_t(r0) * 4; oc.ext_off = fk.data_off; }
-            else if (fk.kind == DK_BOOL) oc.ext_off = fk.val_off + uint64_t(b) * wpb * 4;
-            else oc.ext_off = fk.val_off + uint64_t(r0) * (fk.kind == DK_I32 ? 4 : 8);
-          } else if (c >= d.n_group_by + d.n_aggs) {   // row_number / partition_rows
-            const uint32_t w = c - d.n_group_by - d.n_aggs;
-            oc.name = win_names[w];
-            oc.type = PQ_T_I64;
-            oc.ext_off = win_off[w] + uint64_t(r0) * 8;
-          } else {
-            const uint32_t a = c - d.n_group_by;
-            oc.name = agg_name(a);
-            oc.type = agg_out_type[a];
-            oc.ext_validity_off = fa.valid_off[a] + uint64_t(b) * wpb * 4;
-            if (fa.out_kind[a] == DK_STR) { oc.ext_offsets_off = fa.val_off[a] + uint64_t(r0) * 4; oc.ext_off = fa.astr[a].data_off; }
-            else if (fa.out_kind[a] == DK_BOOL) oc.ext_off = fa.val_off[a] + uint64_t(b) * wpb * 4;
-            else oc.ext_off = fa.val_off[a] + uint64_t(r0) * (fa.out_kind[a] == DK_I32 ? 4 : 8);
-          }
-          ob.cols.push_back(std::move(oc));
-        }
-        batches_.push_back(std::move(ob));
-      }
-    }
-    if (t_enc) {   // the ORDER BY kernels: encode, then pack + sort (the range round trip between them is not counted)
-      float ms = 0, ms2 = 0;
-      cudaEventElapsedTime(&ms, t_enc->a, t_enc->b);
-      if (sort_timed) cudaEventElapsedTime(&ms2, t_sort->a, t_sort->b);
-      metrics.order_ms = double(ms) + double(ms2) + (wrun ? wrun->ms() : 0.0);
-    }
-  } else {
-    // ---- filter / COUNT(*) ----
-    // bitmap-driven stream compaction on the device: per-item prefix, then one CTA per item.  The
-    // selected-row total is needed on the host to size the result; a repeat of the same query shape
-    // sizes it from the previous answer and skips that round trip.
-    DevBuf<unsigned long long> d_item_base, d_total, d_ids;
-    std::shared_ptr<PinnedBlock> ids_block;   // selected row ordinals land in page-locked memory, batches alias it
-    unsigned long long n_ids = 0, total = 0;
-    d_total.alloc(2, stream);   // the selected rows; under PQ_QUERY_ALLREDUCE also the ranks that met a corrupt page
-    d_item_base.alloc(std::max<size_t>(items.size(), 1), stream);
-    if (!items.empty()) {
-      k_item_prefix<<<1, 1024, 0, stream>>>(d_item_counts.p, uint32_t(items.size()), d_item_base.p, d_total.p);
-      launches++;
-    } else {
-      PQB_CUDA(cudaMemsetAsync(d_total.p, 0, 8, stream));
-    }
-    PQB_CUDA(cudaMemcpyAsync(h_counters, d_counters.p, sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
-    PQB_CUDA(cudaMemcpyAsync(&total, d_total.p, 8, cudaMemcpyDeviceToHost, stream));
-    metrics.d2h_bytes += 8 + sizeof(h_counters);
-    const unsigned long long lim = d.limit >= 0 ? (unsigned long long)d.limit : ~0ull;
-    if (projecting || row_order) {
-      // ---- TableProvider::scan(projection): gather the projected columns of the selected rows ----
-      struct PC { uint32_t qcol; uint32_t slot; uint8_t kind; std::string name; int type; };
-      std::vector<PC> pcs;
-      for (uint32_t i = 0; i < d.n_projection; i++) {
-        const uint32_t qc = uint32_t(d.projection[i]);
-        // a Date32 column is projected as 4-byte values (DK_I32: the output layout only, read like Int64)
-        pcs.push_back({qc, uint32_t(slot_of[qc]), is_date(qc) ? uint8_t(DK_I32) : plan.cols[slot_of[qc]].kind, d.columns[qc].name, out_type_of(qc)});
-        if (pcs.back().kind == DK_STR) table->ensure_ent_off(shape_cols[slot_of[qc]], stream);
-      }
-      // an ordered scan without a projection returns its selected row ordinals in order
-      if ((d.flags & PQ_QUERY_EMIT_ROW_IDS) || !projecting) pcs.push_back({0, 0xffffffffu, DK_I64, "__row_id", PQ_T_I64});
-      const uint32_t npc = uint32_t(pcs.size());
-      // the longest string of every projected Utf8 column sizes its bytes (the ranks' merged rows: over every rank)
-      std::vector<uint64_t> str_len(npc, 0);
-      for (uint32_t c = 0; c < npc; c++)
-        if (pcs[c].kind == DK_STR) {
-          const ColSide& cs = table->sides[shape_cols[pcs[c].slot]];
-          str_len[c] = std::max(cs.max_ent_len, cs.max_plain_len);
-        }
-      std::unique_ptr<ScanMerge> smerge;   // PQ_QUERY_ALLGATHER with other ranks
-      std::shared_ptr<PinnedBlock> block;
-      ProjArgs pj{};
-      uint64_t nulls_off = 0, copy_bytes = 0;
-      uint32_t nbatches = 0;
-      const uint32_t wpb = (batch_rows + 31) / 32;
-      unsigned long long n_rows = 0;
-      DevBuf<uint8_t> d_block;
-      // a window's extra columns (Int64, never NULL, after the projection and __row_id): `win_fill` writes them, and the
-      // kept positions, once gather has allocated the block
-      std::vector<std::string> win_names;
-      if (win && (win->flags & PQ_WINDOW_ROW_NUMBER)) win_names.push_back("row_number");
-      if (win && (win->flags & PQ_WINDOW_PARTITION_ROWS)) win_names.push_back("partition_rows");
-      uint64_t win_off[2] = {0, 0};
-      std::function<void(long long*, long long*)> win_fill;
-      // the first `cap` selected rows, or with `handles` the rows at positions kept[0, cap) (ORDER BY ... LIMIT), or with
-      // `owned` the output rows this rank holds of the ranks' merged rows: every byte of the block is then written by one
-      // rank and zero on the others, and the ranks' blocks are summed (their u64 words: disjoint bytes never carry).
-      // String offsets, which every rank computes alike, are computed after the lengths are summed and never summed.
-      auto gather = [&](unsigned long long cap, const unsigned long long* handles, const uint32_t* kept, const unsigned long long* owned) {
-        nbatches = uint32_t((cap + batch_rows - 1) / batch_rows);
-        uint64_t off = 0;
-        auto take = [&](uint64_t bytes) { uint64_t o = off; off = (off + bytes + 63) & ~63ull; return o; };
-        nulls_off = take(uint64_t(npc) * nbatches * 4);
-        for (uint32_t c = 0; c < npc; c++) {
-          ProjCol& pc = pj.cols[c];
-          pc = ProjCol{};
-          pc.slot = pcs[c].slot;
-          pc.kind = pcs[c].kind;
-          pc.valid_off = take(uint64_t(nbatches) * wpb * 4);
-          if (pc.kind == DK_BOOL) pc.val_off = take(uint64_t(nbatches) * wpb * 4);
-          else if (pc.kind == DK_STR) pc.val_off = take((cap + 1) * 4);
-          else pc.val_off = take(cap * (pc.kind == DK_I32 ? 4 : 8));
-        }
-        uint64_t data_lo = off;   // the string bytes of every column: [data_lo, data_hi)
-        for (uint32_t c = 0; c < npc; c++) {
-          ProjCol& pc = pj.cols[c];
-          if (pc.kind != DK_STR) continue;
-          pc.ent = table->sides[shape_cols[pc.slot]].d_ent_off;
-          const uint64_t bound = cap * str_len[c];
-          if (bound > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "projected strings of one result exceed 2 GiB: add a LIMIT");
-          pc.data_off = take(bound);
-        }
-        const uint64_t data_hi = off;
-        for (size_t w = 0; w < win_names.size(); w++) win_off[w] = take(cap * 8);
-        copy_bytes = off;
-        for (uint32_t c = 0; c < npc; c++)
-          if (pj.cols[c].kind == DK_STR) { pj.cols[c].src_off = take(cap * 8); pj.cols[c].len_off = take(cap * 4); }
-        d_block.alloc(off, stream);
-        PQB_CUDA(cudaMemsetAsync(d_block.p, 0, off, stream));
-        pj.arena = table->d_arena;
-        pj.flat = table->d_flat;
-        pj.fpages = table->d_flat_pages;
-        pj.chunks = shape->d_chunks;
-        pj.items = shape->d_items;
-        pj.bitmap = d_bitmap.p;
-        pj.item_counts = d_item_counts.p;
-        pj.item_base = d_item_base.p;
-        pj.out = d_block.p;
-        pj.nulls = reinterpret_cast<uint32_t*>(d_block.p + nulls_off);
-        pj.n_out = cap;
-        pj.n_items = uint32_t(items.size());
-        pj.plan_ncols = ncols;
-        pj.ncols = npc;
-        pj.batch_rows = batch_rows;
-        pj.words_per_batch = wpb;
-        pj.nbatches = nbatches;
-        if (win_fill) {
-          long long* cols[2] = {nullptr, nullptr};
-          for (size_t w = 0; w < win_names.size(); w++) cols[win_names[w] == "row_number" ? 0 : 1] = reinterpret_cast<long long*>(d_block.p + win_off[w]);
-          win_fill(cols[0], cols[1]);
-          launches++;
-        }
-        if (owned) {
-          PQB_CUDA(cudaEventRecord(smerge->t_out.a, stream));
-          k_project_owned<<<uint32_t((cap + 255) / 256), 256, 0, stream>>>(pj, owned);
-          // everything but the string bytes (summed once they are written); the string offsets are still zero
-          comm_allreduce_u64(d_block.p, data_lo / 8, 0 /*sum*/, stream);
-          if (off > data_hi) comm_allreduce_u64(d_block.p + data_hi, (off - data_hi) / 8, 0 /*sum*/, stream);   // the lengths
-        } else if (handles) {
-          k_project_rows<<<uint32_t((cap + 255) / 256), 256, 0, stream>>>(pj, handles, kept);
-        } else {
-          const uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
-          k_project<<<grid, 256, 0, stream>>>(pj);
-        }
-        launches++;
-        for (uint32_t c = 0; c < npc; c++) {
-          if (pj.cols[c].kind != DK_STR) continue;
-          // rows beyond the selected total have length 0: the scan over `cap` rows is exact
-          k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + pj.cols[c].len_off), uint32_t(cap), nullptr,
-                                                 reinterpret_cast<int32_t*>(d_block.p + pj.cols[c].val_off));
-          k_project_bytes<<<uint32_t((cap * 32 + 255) / 256), 256, 0, stream>>>(pj, c, cap, owned);
-          launches += 2;
-        }
-        if (owned) {
-          if (data_hi > data_lo) comm_allreduce_u64(d_block.p + data_lo, (data_hi - data_lo) / 8, 0 /*sum*/, stream);
-          PQB_CUDA(cudaEventRecord(smerge->t_out.b, stream));
-          smerge->out_timed = true;
-        }
-        PQB_CUDA(cudaGetLastError());
-        block = std::make_shared<PinnedBlock>();
-        block->p = ctx.pinned_acquire(copy_bytes);
-        block->bytes = copy_bytes;
-        PQB_CUDA(cudaMemcpyAsync(block->p, d_block.p, copy_bytes, cudaMemcpyDeviceToHost, stream));
-      };
-      if (row_order && (!items.empty() || merge_rows)) {
-        // ---- ORDER BY ... LIMIT: every selected row's terms and handle (k_order_rows_encode), the positions of the first
-        // `keep` rows in order (order_sort), then their projection.  Under PQ_QUERY_ALLGATHER with other ranks, those
-        // first rows of every rank are merged (ScanMerge) and each rank projects the merged rows it holds; without the
-        // flag every shard orders and cuts its own selection.
-        PQB_CUDA(cudaStreamSynchronize(stream));   // the selected-row total sizes the sort
-        unsigned long long keep = std::min(total, lim);   // a window: the kept rows, known after its sort
-        if (merge_rows) {   // the checks below, agreed by every rank
-          uint64_t row_end = 0, row_bytes = 0;
-          for (const DevItem& it : items) row_end = std::max<uint64_t>(row_end, it.global_row0 + it.nrows);
-          for (const PC& pc : pcs) row_bytes += 1 + (pc.kind == DK_STR ? 16 : pc.kind == DK_BOOL ? 1 : 8);   // validity, values / offsets and scratch
-          smerge = std::make_unique<ScanMerge>();
-          smerge->exchange(roa.nterms, keep, total, h_counters[1], row_end, str_len, lim, row_bytes, stream, metrics);
-          str_len = smerge->str_len;
-        } else {
-          if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
-          if (total > 0xffffffffull) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY over more than 2^32 - 1 selected rows");
-          if (!win && keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
-        }
-        const uint32_t n = uint32_t(total);
-        std::unique_ptr<OrderBufs> obuf;   // (the merge reads this rank's encoded rows)
-        DevBuf<unsigned long long> handles;
-        DevBuf<uint32_t> kept;
-        if (win ? total > 0 : keep > 0) {
-          obuf = std::make_unique<OrderBufs>(roa.nterms, n, stream, metrics);
-          OrderBufs& ob = *obuf;
-          handles.alloc(n, stream);
-          roa.arena = table->d_arena;
-          roa.flat = table->d_flat;
-          roa.fpages = d_opages.p ? d_opages.p : table->d_flat_pages;
-          roa.chunks = shape->d_chunks;
-          roa.items = shape->d_items;
-          roa.bitmap = d_bitmap.p;
-          roa.item_counts = d_item_counts.p;
-          roa.item_base = d_item_base.p;
-          roa.n_items = uint32_t(items.size());
-          roa.plan_ncols = ncols;
-          roa.n = n;
-          roa.vals = ob.vals.p;
-          roa.nulls = ob.nulls.p;
-          roa.ranges = ob.ranges.p;
-          roa.handles = handles.p;
-          uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
-          if (const char* g = getenv("PQB_GRID")) grid = std::max(1, atoi(g));   // debugging aid: several items per CTA
-          Timer t_enc, t_sort;
-          bool sort_timed = false;
-          PQB_CUDA(cudaEventRecord(t_enc.a, stream));
-          k_order_rows_encode<<<grid, 256, 0, stream>>>(roa);
-          PQB_CUDA(cudaEventRecord(t_enc.b, stream));
-          std::unique_ptr<WindowRun> wrun;
-          if (win) {
-            // the window: sort and count, then the kept positions and the extra columns in gather's block
-            wrun = std::make_unique<WindowRun>(*win, n, n_part);
-            keep = std::min(wrun->count(ob, row_nulls_first, nullptr, stream, metrics), lim);
-            launches += 1 + wrun->launches;
-            if (keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
-            if (keep) {
-              kept.alloc(keep, stream);
-              win_fill = [&](long long* rn, long long* prows) { wrun->fill(nullptr, keep, kept.p, rn, prows, stream); };
-              gather(keep, handles.p, kept.p, nullptr);
-            }
-          } else {
-            launches += 1 + order_sort(ob, roa.nterms, n, row_nulls_first, uint32_t(keep), nullptr, kept, stream, metrics, t_sort, &sort_timed);
-            if (!smerge) gather(keep, handles.p, kept.p, nullptr);
-          }
-          PQB_CUDA(cudaStreamSynchronize(stream));
-          if (keep && !smerge) metrics.d2h_bytes += copy_bytes;
-          float ms = 0, ms2 = 0;
-          cudaEventElapsedTime(&ms, t_enc.a, t_enc.b);
-          if (sort_timed) cudaEventElapsedTime(&ms2, t_sort.a, t_sort.b);
-          metrics.order_ms = double(ms) + double(ms2) + (wrun ? wrun->ms() : 0.0);
-        }
-        shape->last_total.store(total);
-        if (smerge) {
-          // every rank's first rows: the same candidates and the same order on every rank, each output row projected by
-          // the rank that holds it and the ranks' blocks summed
-          DevBuf<unsigned long long> owned;
-          launches += smerge->merge(obuf ? obuf->vals.p : nullptr, obuf ? obuf->nulls.p : nullptr, n, kept.p, handles.p, shape->d_items,
-                                    row_nulls_first, owned, stream, metrics);
-          keep = smerge->keep;
-          if (keep) {
-            gather(keep, nullptr, nullptr, owned.p);
-            metrics.d2h_bytes += copy_bytes;
-          }
-          PQB_CUDA(cudaStreamSynchronize(stream));
-          smerge->report(verbose, metrics);
-          total = smerge->total;
-        }
-        n_rows = keep;
-      } else if (!items.empty()) {
-        const unsigned long long hint = shape->last_total.load();
-        bool done = false;
-        if (hint != ~0ull) {
-          const unsigned long long cap = std::max<unsigned long long>(1, std::min(lim, hint + hint / 8 + 1024));
-          if (cap > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
-          gather(cap, nullptr, nullptr, nullptr);
-          PQB_CUDA(cudaStreamSynchronize(stream));
-          if (std::min(total, lim) <= cap) { done = true; n_rows = std::min(total, lim); metrics.d2h_bytes += copy_bytes; }
-          else block.reset();
-        } else {
-          PQB_CUDA(cudaStreamSynchronize(stream));
-        }
-        if (!done) {
-          const unsigned long long keep = std::min(total, lim);
-          if (keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
-          if (keep) {
-            gather(keep, nullptr, nullptr, nullptr);
-            PQB_CUDA(cudaStreamSynchronize(stream));
-            metrics.d2h_bytes += copy_bytes;
-          }
-          n_rows = keep;
-        }
-        shape->last_total.store(total);
-      }
-      PQB_CUDA(cudaEventRecord(t_all.b, stream));
-      PQB_CUDA(cudaStreamSynchronize(stream));
-      if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
-      if (block && d_block.p && copy_bytes <= kKeepDeviceResult) { block->dev = d_block.p; d_block.p = nullptr; dev_blocks_.push_back(block); }
-      metrics.rows_selected = total;
-      const uint32_t out_batches = n_rows ? uint32_t((n_rows + batch_rows - 1) / batch_rows) : 1u;
-      for (uint32_t b = 0; b < out_batches; b++) {
-        const unsigned long long r0 = uint64_t(b) * batch_rows;
-        const uint32_t nb = n_rows ? uint32_t(std::min<unsigned long long>(batch_rows, n_rows - r0)) : 0u;
-        OutBatch ob;
-        ob.rows = nb;
-        for (uint32_t c = 0; c < npc; c++) {
-          OutColumn oc;
-          oc.name = pcs[c].name;
-          oc.type = pcs[c].type;
-          if (nb) {
-            const ProjCol& pc = pj.cols[c];
-            oc.ext = block;
-            oc.ext_all = true;
-            oc.null_count = reinterpret_cast<const uint32_t*>(block->p + nulls_off)[c * nbatches + b];
-            oc.ext_validity_off = pc.valid_off + uint64_t(b) * wpb * 4;
-            if (pc.kind == DK_STR) { oc.ext_offsets_off = pc.val_off + r0 * 4; oc.ext_off = pc.data_off; }
-            else if (pc.kind == DK_BOOL) oc.ext_off = pc.val_off + uint64_t(b) * wpb * 4;
-            else oc.ext_off = pc.val_off + r0 * (pc.kind == DK_I32 ? 4 : 8);
-          } else if (oc.type == PQ_T_UTF8) oc.offsets.assign(1, 0);
-          ob.cols.push_back(std::move(oc));
-        }
-        for (size_t w = 0; w < win_names.size(); w++) {
-          OutColumn oc;
-          oc.name = win_names[w];
-          oc.type = PQ_T_I64;
-          if (nb) {
-            oc.ext = block;
-            oc.ext_all = true;
-            oc.ext_off = win_off[w] + r0 * 8;
-          }
-          ob.cols.push_back(std::move(oc));
-        }
-        batches_.push_back(std::move(ob));
-      }
-      float ms = 0;
-      cudaEventElapsedTime(&ms, t_all.a, t_all.b);
-      metrics.device_ms = ms;
-      if (!items.empty() && nrg) { cudaEventElapsedTime(&ms, t_scan.a, t_scan.b); metrics.scan_kernel_ms = ms; }
-      metrics.kernel_launches = launches;
-      return;
-    }
-    if (want_rows && !items.empty()) {
-      unsigned long long hint = shape->last_total.load();
-      bool done = false;
-      if (hint != ~0ull) {
-        // optimistic pass: room for the previous answer plus a margin
-        unsigned long long cap = std::min(lim, hint + hint / 8 + 1024);
-        if (cap) {
-          d_ids.alloc(cap, stream);
-          uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
-          k_compact_row_ids<<<grid, 256, 0, stream>>>(d_bitmap.p, shape->d_items, d_item_counts.p, d_item_base.p, uint32_t(items.size()), d_ids.p, cap);
-          launches++;
-          ids_block = std::make_shared<PinnedBlock>();
-          ids_block->p = ctx.pinned_acquire(cap * 8);
-          ids_block->bytes = cap * 8;
-          PQB_CUDA(cudaMemcpyAsync(ids_block->p, d_ids.p, cap * 8, cudaMemcpyDeviceToHost, stream));
-        }
-        PQB_CUDA(cudaStreamSynchronize(stream));
-        const unsigned long long keep = std::min(total, lim);
-        if (keep <= cap) { done = true; n_ids = keep; metrics.d2h_bytes += cap * 8; }
-        else ids_block.reset();
-      } else {
-        PQB_CUDA(cudaStreamSynchronize(stream));
-      }
-      mark("scan done, selected-row total on host");
-      if (!done) {
-        const unsigned long long keep = std::min(total, lim);
-        if (keep) {
-          DevBuf<unsigned long long> d_ids2;
-          d_ids2.alloc(keep, stream);
-          uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
-          k_compact_row_ids<<<grid, 256, 0, stream>>>(d_bitmap.p, shape->d_items, d_item_counts.p, d_item_base.p, uint32_t(items.size()), d_ids2.p, keep);
-          launches++;
-          ids_block = std::make_shared<PinnedBlock>();
-          ids_block->p = ctx.pinned_acquire(keep * 8);
-          ids_block->bytes = keep * 8;
-          n_ids = keep;
-          PQB_CUDA(cudaMemcpyAsync(ids_block->p, d_ids2.p, keep * 8, cudaMemcpyDeviceToHost, stream));
-          PQB_CUDA(cudaStreamSynchronize(stream));
-          metrics.d2h_bytes += keep * 8;
-        }
-      }
-      shape->last_total.store(total);
-    }
-    PQB_CUDA(cudaEventRecord(t_all.b, stream));
+    batches.push_back(std::move(ob));
+  }
+}
+
+// One row built on the host (a global aggregate over zero rows, COUNT(*) alone) in a heap block: every aggregate holds
+// `value`, or NULL where `null` says so, and a window's columns hold 1 (the one row of its one partition)
+void ResultTail::one_row(std::vector<BlockCol> cols, const std::vector<bool>& null, unsigned long long value) {
+  const size_t naggs = cols.size();
+  for (const std::string& w : win_names) cols.push_back({w});
+  BlockLayout L(1, batch_rows, uint32_t(cols.size()));
+  for (BlockCol& c : cols) L.column(c);
+  const std::shared_ptr<PinnedBlock> block = heap_block(L.off);
+  for (size_t c = 0; c < cols.size(); c++) {
+    const unsigned long long v = c < naggs ? value : 1;
+    if (c < naggs && null[c]) reinterpret_cast<uint32_t*>(block->p + L.nulls_off)[c] = 1;   // one batch: column c's count
+    else std::memcpy(block->p + cols[c].val_off, &v, 8);
+  }
+  slice(L, cols, block, 1);
+}
+
+// A filter scan's result sized from the rows the last scan of this shape selected.  fill(cap) queues a result for `cap`
+// rows into `block` and returns the bytes it copies back.  A repeat of the query lays the result out for the previous
+// answer plus a margin (at least min_cap rows) before the selected-row total is on the host, and keeps it when the rows
+// fit; otherwise, and on a first run, it is laid out for the rows once the total is known.  `then` marks the verbose
+// timeline once the total is on the host.  Returns the rows kept, min(total, LIMIT).
+template <class Fill>
+unsigned long long ResultTail::sized_pass(unsigned long long min_cap, std::shared_ptr<PinnedBlock>& block, Fill fill, const char* then) {
+  const unsigned long long hint = shape.last_total.load();
+  bool done = false;
+  if (hint != ~0ull) {
+    const unsigned long long cap = std::max(min_cap, std::min(lim, hint + hint / 8 + 1024));
+    const uint64_t bytes = fill(cap);
     PQB_CUDA(cudaStreamSynchronize(stream));
-    mark("results on host");
-    metrics.rows_selected = total;
-    unsigned long long corrupt_ranks = 0;
-    if (has_aggs && allreduce) {
-      // SELECT COUNT(*) under PQ_QUERY_ALLREDUCE: the total's all-reduce also counts the ranks that met a corrupt page,
-      // so that every rank throws, not only the ones that met it
-      const unsigned long long bad = h_counters[1] ? 1ull : 0ull;
-      PQB_CUDA(cudaMemcpyAsync(d_total.p + 1, &bad, 8, cudaMemcpyHostToDevice, stream));
-      comm_allreduce_u64(d_total.p, 2, 0, stream);
-      unsigned long long w[2];
-      PQB_CUDA(cudaMemcpyAsync(w, d_total.p, 16, cudaMemcpyDeviceToHost, stream));
-      PQB_CUDA(cudaStreamSynchronize(stream));
-      total = w[0];
-      corrupt_ranks = w[1];
+    if (std::min(total, lim) <= cap) { done = true; metrics.d2h_bytes += bytes; }
+    else block.reset();
+  } else {
+    PQB_CUDA(cudaStreamSynchronize(stream));
+  }
+  if (then) mark(then);
+  const unsigned long long keep = std::min(total, lim);
+  if (!done && keep) {
+    const uint64_t bytes = fill(keep);
+    PQB_CUDA(cudaStreamSynchronize(stream));
+    metrics.d2h_bytes += bytes;
+  }
+  shape.last_total.store(total);
+  return keep;
+}
+
+// bitmap-driven stream compaction on the device: per-item prefix, then one CTA per item.  The selected-row total is
+// needed on the host to size the result; a repeat of the same query shape sizes it from the previous answer and skips
+// that round trip (sized_pass).
+void ResultTail::count_selected() {
+  d_total.alloc(2, stream);   // the selected rows; under PQ_QUERY_ALLREDUCE also the ranks that met a corrupt page
+  d_item_base.alloc(std::max<size_t>(items.size(), 1), stream);
+  if (!items.empty()) {
+    k_item_prefix<<<1, 1024, 0, stream>>>(d_item_counts.p, uint32_t(items.size()), d_item_base.p, d_total.p);
+    launches++;
+  } else {
+    PQB_CUDA(cudaMemsetAsync(d_total.p, 0, 8, stream));
+  }
+  PQB_CUDA(cudaMemcpyAsync(h_counters, d_counters.p, sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
+  PQB_CUDA(cudaMemcpyAsync(&total, d_total.p, 8, cudaMemcpyDeviceToHost, stream));
+  metrics.d2h_bytes += 8 + sizeof(h_counters);
+}
+
+// an aggregate table: the all-reduce or hashed merge of the ranks' tables, MEDIAN / PERCENTILE_CONT, ORDER BY or a
+// window, the result block assembled on the device
+void ResultTail::groups() {
+  // multi-GPU: the partial tables meet in ONE grouped all-reduce (SURVEY §8e): one NCCL launch,
+  // per array the reduction its aggregate needs
+  Timer t_ar;
+  std::unique_ptr<MergeRun> merge;   // a hashed GROUP BY: every rank's listed groups gathered and merged instead
+  if (allreduce && plan.hashed) {
+    merge = std::make_unique<MergeRun>();
+    launches += merge->run(plan, cells, key_space, std::min<uint64_t>(plan.nslots, std::max<uint64_t>(metrics.rows_scanned, 1)),
+                           d_acc, d_hkeys, d_counters.p, stream, metrics);
+  } else if (allreduce) {
+    PQB_CUDA(cudaEventRecord(t_ar.a, stream));
+    comm_group_begin();
+    comm_allreduce_u64(d_acc.p, plan.nslots, 0, stream);
+    for (uint32_t a = 0; a < plan.n_acc; a++) {
+      uint8_t how = plan.acc_init[a];
+      comm_allreduce_u64(d_acc.p + size_t(1 + a) * plan.nslots, plan.nslots, how == 0 ? 0 : how == 1 ? 3 : how == 2 ? 1 : 2, stream);
     }
-    if (h_counters[1]) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device (code " + std::to_string(h_counters[1]) + ")");
-    if (corrupt_ranks) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device of " + std::to_string(corrupt_ranks) + " other rank(s)");
-    if (has_aggs) {  // SELECT COUNT(*) [, COUNT(*)...] WHERE ...
-      metrics.groups_total = 1;
-      // one row, ordered trivially; LIMIT 0 keeps none, and a window keeps it when its rank range holds rn = 1
-      const bool win_drops = win && !(win->offset == 0 && win->fetch != 0);
-      if ((ordered && d.limit == 0) || win_drops) {
-        metrics.groups = 0;
+    if (plan.n_nn) comm_allreduce_u64(d_acc.p + size_t(1 + plan.n_acc) * plan.nslots, size_t(plan.n_nn) * plan.nslots, 0, stream);
+    comm_group_end();
+    PQB_CUDA(cudaEventRecord(t_ar.b, stream));
+  }
+  // ---- non-empty groups in ascending slot order (deterministic: the mixed radix of the group ids) ----
+  const uint32_t ntiles = (plan.nslots + kSlotTile - 1) / kSlotTile;
+  const uint64_t out_cap = std::min<uint64_t>(plan.nslots, std::max<uint64_t>(allreduce ? plan.nslots : metrics.rows_scanned, 1));
+  DevBuf<uint32_t> d_tile_counts, d_out_slot;
+  DevBuf<unsigned long long> d_tile_base, d_totals;
+  d_tile_counts.alloc(ntiles, stream);
+  d_tile_base.alloc(ntiles, stream);
+  d_totals.alloc(2, stream);
+  d_out_slot.alloc(out_cap, stream);
+  const uint32_t* order = tuple ? tuple->d_order : nullptr;   // tuple slots: listed in the order of their mixed-radix ids
+  k_slot_tile_counts<<<ntiles, 256, 0, stream>>>(d_acc.p, plan.nslots, d_tile_counts.p, order);
+  k_item_prefix<<<1, 1024, 0, stream>>>(d_tile_counts.p, ntiles, d_tile_base.p, d_totals.p);
+  k_slot_compact<<<ntiles, 256, 0, stream>>>(d_acc.p, plan.nslots, d_tile_base.p, d_out_slot.p, order);
+  // rows this rank selected (its own items)
+  d_item_base.alloc(std::max<size_t>(items.size(), 1), stream);
+  if (!items.empty()) k_item_prefix<<<1, 1024, 0, stream>>>(d_item_counts.p, uint32_t(items.size()), d_item_base.p, d_totals.p + 1);
+  else PQB_CUDA(cudaMemsetAsync(d_totals.p + 1, 0, 8, stream));
+  launches += 4;
+  std::unique_ptr<WindowRun> wrun;       // only for a query with a window over at least one group
+  // ---- the result block: every buffer of every batch for n_out groups, assembled on the device and copied to page-locked
+  // memory (no synchronise).  n_dev != nullptr: n_out is a capacity, the kernels read the group count on the device.
+  // cut: ORDER BY ... LIMIT keeps a subset of the groups ----
+  struct Assembled {
+    BlockLayout L;       // L.rows: the groups the block has room for (0: none assembled)
+    std::vector<BlockCol> cols;
+    FinishArgs fa{};
+    std::unique_ptr<DevBuf<uint8_t>> d_block;
+    std::shared_ptr<PinnedBlock> block;
+  };
+  auto assemble = [&](uint32_t n_out, const unsigned long long* n_dev) -> Assembled {
+    Assembled r;
+    r.L = BlockLayout(n_out, batch_rows, d.n_group_by + d.n_aggs + uint32_t(win_names.size()));
+    BlockLayout& L = r.L;
+    FinishArgs& fa = r.fa;
+    for (uint32_t k = 0; k < d.n_group_by; k++) {
+      FinishKey& fk = fa.keys[k];
+      const uint32_t qc = uint32_t(d.group_by[k]);
+      const uint8_t kind = plan.cols[plan.keys[k].col].kind;
+      fk.kind = (!qk[k].is_bin && out_type[qc] == PQ_T_DATE32) ? uint8_t(DK_I32) : kind;   // Date32: 4-byte values
+      fk.stride = plan.keys[k].stride;
+      fk.wstride = plan.keys[k].wstride;
+      fk.card = qk[k].card;
+      r.cols.push_back({qk[k].is_bin ? std::string("date_bin(") + d.columns[qc].name + ")" : std::string(d.columns[qc].name),
+                        qk[k].is_bin ? PQ_T_TS_MS : out_type[qc], uint8_t(fk.kind)});
+      L.column(r.cols.back());
+      fk.valid_off = r.cols.back().valid_off;
+      fk.val_off = r.cols.back().val_off;
+      if (qk[k].is_bin) {
+        fk.is_bin = 1;
+        fk.bin_base = plan.keys[k].bin_base;
+        fk.bin_width = plan.keys[k].bin_width;
+      } else if (kind != DK_BOOL) {
+        const ColSide& cs = table->sides[shape_cols[plan.keys[k].col]];
+        if (multi) {   // the dictionary every rank agreed on
+          fk.kd_offs = cs.d_glob_kd_offs;
+          fk.kd_bytes = cs.d_glob_kd_bytes;
+        } else {
+          fk.kd_offs = cs.d_kd_offs;
+          fk.kd_bytes = cs.d_kd_bytes;
+        }
+      }
+    }
+    for (uint32_t a = 0; a < d.n_aggs; a++) {
+      fa.aggs[a] = plan.aggs[a];
+      fa.nn_is_rows[a] = nn_is_rows[a];
+      fa.out_kind[a] = agg_kind(a);
+      r.cols.push_back({agg_name(a), agg_out_type[a], fa.out_kind[a]});
+      L.column(r.cols.back());
+      fa.valid_off[a] = r.cols.back().valid_off;
+      fa.val_off[a] = r.cols.back().val_off;
+    }
+    // MIN / MAX over Utf8: the winning values' bytes, bounded by rows x the longest value of the numbering (any group may
+    // hold the longest one)
+    for (uint32_t a = 0; a < d.n_aggs; a++) {
+      if (fa.out_kind[a] != DK_STR) continue;
+      FinishAggStr& s = fa.astr[a];
+      const ColSide& cs = table->sides[shape_cols[plan.aggs[a].col]];
+      s.kd_offs = multi ? cs.d_glob_kd_offs : cs.d_kd_offs;
+      s.kd_bytes = multi ? cs.d_glob_kd_bytes : cs.d_kd_bytes;
+      s.inv = rank_luts[a] ? rank_luts[a]->inv : nullptr;   // nullptr: a column in no file, every group NULL
+      const uint64_t bound = rank_luts[a] ? uint64_t(n_out) * (multi ? cs.glob_max_len : cs.kd_max_len) : 0;
+      if (bound > 0x7fffffffull)
+        throw Error(PQ_ERR_UNSUPPORTED, std::string(plan.aggs[a].fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
+                                            "): the strings of one result may exceed 2 GiB");
+      s.data_off = r.cols[d.n_group_by + a].data_off = L.take(bound);
+    }
+    for (const std::string& w : win_names) {
+      r.cols.push_back({w});
+      r.cols.back().val_off = L.per_row(8);
+    }
+    // string key bytes: an upper bound keeps the copy to one round trip.  Rows x the longest distinct value; or, as one
+    // value of key k sits in at most prod_{j != k}(card_j + 1) groups, that many copies of all its distinct values.
+    // Both hold for any subset of the groups (a result cut by ORDER BY ... LIMIT).  Where that bound is large, the
+    // exact bytes of the output rows are counted on the device first (one more round trip)
+    for (uint32_t k = 0; k < d.n_group_by; k++) {
+      FinishKey& fk = fa.keys[k];
+      if (fk.kind != DK_STR) continue;
+      uint64_t max_len = 0;
+      const KeyDict* kd = qk[k].kd;
+      max_len = multi ? table->sides[shape_cols[plan.keys[k].col]].glob_max_len : table->sides[shape_cols[plan.keys[k].col]].kd_max_len;
+      uint64_t copies = 1;
+      for (uint32_t j = 0; j < d.n_group_by; j++)
+        if (j != k) copies = std::min<uint64_t>(uint64_t(n_out), copies * (uint64_t(qk[j].card) + 1));
+      uint64_t bound = std::min<uint64_t>(uint64_t(n_out) * max_len, copies * kd->bytes.size());
+      if (bound > kExactKeyBytes && !wrun) {
+        fa.wide = plan.hashed ? d_hkeys.p : tuple ? tuple->d_wide : nullptr;
+        fa.out_slot = d_out_slot.p;
+        fa.n_out = n_out;
+        fa.n_dev = n_dev;
+        DevBuf<unsigned long long> total;
+        total.alloc(1, stream);
+        total.zero();
+        k_key_bytes_total<<<std::min<uint32_t>(1024, (n_out + 255) / 256), 256, 0, stream>>>(fa, k, total.p);
+        launches++;
+        PQB_CUDA(cudaGetLastError());
+        unsigned long long exact = 0;
+        PQB_CUDA(cudaMemcpyAsync(&exact, total.p, 8, cudaMemcpyDeviceToHost, stream));
+        PQB_CUDA(cudaStreamSynchronize(stream));
+        bound = exact;
+      }
+      if (bound > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "group key strings of one result exceed 2 GiB");
+      fk.data_off = r.cols[k].data_off = L.take(bound);
+    }
+    L.copy_bytes = L.off;
+    for (uint32_t k = 0; k < d.n_group_by; k++)
+      if (fa.keys[k].kind == DK_STR) fa.keys[k].len_off = L.per_row(4);   // device-only scratch behind the copied part
+    for (uint32_t a = 0; a < d.n_aggs; a++)
+      if (fa.out_kind[a] == DK_STR) fa.astr[a].len_off = L.per_row(4);
+    r.d_block = std::make_unique<DevBuf<uint8_t>>();
+    DevBuf<uint8_t>& d_block = *r.d_block;
+    d_block.alloc(L.off, stream);
+    PQB_CUDA(cudaMemsetAsync(d_block.p, 0, L.copy_bytes, stream));
+    if (wrun) {   // the kept groups' slots in output order, their row_number / partition_rows into the block
+      DevBuf<uint32_t> slots;
+      slots.alloc(n_out, stream);
+      auto col = [&](uint32_t flag) -> long long* {
+        if (!(win->flags & flag)) return nullptr;
+        const size_t w = (flag == PQ_WINDOW_PARTITION_ROWS && (win->flags & PQ_WINDOW_ROW_NUMBER)) ? 1 : 0;
+        return reinterpret_cast<long long*>(d_block.p + r.cols[d.n_group_by + d.n_aggs + w].val_off);
+      };
+      wrun->fill(d_out_slot.p, n_out, slots.p, col(PQ_WINDOW_ROW_NUMBER), col(PQ_WINDOW_PARTITION_ROWS), stream);
+      launches++;
+      std::swap(d_out_slot.p, slots.p);   // the old list is freed with `slots`
+      std::swap(d_out_slot.n, slots.n);
+    }
+    fa.acc = d_acc.p;
+    fa.wide = plan.hashed ? d_hkeys.p : tuple ? tuple->d_wide : nullptr;
+    fa.out_slot = d_out_slot.p;
+    fa.out = d_block.p;
+    fa.nulls = reinterpret_cast<uint32_t*>(d_block.p + L.nulls_off);
+    fa.n_out = n_out;
+    fa.n_dev = n_dev;
+    fa.nslots = plan.nslots;
+    fa.n_acc = plan.n_acc;
+    fa.naggs = d.n_aggs;
+    fa.nkeys = d.n_group_by;
+    fa.batch_rows = batch_rows;
+    fa.words_per_batch = L.wpb;
+    fa.nbatches = L.nbatches;
+    k_agg_finish<<<(n_out + 255) / 256, 256, 0, stream>>>(fa);
+    launches++;
+    for (uint32_t k = 0; k < d.n_group_by; k++) {
+      if (fa.keys[k].kind != DK_STR) continue;
+      k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.keys[k].len_off), n_out, n_dev,
+                                             reinterpret_cast<int32_t*>(d_block.p + fa.keys[k].val_off));
+      k_key_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, k);
+      launches += 2;
+    }
+    for (uint32_t a = 0; a < d.n_aggs; a++) {
+      if (fa.out_kind[a] != DK_STR) continue;
+      k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + fa.astr[a].len_off), n_out, n_dev,
+                                             reinterpret_cast<int32_t*>(d_block.p + fa.val_off[a]));
+      k_agg_str_gather<<<uint32_t((uint64_t(n_out) * 32 + 255) / 256), 256, 0, stream>>>(fa, a);
+      launches += 2;
+    }
+    PQB_CUDA(cudaGetLastError());
+    r.block = std::make_shared<PinnedBlock>();
+    r.block->p = ctx.pinned_acquire(L.copy_bytes);
+    r.block->bytes = L.copy_bytes;
+    PQB_CUDA(cudaMemcpyAsync(r.block->p, d_block.p, L.copy_bytes, cudaMemcpyDeviceToHost, stream));
+    PQB_CUDA(cudaEventRecord(t_all.b, stream));
+    metrics.d2h_bytes += L.copy_bytes;
+    return r;
+  };
+  // ---- one round trip: an unordered GROUP BY whose plan this shape has answered before lays its result block out for
+  // that many groups now, and the block comes back with the group count.  Should the count have grown (other ranks'
+  // tables under PQ_QUERY_ALLREDUCE), the block is laid out again after the round trip.  ORDER BY / windows (the count
+  // sizes their sort), MEDIAN / PERCENTILE_CONT (their pick runs on the groups) and global aggregates keep two ----
+  Assembled pre;
+  const bool tail_hint = d.n_group_by && !ordered && !plan.npct;
+  uint64_t tail_key = 0;
+  if (tail_hint) {
+    tail_key = plan_hash(plan, lit_pool, batch_rows) ^ (tuple ? 0x9e3779b97f4a7c15ull : 0ull);   // a tuple plan is not its per-key plan
+    uint32_t cap = 0;
+    {
+      std::lock_guard<std::mutex> lk(shape.hint_mu);
+      auto it = shape.groups_hint.find(tail_key);
+      if (it != shape.groups_hint.end()) cap = it->second;
+    }
+    if (const char* e = getenv("PQB_TAIL_CAP")) cap = uint32_t(atoi(e));   // test switch: the block's room in groups
+    cap = uint32_t(std::min<uint64_t>(cap, out_cap));
+    if (verbose) fprintf(stderr, "[pqb] result tail: %s\n", cap ? ("one round trip, block for " + std::to_string(cap) + " groups").c_str()
+                                                                   : "no earlier answer of this plan: two round trips");
+    if (cap) pre = assemble(cap, d_totals.p);
+  }
+  unsigned long long totals[2] = {0, 0};
+  std::vector<unsigned int> pct_count(plan.npct, 0u);
+  {   // into page-locked memory: a copy to pageable memory holds the host until it is done, and the next copy waits for
+      // that.  pinned_acquire hands out any free block of the context's pool that is large enough (1 MB at least)
+    PinnedBlock small;
+    small.p = ctx.pinned_acquire(16 + sizeof(h_counters) + plan.npct * 4);
+    PQB_CUDA(cudaMemcpyAsync(small.p, d_totals.p, 16, cudaMemcpyDeviceToHost, stream));
+    PQB_CUDA(cudaMemcpyAsync(small.p + 16, d_counters.p, sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
+    if (plan.npct) PQB_CUDA(cudaMemcpyAsync(small.p + 16 + sizeof(h_counters), d_pct_count.p, plan.npct * 4, cudaMemcpyDeviceToHost, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+    std::memcpy(totals, small.p, 16);
+    std::memcpy(h_counters, small.p + 16, sizeof(h_counters));
+    if (plan.npct) std::memcpy(pct_count.data(), small.p + 16 + sizeof(h_counters), plan.npct * 4);
+  }
+  metrics.d2h_bytes += 16 + sizeof(h_counters) + plan.npct * 4;
+  if (merge) {   // G is the same on every rank, and no collective follows: every rank throws alike
+    merge->report(verbose, uint32_t(totals[0]), metrics);
+    if (totals[0] > (1ull << 26)) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: more distinct groups than the hashed accumulator table holds (2^26)");
+  }
+  if (plan.hashed && h_counters[1] == 100) throw Error(PQ_ERR_UNSUPPORTED, "GROUP BY: more distinct groups than the hashed accumulator table holds (2^26)");
+  if (plan.ndist && h_counters[1] == kDistinctFull) throw Error(PQ_ERR_UNSUPPORTED, "COUNT(DISTINCT): more distinct (group, value) pairs than the pair set holds (2^27)");
+  check_corrupt();
+  uint32_t n_out = uint32_t(totals[0]);
+  metrics.rows_selected = totals[1];
+  if (tail_hint && n_out) {
+    std::lock_guard<std::mutex> lk(shape.hint_mu);
+    if (shape.groups_hint.size() >= 64 && !shape.groups_hint.count(tail_key)) shape.groups_hint.clear();   // a bound, not an LRU
+    shape.groups_hint[tail_key] = n_out;
+  }
+  if (allreduce && !merge) { float ms = 0; cudaEventElapsedTime(&ms, t_ar.a, t_ar.b); metrics.allreduce_ms = ms; }
+  // ---- MEDIAN / PERCENTILE_CONT: sort each column's pairs, pick every group's results into the aggregates' cells ----
+  if (plan.npct && n_out) {
+    double pct_ms = 0.0;
+    for (uint32_t i = 0; i < plan.npct; i++) {
+      PctPickArgs pk{};
+      for (uint32_t a = 0; a < d.n_aggs; a++) {
+        const DevAgg& ag = plan.aggs[a];
+        if ((ag.fn != AG_MEDIAN && ag.fn != AG_PERCENTILE_CONT) || ag.dset != i) continue;
+        pk.a[pk.naggs].p = pct_p[a];
+        pk.a[pk.naggs].median = ag.fn == AG_MEDIAN ? 1 : 0;
+        pk.a[pk.naggs].acc_slot = ag.acc_slot;
+        pk.naggs++;
+      }
+      const uint32_t n = pct_count[i];
+      if (verbose) fprintf(stderr, "[pqb] percentile column %u: %u pairs, %u aggregates\n", i, n, pk.naggs);
+      if (n == 0) continue;   // every input NULL: the non-NULL counts make every result NULL
+      launches += pct_finish(d_pct_slots[i], d_pct_keys[i], n, pk, d_out_slot.p, n_out, d_acc.p, plan.nslots,
+                             plan.pct[i].enc == OE_F64, stream, metrics, pct_ms);
+    }
+    metrics.percentile_ms = pct_ms;
+  }
+  // ---- ORDER BY [LIMIT]: permute and cut out_slot; after the all-reduce, so every rank orders identical tables ----
+  const uint64_t n_total = (d.n_group_by == 0 && n_out == 0) ? 1 : n_out;   // a global aggregate over zero rows is one row
+  uint64_t keep = n_total;
+  metrics.groups_total = n_total;
+  std::unique_ptr<Timer> t_enc, t_sort;   // only for a query with ORDER BY
+  bool sort_timed = false;
+  std::unique_ptr<OrderBufs> wbufs;
+  if (ordered) {
+    if (d.limit >= 0) keep = std::min<uint64_t>(keep, uint64_t(d.limit));
+    if (win ? n_out > 0 : keep && n_out > 1) {
+      OrderArgs oa{};
+      uint8_t nulls_first[kMaxOrder];
+      oa.acc = d_acc.p;
+      oa.wide = plan.hashed ? d_hkeys.p : tuple ? tuple->d_wide : nullptr;
+      oa.out_slot = d_out_slot.p;
+      oa.n = n_out;
+      oa.nslots = plan.nslots;
+      oa.n_acc = plan.n_acc;
+      oa.nterms = n_part + d.n_order_by;   // a window sorts by its partition terms first
+      std::vector<std::shared_ptr<const uint32_t>> rank_hold;   // a concurrent unify_key may replace the column's ranks
+      for (uint32_t t = 0; t < oa.nterms; t++) {
+        const PqOrderBy& ob = t < n_part ? win->partition_by[t] : d.order_by[t - n_part];
+        OrderTerm& ot = oa.t[t];
+        ot.target = uint8_t(ob.target);
+        ot.desc = (ob.flags & PQ_ORDER_DESC) ? 1 : 0;
+        nulls_first[t] = (ob.flags & PQ_ORDER_NULLS_FIRST) ? 1 : 0;
+        if (ob.target == PQ_ORDER_AGG) {
+          const DevAgg& ag = plan.aggs[ob.index];
+          ot.agg = ag;
+          ot.nn_is_rows = nn_is_rows[ob.index];
+          ot.enc = (ag.fn == AG_AVG || ag.fn == AG_PERCENTILE_CONT ||
+                    ((ag.fn == AG_SUM || ag.fn == AG_MIN || ag.fn == AG_MAX || ag.fn == AG_MEDIAN) && ag.kind == DK_F64)) ? OE_F64 : OE_I64;
+          continue;
+        }
+        const DevKey& key = plan.keys[ob.index];
+        const uint8_t kind = plan.cols[key.col].kind;
+        ot.card = qk[ob.index].card;
+        ot.wstride = key.wstride;
+        if (qk[ob.index].is_bin || kind == DK_BOOL) { ot.enc = OE_RAW; ot.source = OS_GID; continue; }   // bins ascend with their start
+        const ColSide& cs = table->sides[shape_cols[key.col]];
+        ot.kd_offs = multi ? cs.d_glob_kd_offs : cs.d_kd_offs;
+        ot.kd_bytes = multi ? cs.d_glob_kd_bytes : cs.d_kd_bytes;
+        if (kind == DK_STR) {
+          ot.enc = OE_RAW;
+          ot.source = OS_RANK;
+          rank_hold.push_back(table->ensure_kd_rank(shape_cols[key.col], multi, stream));
+          ot.rank = rank_hold.back().get();
+        } else {
+          ot.enc = kind == DK_F64 ? OE_F64 : OE_I64;
+          ot.source = OS_VALUE;
+        }
+      }
+      t_enc = std::make_unique<Timer>();
+      t_sort = std::make_unique<Timer>();
+      if (win) {
+        // the window: encode, then sort and count (WindowRun); the kept groups' slots are written once the result
+        // block is allocated
+        wbufs = std::make_unique<OrderBufs>(oa.nterms, oa.n, stream, metrics);
+        oa.vals = wbufs->vals.p;
+        oa.nulls = wbufs->nulls.p;
+        oa.ranges = wbufs->ranges.p;
+        PQB_CUDA(cudaEventRecord(t_enc->a, stream));
+        k_order_encode<<<(oa.n + 255) / 256, 256, 0, stream>>>(oa);
+        PQB_CUDA(cudaEventRecord(t_enc->b, stream));
+        wrun = std::make_unique<WindowRun>(*win, n_out, n_part);
+        const unsigned long long kept = wrun->count(*wbufs, nulls_first, d_out_slot.p, stream, metrics);
+        launches += 1 + wrun->launches;
+        keep = d.limit >= 0 ? std::min<uint64_t>(kept, uint64_t(d.limit)) : kept;
       } else {
-        OutBatch ob;
-        ob.rows = 1;
-        for (uint32_t a = 0; a < d.n_aggs; a++) {
-          OutColumn oc;
-          oc.name = "count(*)";
-          oc.type = PQ_T_I64;
-          oc.values.resize(8);
-          std::memcpy(oc.values.data(), &total, 8);
-          ob.cols.push_back(std::move(oc));
-        }
-        for (uint32_t f : {PQ_WINDOW_ROW_NUMBER, PQ_WINDOW_PARTITION_ROWS}) {   // the one partition of one row
-          if (!win || !(win->flags & f)) continue;
-          OutColumn oc;
-          oc.name = f == PQ_WINDOW_ROW_NUMBER ? "row_number" : "partition_rows";
-          oc.type = PQ_T_I64;
-          oc.values.assign(8, 0);
-          oc.values[0] = 1;
-          ob.cols.push_back(std::move(oc));
-        }
-        metrics.groups = 1;
-        batches_.push_back(std::move(ob));
+        launches += order_groups(oa, nulls_first, uint32_t(keep), d_out_slot, stream, metrics, *t_enc, *t_sort, &sort_timed);
       }
-    } else if (want_rows) {
-      // selected row ordinals, ascending
-      for (size_t r0 = 0; r0 < n_ids || (r0 == 0 && n_ids == 0); r0 += batch_rows) {
-        size_t nb = std::min<size_t>(batch_rows, n_ids - r0);
-        OutBatch ob;
-        ob.rows = int64_t(nb);
-        OutColumn oc;
-        oc.name = "__row_id";
-        oc.type = PQ_T_I64;
-        if (nb) { oc.ext = ids_block; oc.ext_off = r0 * 8; }
-        ob.cols.push_back(std::move(oc));
-        batches_.push_back(std::move(ob));
-        if (n_ids == 0) break;
-      }
+      n_out = uint32_t(keep);
+    } else if (win) {   // a global aggregate over zero rows: its one row has rn = 1
+      if (!(win->offset == 0 && win->fetch != 0)) keep = 0;
     }
   }
+  if (keep == 0) {   // ORDER BY ... LIMIT 0
+    metrics.groups = 0;
+    PQB_CUDA(cudaEventRecord(t_all.b, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+  } else if (d.n_group_by == 0 && n_out == 0) {
+    // SQL: a global aggregate over zero rows still yields one row: COUNT = 0, everything else NULL
+    std::vector<BlockCol> cols;
+    std::vector<bool> null;
+    for (uint32_t a = 0; a < d.n_aggs; a++) {
+      cols.push_back({agg_name(a), agg_out_type[a], agg_kind(a)});
+      null.push_back(plan.aggs[a].fn != AG_COUNT_STAR && plan.aggs[a].fn != AG_COUNT && plan.aggs[a].fn != AG_COUNT_DISTINCT);
+    }
+    one_row(cols, null, 0);
+    metrics.groups = 1;
+    PQB_CUDA(cudaEventRecord(t_all.b, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+  } else if (n_out == 0) {
+    metrics.groups = 0;
+    PQB_CUDA(cudaEventRecord(t_all.b, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+  } else {
+    if (pre.L.rows < n_out) {   // no block yet, or one too small for the groups: lay it out for n_out
+      if (pre.L.rows && verbose) fprintf(stderr, "[pqb] result tail: %u groups, the block had room for %u: second copy\n", n_out, uint32_t(pre.L.rows));
+      pre = assemble(n_out, nullptr);
+      PQB_CUDA(cudaStreamSynchronize(stream));
+    }
+    keep_device(pre.block, *pre.d_block, pre.L.copy_bytes);
+    metrics.groups = n_out;
+    slice(pre.L, pre.cols, pre.block, n_out);
+  }
+  if (t_enc) {   // the ORDER BY kernels: encode, then pack + sort (the range round trip between them is not counted)
+    float ms = 0, ms2 = 0;
+    cudaEventElapsedTime(&ms, t_enc->a, t_enc->b);
+    if (sort_timed) cudaEventElapsedTime(&ms2, t_sort->a, t_sort->b);
+    metrics.order_ms = double(ms) + double(ms2) + (wrun ? wrun->ms() : 0.0);
+  }
+}
+
+// TableProvider::scan(projection): the projected columns of the selected rows, or an ordered scan (merged across ranks
+// under PQ_QUERY_ALLGATHER)
+void ResultTail::rows() {
+  count_selected();
+  // ---- TableProvider::scan(projection): gather the projected columns of the selected rows ----
+  std::vector<BlockCol> pcs;   // the projected columns, then a window's
+  std::vector<uint32_t> slots;
+  for (uint32_t i = 0; i < d.n_projection; i++) {
+    const uint32_t qc = uint32_t(d.projection[i]);
+    // a Date32 column is projected as 4-byte values (DK_I32: the output layout only, read like Int64)
+    pcs.push_back({d.columns[qc].name, out_type[qc], out_type[qc] == PQ_T_DATE32 ? uint8_t(DK_I32) : plan.cols[slot_of[qc]].kind});
+    slots.push_back(uint32_t(slot_of[qc]));
+    if (pcs.back().kind == DK_STR) table->ensure_ent_off(shape_cols[slot_of[qc]], stream);
+  }
+  // an ordered scan without a projection returns its selected row ordinals in order
+  if ((d.flags & PQ_QUERY_EMIT_ROW_IDS) || !d.n_projection) {
+    pcs.push_back({"__row_id"});
+    slots.push_back(0xffffffffu);
+  }
+  const uint32_t npc = uint32_t(pcs.size());
+  for (const std::string& w : win_names) pcs.push_back({w});
+  // the longest string of every projected Utf8 column sizes its bytes (the ranks' merged rows: over every rank)
+  std::vector<uint64_t> str_len(npc, 0);
+  for (uint32_t c = 0; c < npc; c++)
+    if (pcs[c].kind == DK_STR) {
+      const ColSide& cs = table->sides[shape_cols[slots[c]]];
+      str_len[c] = std::max(cs.max_ent_len, cs.max_plain_len);
+    }
+  std::unique_ptr<ScanMerge> smerge;   // PQ_QUERY_ALLGATHER with other ranks
+  std::shared_ptr<PinnedBlock> block;
+  ProjArgs pj{};
+  BlockLayout L;
+  uint64_t data_lo = 0, data_hi = 0;   // the string bytes of every column: [data_lo, data_hi)
+  unsigned long long n_rows = 0;
+  DevBuf<uint8_t> d_block;
+  // a window's columns (after the projection and __row_id): `win_fill` writes them, and the kept positions, once gather
+  // has allocated the block
+  std::function<void(long long*, long long*)> win_fill;
+  auto lay_out = [&](unsigned long long cap) {
+    L = BlockLayout(cap, batch_rows, npc);
+    for (uint32_t c = 0; c < npc; c++) {
+      ProjCol& pc = pj.cols[c];
+      pc = ProjCol{};
+      pc.slot = slots[c];
+      pc.kind = pcs[c].kind;
+      L.column(pcs[c]);
+      pc.valid_off = pcs[c].valid_off;
+      pc.val_off = pcs[c].val_off;
+    }
+    data_lo = L.off;
+    for (uint32_t c = 0; c < npc; c++) {
+      ProjCol& pc = pj.cols[c];
+      if (pc.kind != DK_STR) continue;
+      pc.ent = table->sides[shape_cols[pc.slot]].d_ent_off;
+      const uint64_t bound = cap * str_len[c];
+      if (bound > 0x7fffffffull) throw Error(PQ_ERR_UNSUPPORTED, "projected strings of one result exceed 2 GiB: add a LIMIT");
+      pc.data_off = pcs[c].data_off = L.take(bound);
+    }
+    data_hi = L.off;
+    for (size_t w = 0; w < win_names.size(); w++) pcs[npc + w].val_off = L.per_row(8);
+    L.copy_bytes = L.off;
+    for (uint32_t c = 0; c < npc; c++)
+      if (pj.cols[c].kind == DK_STR) { pj.cols[c].src_off = L.per_row(8); pj.cols[c].len_off = L.per_row(4); }
+  };
+  // the first `cap` selected rows, or with `handles` the rows at positions kept[0, cap) (ORDER BY ... LIMIT), or with
+  // `owned` the output rows this rank holds of the ranks' merged rows: every byte of the block is then written by one
+  // rank and zero on the others, and the ranks' blocks are summed (their u64 words: disjoint bytes never carry).
+  // String offsets, which every rank computes alike, are computed after the lengths are summed and never summed.
+  auto gather = [&](unsigned long long cap, const unsigned long long* handles, const uint32_t* kept, const unsigned long long* owned) {
+    lay_out(cap);
+    d_block.alloc(L.off, stream);
+    PQB_CUDA(cudaMemsetAsync(d_block.p, 0, L.off, stream));
+    pj.arena = table->d_arena;
+    pj.flat = table->d_flat;
+    pj.fpages = table->d_flat_pages;
+    pj.chunks = shape.d_chunks;
+    pj.items = shape.d_items;
+    pj.bitmap = d_bitmap.p;
+    pj.item_counts = d_item_counts.p;
+    pj.item_base = d_item_base.p;
+    pj.out = d_block.p;
+    pj.nulls = reinterpret_cast<uint32_t*>(d_block.p + L.nulls_off);
+    pj.n_out = cap;
+    pj.n_items = uint32_t(items.size());
+    pj.plan_ncols = ncols;
+    pj.ncols = npc;
+    pj.batch_rows = batch_rows;
+    pj.words_per_batch = L.wpb;
+    pj.nbatches = L.nbatches;
+    if (win_fill) {
+      long long* cols[2] = {nullptr, nullptr};
+      for (size_t w = 0; w < win_names.size(); w++) cols[win_names[w] == "row_number" ? 0 : 1] = reinterpret_cast<long long*>(d_block.p + pcs[npc + w].val_off);
+      win_fill(cols[0], cols[1]);
+      launches++;
+    }
+    if (owned) {
+      PQB_CUDA(cudaEventRecord(smerge->t_out.a, stream));
+      k_project_owned<<<uint32_t((cap + 255) / 256), 256, 0, stream>>>(pj, owned);
+      // everything but the string bytes (summed once they are written); the string offsets are still zero
+      comm_allreduce_u64(d_block.p, data_lo / 8, 0 /*sum*/, stream);
+      if (L.off > data_hi) comm_allreduce_u64(d_block.p + data_hi, (L.off - data_hi) / 8, 0 /*sum*/, stream);   // the lengths
+    } else if (handles) {
+      k_project_rows<<<uint32_t((cap + 255) / 256), 256, 0, stream>>>(pj, handles, kept);
+    } else {
+      const uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
+      k_project<<<grid, 256, 0, stream>>>(pj);
+    }
+    launches++;
+    for (uint32_t c = 0; c < npc; c++) {
+      if (pj.cols[c].kind != DK_STR) continue;
+      // rows beyond the selected total have length 0: the scan over `cap` rows is exact
+      k_offsets_scan<<<1, 1024, 0, stream>>>(reinterpret_cast<const uint32_t*>(d_block.p + pj.cols[c].len_off), uint32_t(cap), nullptr,
+                                             reinterpret_cast<int32_t*>(d_block.p + pj.cols[c].val_off));
+      k_project_bytes<<<uint32_t((cap * 32 + 255) / 256), 256, 0, stream>>>(pj, c, cap, owned);
+      launches += 2;
+    }
+    if (owned) {
+      if (data_hi > data_lo) comm_allreduce_u64(d_block.p + data_lo, (data_hi - data_lo) / 8, 0 /*sum*/, stream);
+      PQB_CUDA(cudaEventRecord(smerge->t_out.b, stream));
+      smerge->out_timed = true;
+    }
+    PQB_CUDA(cudaGetLastError());
+    block = std::make_shared<PinnedBlock>();
+    block->p = ctx.pinned_acquire(L.copy_bytes);
+    block->bytes = L.copy_bytes;
+    PQB_CUDA(cudaMemcpyAsync(block->p, d_block.p, L.copy_bytes, cudaMemcpyDeviceToHost, stream));
+  };
+  if (row_order && (!items.empty() || merge_rows)) {
+    // ---- ORDER BY ... LIMIT: every selected row's terms and handle (k_order_rows_encode), the positions of the first
+    // `keep` rows in order (order_sort), then their projection.  Under PQ_QUERY_ALLGATHER with other ranks, those
+    // first rows of every rank are merged (ScanMerge) and each rank projects the merged rows it holds; without the
+    // flag every shard orders and cuts its own selection.
+    PQB_CUDA(cudaStreamSynchronize(stream));   // the selected-row total sizes the sort
+    unsigned long long keep = std::min(total, lim);   // a window: the kept rows, known after its sort
+    if (merge_rows) {   // the checks below, agreed by every rank
+      uint64_t row_end = 0, row_bytes = 0;
+      for (const DevItem& it : items) row_end = std::max<uint64_t>(row_end, it.global_row0 + it.nrows);
+      for (uint32_t c = 0; c < npc; c++) row_bytes += 1 + (pcs[c].kind == DK_STR ? 16 : pcs[c].kind == DK_BOOL ? 1 : 8);   // validity, values / offsets and scratch
+      smerge = std::make_unique<ScanMerge>();
+      smerge->exchange(roa.nterms, keep, total, h_counters[1], row_end, str_len, lim, row_bytes, stream, metrics);
+      str_len = smerge->str_len;
+    } else {
+      check_corrupt();
+      if (total > 0xffffffffull) throw Error(PQ_ERR_UNSUPPORTED, "row-level ORDER BY over more than 2^32 - 1 selected rows");
+      if (!win && keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
+    }
+    const uint32_t n = uint32_t(total);
+    std::unique_ptr<OrderBufs> obuf;   // (the merge reads this rank's encoded rows)
+    DevBuf<unsigned long long> handles;
+    DevBuf<uint32_t> kept;
+    if (win ? total > 0 : keep > 0) {
+      obuf = std::make_unique<OrderBufs>(roa.nterms, n, stream, metrics);
+      OrderBufs& ob = *obuf;
+      handles.alloc(n, stream);
+      roa.arena = table->d_arena;
+      roa.flat = table->d_flat;
+      roa.fpages = d_opages.p ? d_opages.p : table->d_flat_pages;
+      roa.chunks = shape.d_chunks;
+      roa.items = shape.d_items;
+      roa.bitmap = d_bitmap.p;
+      roa.item_counts = d_item_counts.p;
+      roa.item_base = d_item_base.p;
+      roa.n_items = uint32_t(items.size());
+      roa.plan_ncols = ncols;
+      roa.n = n;
+      roa.vals = ob.vals.p;
+      roa.nulls = ob.nulls.p;
+      roa.ranges = ob.ranges.p;
+      roa.handles = handles.p;
+      uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
+      if (const char* g = getenv("PQB_GRID")) grid = std::max(1, atoi(g));   // debugging aid: several items per CTA
+      Timer t_enc, t_sort;
+      bool sort_timed = false;
+      PQB_CUDA(cudaEventRecord(t_enc.a, stream));
+      k_order_rows_encode<<<grid, 256, 0, stream>>>(roa);
+      PQB_CUDA(cudaEventRecord(t_enc.b, stream));
+      std::unique_ptr<WindowRun> wrun;
+      if (win) {
+        // the window: sort and count, then the kept positions and the extra columns in gather's block
+        wrun = std::make_unique<WindowRun>(*win, n, n_part);
+        keep = std::min(wrun->count(ob, row_nulls_first, nullptr, stream, metrics), lim);
+        launches += 1 + wrun->launches;
+        if (keep > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
+        if (keep) {
+          kept.alloc(keep, stream);
+          win_fill = [&](long long* rn, long long* prows) { wrun->fill(nullptr, keep, kept.p, rn, prows, stream); };
+          gather(keep, handles.p, kept.p, nullptr);
+        }
+      } else {
+        launches += 1 + order_sort(ob, roa.nterms, n, row_nulls_first, uint32_t(keep), nullptr, kept, stream, metrics, t_sort, &sort_timed);
+        if (!smerge) gather(keep, handles.p, kept.p, nullptr);
+      }
+      PQB_CUDA(cudaStreamSynchronize(stream));
+      if (keep && !smerge) metrics.d2h_bytes += L.copy_bytes;
+      float ms = 0, ms2 = 0;
+      cudaEventElapsedTime(&ms, t_enc.a, t_enc.b);
+      if (sort_timed) cudaEventElapsedTime(&ms2, t_sort.a, t_sort.b);
+      metrics.order_ms = double(ms) + double(ms2) + (wrun ? wrun->ms() : 0.0);
+    }
+    shape.last_total.store(total);
+    if (smerge) {
+      // every rank's first rows: the same candidates and the same order on every rank, each output row projected by
+      // the rank that holds it and the ranks' blocks summed
+      DevBuf<unsigned long long> owned;
+      launches += smerge->merge(obuf ? obuf->vals.p : nullptr, obuf ? obuf->nulls.p : nullptr, n, kept.p, handles.p, shape.d_items,
+                                row_nulls_first, owned, stream, metrics);
+      keep = smerge->keep;
+      if (keep) {
+        gather(keep, nullptr, nullptr, owned.p);
+        metrics.d2h_bytes += L.copy_bytes;
+      }
+      PQB_CUDA(cudaStreamSynchronize(stream));
+      smerge->report(verbose, metrics);
+      total = smerge->total;
+    }
+    n_rows = keep;
+  } else if (!items.empty()) {
+    n_rows = sized_pass(1, block, [&](unsigned long long cap) {
+      if (cap > 0x7ffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "more than 2^31 projected rows in one result: add a LIMIT");
+      gather(cap, nullptr, nullptr, nullptr);
+      return L.copy_bytes;
+    }, nullptr);
+  }
+  PQB_CUDA(cudaEventRecord(t_all.b, stream));
+  PQB_CUDA(cudaStreamSynchronize(stream));
+  check_corrupt();
+  keep_device(block, d_block, L.copy_bytes);
+  metrics.rows_selected = total;
+  if (!n_rows) {   // one empty batch, in a heap block
+    lay_out(0);
+    block = heap_block(L.off);
+  }
+  slice(L, pcs, block, n_rows);
+}
+
+// selected row ordinals, ascending, or the one row of SELECT COUNT(*) [, COUNT(*)...] WHERE ...
+void ResultTail::selection() {
+  count_selected();
+  std::shared_ptr<PinnedBlock> ids_block;   // selected row ordinals land in page-locked memory, batches alias it
+  unsigned long long n_ids = 0;
+  DevBuf<unsigned long long> d_ids;
+  if (want_rows && !items.empty()) {
+    n_ids = sized_pass(0, ids_block, [&](unsigned long long cap) -> uint64_t {
+      if (!cap) return 0;
+      d_ids.alloc(cap, stream);
+      const uint32_t grid = std::min<uint32_t>(uint32_t(items.size()), uint32_t(ctx.sm_count() * 8));
+      k_compact_row_ids<<<grid, 256, 0, stream>>>(d_bitmap.p, shape.d_items, d_item_counts.p, d_item_base.p, uint32_t(items.size()), d_ids.p, cap);
+      launches++;
+      ids_block = std::make_shared<PinnedBlock>();
+      ids_block->p = ctx.pinned_acquire(cap * 8);
+      ids_block->bytes = cap * 8;
+      PQB_CUDA(cudaMemcpyAsync(ids_block->p, d_ids.p, cap * 8, cudaMemcpyDeviceToHost, stream));
+      return cap * 8;
+    }, "scan done, selected-row total on host");
+  }
+  PQB_CUDA(cudaEventRecord(t_all.b, stream));
+  PQB_CUDA(cudaStreamSynchronize(stream));
+  mark("results on host");
+  metrics.rows_selected = total;
+  unsigned long long corrupt_ranks = 0;
+  if (d.n_aggs && allreduce) {
+    // SELECT COUNT(*) under PQ_QUERY_ALLREDUCE: the total's all-reduce also counts the ranks that met a corrupt page,
+    // so that every rank throws, not only the ones that met it
+    const unsigned long long bad = h_counters[1] ? 1ull : 0ull;
+    PQB_CUDA(cudaMemcpyAsync(d_total.p + 1, &bad, 8, cudaMemcpyHostToDevice, stream));
+    comm_allreduce_u64(d_total.p, 2, 0, stream);
+    unsigned long long w[2];
+    PQB_CUDA(cudaMemcpyAsync(w, d_total.p, 16, cudaMemcpyDeviceToHost, stream));
+    PQB_CUDA(cudaStreamSynchronize(stream));
+    total = w[0];
+    corrupt_ranks = w[1];
+  }
+  check_corrupt();
+  if (corrupt_ranks) throw Error(PQ_ERR_CORRUPT, "corrupt or unsupported page encoding met on the device of " + std::to_string(corrupt_ranks) + " other rank(s)");
+  if (d.n_aggs) {
+    metrics.groups_total = 1;
+    // one row, ordered trivially; LIMIT 0 keeps none, and a window keeps it when its rank range holds rn = 1
+    const bool win_drops = win && !(win->offset == 0 && win->fetch != 0);
+    if ((ordered && d.limit == 0) || win_drops) {
+      metrics.groups = 0;
+    } else {
+      one_row(std::vector<BlockCol>(d.n_aggs, BlockCol{"count(*)"}), std::vector<bool>(d.n_aggs, false), total);
+      metrics.groups = 1;
+    }
+  } else if (want_rows) {
+    if (!n_ids) ids_block = heap_block(0);   // one empty batch
+    slice(BlockLayout(n_ids, batch_rows, 0), {BlockCol{"__row_id"}}, ids_block, n_ids);   // 8-byte ids, no NULL counts
+  }
+}
+
+void ResultTail::finish() {
   float ms = 0;
   cudaEventElapsedTime(&ms, t_all.a, t_all.b);
   metrics.device_ms = ms;
@@ -3977,10 +4029,13 @@ void Query::json(uint32_t flags, const char** out, uint64_t* len) {
   ja.lines = lines ? 1u : 0u;
   ja.batch_rows = batch_rows_;
   ja.words_per_batch = (batch_rows_ + 31) / 32;
-  size_t nonempty = 0;
-  for (const OutBatch& b : batches_) nonempty += b.rows ? 1 : 0;
+  // every column of the result is a slice of one block: its kept device copy, the mapped page-locked copy, or (a heap
+  // block, one row) a copy uploaded here
+  const PinnedBlock& blk = *first->cols[0].block;
+  DevBuf<uint64_t> up;
+  if (!blk.dev && !blk.heap.empty()) up.upload(blk.heap, stream);
+  const uint8_t* base = blk.dev ? blk.dev : up.p ? reinterpret_cast<const uint8_t*>(up.p) : blk.p;
   std::vector<uint8_t> keys;
-  std::vector<DevBuf<uint8_t>> temps(ncols * 3);
   for (size_t c = 0; c < ncols; c++) {
     const OutColumn& oc = first->cols[c];
     JsonCol& jc = ja.cols[c];
@@ -3996,37 +4051,9 @@ void Query::json(uint32_t flags, const char** out, uint64_t* len) {
     jc.key_len = uint32_t(keys.size()) - jc.key_off;
     bool any_nulls = false;
     for (const OutBatch& b : batches_) if (b.rows) any_nulls = any_nulls || b.cols[c].null_count != 0;
-    if (oc.ext_all) {
-      // device-assembled result: one regular layout over all batches (values and offsets contiguous, bit-packed buffers per batch)
-      const uint8_t* base = oc.ext->dev ? oc.ext->dev : oc.ext->p;   // the kept device block, or the mapped page-locked copy
-      jc.values = base + oc.ext_off;
-      jc.validity = any_nulls ? reinterpret_cast<const uint32_t*>(base + oc.ext_validity_off) : nullptr;
-      jc.offsets = oc.type == PQ_T_UTF8 ? reinterpret_cast<const int32_t*>(base + oc.ext_offsets_off) : nullptr;
-    } else if (oc.ext) {
-      if (oc.null_count || oc.type == PQ_T_UTF8 || oc.type == PQ_T_BOOL) throw Error(PQ_ERR_UNSUPPORTED, "JSON egress: result layout not supported");
-      jc.values = oc.ext->p + oc.ext_off;   // 8-byte values of all batches, contiguous (row ids)
-    } else {
-      // a small host-built batch (a global aggregate over zero rows, COUNT(*) only): its buffers go up as they are
-      if (nonempty != 1) throw Error(PQ_ERR_UNSUPPORTED, "JSON egress: result layout not supported");
-      ja.batch_rows = 0x7fffffffu;
-      ja.words_per_batch = 0;
-      std::vector<uint8_t> v = oc.values;
-      v.resize(std::max<size_t>((v.size() + 7) & ~size_t(7), 8), 0);   // 8-byte values / whole words of bit-packed booleans
-      temps[3 * c].upload(v, stream);
-      jc.values = temps[3 * c].p;
-      if (oc.null_count) {
-        std::vector<uint8_t> vv = oc.validity;
-        vv.resize((vv.size() + 7) & ~size_t(7), 0);   // the kernel reads whole 32-bit words
-        temps[3 * c + 1].upload(vv, stream);
-        jc.validity = reinterpret_cast<const uint32_t*>(temps[3 * c + 1].p);
-      }
-      if (oc.type == PQ_T_UTF8) {
-        std::vector<uint8_t> o(oc.offsets.size() * 4);
-        std::memcpy(o.data(), oc.offsets.data(), o.size());
-        temps[3 * c + 2].upload(o, stream);
-        jc.offsets = reinterpret_cast<const int32_t*>(temps[3 * c + 2].p);
-      }
-    }
+    jc.values = base + oc.values_off;   // values and offsets contiguous over all batches, bit-packed buffers per batch
+    jc.validity = any_nulls ? reinterpret_cast<const uint32_t*>(base + oc.validity_off) : nullptr;
+    jc.offsets = oc.type == PQ_T_UTF8 ? reinterpret_cast<const int32_t*>(base + oc.offsets_off) : nullptr;
   }
   DevBuf<uint8_t> d_keys; d_keys.upload(keys, stream);
   ja.keys = d_keys.p;

@@ -139,7 +139,7 @@ bool Context::is_pinned(const void* p) {
 }
 
 PinnedBlock::~PinnedBlock() {
-  if (p) Context::get().pinned_release(p);
+  if (p && heap.empty()) Context::get().pinned_release(p);
 }
 
 // ---------------- HostFile ----------------

@@ -15,7 +15,7 @@ from oracle.oracle import Oracle
 from parseable_b200 import _lib as L
 from parseable_b200 import synth
 from parseable_b200.query import (DeviceTable, HostFile, Query, QueryError, StandardTableProvider, TimeRange,
-                                  avg, col, count, count_star, execute, lit, max_, min_, sum_)
+                                  Window, avg, col, count, count_star, execute, lit, max_, min_, sum_)
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -879,3 +879,22 @@ def test_json_egress_on_device(data_dir, built):
     assert prov.scan(projection=["v"], filters=[col("k") == 99], json="lines").json_text == b""
     res = prov.aggregate([], [count_star(), sum_("v")], [col("k") == 99], json="array")              # one host-built row: COUNT 0, SUM NULL
     assert res.to_json() == [{"count(*)": 0}]
+    # results laid out on the host, as JSON and as Arrow (twice: the second run of a scan sizes its result from the first)
+    none = [col("k") == 99]
+    aggs = [count_star(), count("x"), sum_("v"), min_("s"), max_("flag"), avg("x")]
+    res = prov.aggregate([], aggs, none, json="array")                                    # a global aggregate over zero rows
+    assert res.to_json() == [{"count(*)": 0, "count(x)": 0}]
+    assert res.table().to_pylist() == [{"count(*)": 0, "count(x)": 0, "sum(v)": None, "min(s)": None, "max(flag)": None, "avg(x)": None}]
+    assert [f.type for f in res.table().schema] == [pa.int64(), pa.int64(), pa.int64(), pa.string(), pa.bool_(), pa.float64()]
+    n1 = ora.count([col("k") == 1])
+    for window, extra in ((None, {}), (Window(row_number=True, partition_rows=True), {"row_number": 1, "partition_rows": 1})):
+        for mode in ("array", "lines"):
+            res = prov.aggregate([], [count_star()], [col("k") == 1], json=mode, window=window)   # COUNT(*) alone
+            assert res.to_json() == res.table().to_pylist() == [{"count(*)": n1, **extra}]
+    for _ in range(2):
+        res = prov.scan(projection=["v", "s", "flag", "p_timestamp"], filters=none, json="array")   # an empty projection
+        assert res.json_text == b"[]" and len(res.batches) == 1
+        assert res.table().num_rows == 0 and res.table().schema.types == [pa.int64(), pa.string(), pa.bool_(), pa.timestamp("ms")]
+        res = prov.scan(filters=none, json="lines")                                                  # empty row ids
+        assert res.json_text == b"" and len(res.batches) == 1
+        assert res.table().num_rows == 0 and res.table().column_names == ["__row_id"]

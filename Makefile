@@ -49,7 +49,7 @@ oracle/liboracle.so: oracle/oracle.c
 	$(CC) -O2 -std=c11 -fPIC -shared -Wall -o $@ $< -lm
 
 tools: tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so \
-       tools/liblz_host.so tools/liblz_host_desc.so tools/libdecomp_dev.so tools/libhash_merge_host.so
+       tools/liblz_host.so tools/liblz_host_desc.so tools/libdecomp_dev.so tools/libhash_merge_host.so tools/libin_set_host.so
 # the LZ4_RAW / SNAPPY decoders on the host, lanes in ascending and in descending order
 tools/liblz_host.so: tools/lz_host.cpp $(CSRC)/lz_decode.cuh $(CSRC)/zstd_decode.cuh
 	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
@@ -65,6 +65,9 @@ tools/liborder_keys_host.so: tools/order_keys_host.cpp $(CSRC)/order_keys.cuh $(
 # the merge of a hashed GROUP BY's rank tables on the host (f64 sums bit for bit: no contraction)
 tools/libhash_merge_host.so: tools/hash_merge_host.cpp $(CSRC)/hash_merge.cuh $(CSRC)/decode_core.cuh $(CSRC)/device_structs.hpp
 	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -shared -Wall -I$(CSRC) -o $@ $<
+# the membership set of PQ_OP_IN on the host
+tools/libin_set_host.so: tools/in_set_host.cpp $(CSRC)/in_set.cuh $(CSRC)/decode_core.cuh $(CSRC)/device_structs.hpp
+	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -I$(CSRC) -o $@ $<
 tools/libjson_host.so: tools/json_host.cpp $(CSRC)/json_egress.cuh $(CSRC)/ryu_f64.cuh $(CSRC)/ryu_tables.inc
 	$(CXX) -O2 -std=c++17 -fPIC -shared -Wall -Wno-maybe-uninitialized -I$(CSRC) -o $@ $<
 tools/libzstd_host.so: tools/zstd_host.cpp $(CSRC)/zstd_decode.cuh $(CSRC)/inflate_decode.cuh
@@ -74,6 +77,6 @@ tools/libdecode_core_host.so: tools/decode_core_host.cpp $(CSRC)/decode_core.cuh
 
 clean:
 	rm -rf $(OBJDIR) $(LIB) $(HOSTCOMM_LIB) oracle/liboracle.so tools/libdecode_core_host.so tools/libzstd_host.so tools/libjson_host.so tools/liborder_keys_host.so tools/libregex_host.so \
-	      tools/liblz_host.so tools/liblz_host_desc.so tools/libdecomp_dev.so tools/libhash_merge_host.so
+	      tools/liblz_host.so tools/liblz_host_desc.so tools/libdecomp_dev.so tools/libhash_merge_host.so tools/libin_set_host.so
 
 .PHONY: all oracle tools clean

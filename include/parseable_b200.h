@@ -124,7 +124,8 @@ typedef enum {
   PQ_OP_OR = 6,       /* pop 2, push Kleene OR                                        */
   PQ_OP_NOT = 7,      /* pop 1, push Kleene NOT                                       */
   PQ_OP_CONST = 8,    /* push literal TRUE/FALSE/NULL (lit.type BOOL or NULL)         */
-  PQ_OP_REGEX = 9     /* push  col ~ pattern  (flags: NOT, case-insens; see below)    */
+  PQ_OP_REGEX = 9,    /* push  col ~ pattern  (flags: NOT, case-insens; see below)    */
+  PQ_OP_IN = 10       /* push  col [NOT] IN (e1, ..., en)  (flags: NOT, has NULL; below) */
 } PqOpKind;
 
 typedef enum { PQ_EQ = 0, PQ_NE = 1, PQ_LT = 2, PQ_LE = 3, PQ_GT = 4, PQ_GE = 5 } PqCmp;
@@ -155,6 +156,30 @@ typedef enum { PQ_EQ = 0, PQ_NE = 1, PQ_LT = 2, PQ_LE = 3, PQ_GT = 4, PQ_GE = 5 
  *     DFA". */
 #define PQ_REGEX_NEGATED 1u
 #define PQ_REGEX_CASE_INSENSITIVE 2u
+
+/* PQ_OP_IN: `col IN (e1, ..., en)` (`NOT IN` with PQ_IN_NEGATED), DataFusion's InList, restated, not checked: the Kleene
+ * OR of `col = ei`, each exactly what PQ_OP_CMP with PQ_EQ computes, and NOT IN its Kleene NOT.
+ *   - NULL input -> NULL; a column missing from a file reads as NULL.  PQ_IN_HAS_NULL: the list also holds a NULL, so a
+ *     row that matches no element gives NULL, not FALSE (`x NOT IN (1, NULL)` is never TRUE).  Duplicates are allowed.
+ *   - lit.type is the elements' PqType, lit.i64 their count n, and lit.str / lit.str_len the packed elements: for I64,
+ *     TS_MS, DATE32, F64 (IEEE bits) and BOOL (0 / 1), n little-endian 8-byte values (str_len == 8 n); for UTF8, n
+ *     entries of (u32 little-endian length, bytes), the PLAIN BYTE_ARRAY layout, which must fill str_len exactly.  n == 0
+ *     only with PQ_IN_HAS_NULL: `x IN (NULL)` is NULL on every row.
+ *   - Each element is coerced as a PQ_OP_CMP / PQ_EQ literal and refused the same way: Int64 / Timestamp(ms) take I64
+ *     and TS_MS elements, and an F64 element that is integral (2^63 matches what `= 2^63` matches); Float64 takes F64
+ *     and I64 elements and compares bits (-0.0 and 0.0 differ, a NaN matches only its own payload); Utf8 takes UTF8,
+ *     bytewise; Date32 takes DATE32 only; Boolean takes BOOL.  An element the column cannot take returns the code
+ *     PQ_OP_CMP returns for it, with a message that names the element's index.
+ *   - PQ_ERR_INVALID_ARG: n == 0 without PQ_IN_HAS_NULL, n < 0, str_len that does not match n, str == NULL with n > 0,
+ *     unknown flags.
+ *   - PQ_ERR_UNSUPPORTED: more than 2^20 elements or 64 MiB of element bytes in one list, and a query that reads pages
+ *     without a flat-store copy.
+ *   - One IN is one leaf predicate whatever n is (two for an Int64 column whose list holds 2^63); PQ_IN_HAS_NULL, and
+ *     2^63, add two postfix ops, and PQ_IN_NEGATED one, within the program's 40 ops and the stack depth of 8.
+ * Dictionary pages answer the list once per dictionary entry; pages without a dictionary probe a hash set per row.  Row
+ * groups whose footer [min, max] holds no element are pruned. */
+#define PQ_IN_NEGATED 1u
+#define PQ_IN_HAS_NULL 2u
 
 typedef struct {
   int32_t type; /* PqType */

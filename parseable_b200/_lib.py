@@ -21,10 +21,11 @@ ERR_NAMES = {-1: "PQ_ERR_INVALID_ARG", -2: "PQ_ERR_UNSUPPORTED", -3: "PQ_ERR_IO"
 
 PQ_T_NULL, PQ_T_BOOL, PQ_T_I64, PQ_T_F64, PQ_T_UTF8, PQ_T_TS_MS = range(6)
 PQ_T_DATE32 = 7   # Date32: days since 1970-01-01 in PqLiteral.i64 (6 is PQ_T_TS_NS, planning only)
-PQ_OP_CMP, PQ_OP_IS_NULL, PQ_OP_IS_NOT_NULL, PQ_OP_LIKE, PQ_OP_AND, PQ_OP_OR, PQ_OP_NOT, PQ_OP_CONST, PQ_OP_REGEX = range(1, 10)
+PQ_OP_CMP, PQ_OP_IS_NULL, PQ_OP_IS_NOT_NULL, PQ_OP_LIKE, PQ_OP_AND, PQ_OP_OR, PQ_OP_NOT, PQ_OP_CONST, PQ_OP_REGEX, PQ_OP_IN = range(1, 11)
 PQ_EQ, PQ_NE, PQ_LT, PQ_LE, PQ_GT, PQ_GE = range(6)
 PQ_LIKE_NEGATED, PQ_LIKE_CASE_INSENSITIVE = 1, 2
 PQ_REGEX_NEGATED, PQ_REGEX_CASE_INSENSITIVE = 1, 2
+PQ_IN_NEGATED, PQ_IN_HAS_NULL = 1, 2
 (PQ_AGG_COUNT_STAR, PQ_AGG_COUNT, PQ_AGG_SUM, PQ_AGG_MIN, PQ_AGG_MAX, PQ_AGG_AVG, PQ_AGG_COUNT_DISTINCT, PQ_AGG_MEDIAN,
  PQ_AGG_PERCENTILE_CONT) = range(9)
 PQ_QUERY_COUNT_ONLY, PQ_QUERY_ALLREDUCE, PQ_QUERY_EMIT_ROW_IDS, PQ_QUERY_ALLGATHER = 1, 2, 4, 8

@@ -105,12 +105,12 @@ struct DevColumn {
   uint32_t has_delta, has_plain, has_dict;
 };
 
-enum DevLeafKind : uint8_t { LK_CMP = 1, LK_IS_NULL = 2, LK_IS_NOT_NULL = 3, LK_LIKE = 4, LK_REGEX = 5 };
+enum DevLeafKind : uint8_t { LK_CMP = 1, LK_IS_NULL = 2, LK_IS_NOT_NULL = 3, LK_LIKE = 4, LK_REGEX = 5, LK_IN = 6 };
 // leaves answered by the column's value (per dictionary entry through a LUT, or per row), not by its validity alone
 #ifdef __CUDACC__
 __host__ __device__
 #endif
-inline bool value_leaf(uint32_t kind) { return kind == LK_CMP || kind == LK_LIKE || kind == LK_REGEX; }
+inline bool value_leaf(uint32_t kind) { return kind == LK_CMP || kind == LK_LIKE || kind == LK_REGEX || kind == LK_IN; }
 
 struct DevLeaf {
   uint8_t kind;                // DevLeafKind
@@ -119,7 +119,7 @@ struct DevLeaf {
   uint8_t lit_kind;            // DevKind of the literal after coercion
   uint32_t flags;              // LIKE / REGEX flags
   int64_t lit_i64;             // I64/TS/BOOL literal or f64 bits
-  uint32_t str_off, str_len;   // UTF8 literal / LIKE pattern / REGEX DFA blob (8-aligned) in the literal pool
+  uint32_t str_off, str_len;   // UTF8 literal / LIKE pattern / REGEX DFA blob / IN set (both 8-aligned) in the literal pool
   uint32_t lut_off;            // this leaf's per-dictionary-entry LUT (bytes) starts at lut_off; entry = chunk.lut_base+idx
   uint32_t _pad;
 };

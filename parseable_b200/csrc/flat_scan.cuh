@@ -37,6 +37,7 @@
 #include "decode_core.cuh"
 #include "device_structs.hpp"
 #include "flat_store.cuh"
+#include "in_set.cuh"
 #include "order_keys.cuh"       // order_encode: the value keys of MEDIAN / PERCENTILE_CONT pairs
 #include "ptx_utils.cuh"
 #include "regex_match.cuh"
@@ -316,7 +317,9 @@ __device__ __forceinline__ uint32_t row_id(const ColCtx& c, bool is_bool, const 
 // ---- leaves -------------------------------------------------------------------------------------
 // Everything a consumer needs about one leaf for the CURRENT slab; built once per slab (warp uniform)
 // so that the row loops below carry no interpretation: the switch on the page kind sits outside them.
-enum LeafMode : uint32_t { LM_FALSE = 0, LM_TRUE = 1, LM_REGLUT = 2, LM_MEMLUT = 3, LM_PLAIN8 = 4, LM_BITS = 5, LM_BYTES = 6 };
+// LM_INSET: an IN leaf over a page without a dictionary (PLAIN8 values or PLAIN byte arrays), probed row by row
+enum LeafMode : uint32_t { LM_FALSE = 0, LM_TRUE = 1, LM_REGLUT = 2, LM_MEMLUT = 3, LM_PLAIN8 = 4, LM_BITS = 5, LM_BYTES = 6,
+                           LM_INSET = 7 };
 struct LeafCtx {
   ColCtx c;
   const uint8_t* lut;        // this leaf's LUT bytes for the chunk (global); LM_BYTES: the page's values section instead
@@ -331,7 +334,8 @@ struct LeafCtx {
   bool f64;
 };
 
-template <bool DIRECT8>
+// INSET = false: an IN leaf keeps LM_PLAIN8 / LM_BYTES (the k_flat_agg instantiations that are never launched for one)
+template <bool DIRECT8, bool INSET = true>
 __device__ __forceinline__ void leaf_ctx(LeafCtx& x, const DevPlan& plan, const DevScanArgs& a, const FlatStage& st,
                                          const uint8_t* stage_base, const FlatLayout& L, uint32_t l) {
   const DevLeaf& lf = plan.leaves[l];
@@ -347,12 +351,13 @@ __device__ __forceinline__ void leaf_ctx(LeafCtx& x, const DevPlan& plan, const 
   x.lf = &lf;
   x.lit_pool = a.lit_pool;
   if (lf.kind == LK_IS_NULL || lf.kind == LK_IS_NOT_NULL || x.c.absent) x.mode = LM_FALSE;   // answered by the validity alone
-  else if (sc.fkind == FK_BYTES) { x.mode = LM_BYTES; x.lut = a.arena + sc.dict8; }
+  else if (sc.fkind == FK_BYTES) { x.mode = INSET && lf.kind == LK_IN ? LM_INSET : LM_BYTES; x.lut = a.arena + sc.dict8; }
   else if (sc.fkind == FK_INDEX) {
     if ((st.regmask >> l) & 1u) x.mode = LM_REGLUT;
     else if (sc.bw == 0) x.mode = __ldg(x.lut) ? LM_TRUE : LM_FALSE;   // one-entry dictionary: no bits at all
     else x.mode = LM_MEMLUT;
-  } else x.mode = sc.fkind == FK_PLAIN8 ? LM_PLAIN8 : LM_BITS;
+  } else if (sc.fkind == FK_PLAIN8) x.mode = INSET && lf.kind == LK_IN ? LM_INSET : LM_PLAIN8;
+  else x.mode = LM_BITS;
 }
 
 __device__ __forceinline__ bool plain_cmp(uint64_t bits, const LeafCtx& x) {
@@ -385,9 +390,49 @@ __device__ __forceinline__ uint64_t regex_rows(const LeafCtx& x, uint32_t sel, u
   return regex_rows(x.lut, x.c.colw, x.c.phase, x.c.vw, x.c.vphase, x.lit_pool + x.lf->str_off, x.lf->flags, sel, row0);
 }
 
+// An IN list over rows without a dictionary: the hash-set probe stays out of line for the same reason.  One row
+// (k_flat_filter; a string's bytes s[0, n), or a number's 8 bytes v) ...
+__device__ __noinline__ bool inset_row(const uint8_t* set, const uint8_t* s, uint32_t n, uint64_t v) {
+  return in_set_has(set, s, n, v);
+}
+__device__ __forceinline__ bool inset_row(const LeafCtx& x, uint32_t row) {
+  const uint8_t* set = x.lit_pool + x.lf->str_off;
+  if (x.c.fkind == FK_BYTES) {
+    const uint8_t* sp = x.lut + bits32_at(x.c.colw, x.c.phase + row * 32);
+    return inset_row(set, sp, load_u32_unaligned(sp - 4), 0);
+  }
+  return inset_row(set, nullptr, 0, x.c.v8[row]);
+}
+// ... or the rows `sel` of one k_flat_agg<.., RX = true> thread, as regex_rows: `vals` the PLAIN byte arrays' values
+// section, or nullptr and `v8` the PLAIN8 values.  Returns the TRUE rows in the low word, the NULL rows in the high word.
+__device__ __noinline__ uint64_t inset_rows(const uint8_t* vals, const uint64_t* v8, const uint32_t* colw, uint32_t phase,
+                                            const uint32_t* vw, uint32_t vphase, const uint8_t* set, uint32_t sel, uint32_t row0) {
+  uint32_t t = 0, n = 0;
+  for (; sel; sel &= sel - 1) {
+    const uint32_t i = __ffs(sel) - 1, row = row0 + i * kAggConsumers;
+    if (vw) {
+      const uint32_t b = vphase + row;
+      if (!((vw[b >> 5] >> (b & 31)) & 1u)) { n |= 1u << i; continue; }
+    }
+    bool in;
+    if (vals) {
+      const uint8_t* sp = vals + bits32_at(colw, phase + row * 32);
+      in = in_set_has_bytes(set, sp, load_u32_unaligned(sp - 4));
+    } else {
+      in = in_set_has_u64(set, v8[row]);
+    }
+    if (in) t |= 1u << i;
+  }
+  return (uint64_t(n) << 32) | t;
+}
+__device__ __forceinline__ uint64_t inset_rows(const LeafCtx& x, uint32_t sel, uint32_t row0) {
+  return inset_rows(x.c.fkind == FK_BYTES ? x.lut : nullptr, x.c.v8, x.c.colw, x.c.phase, x.c.vw, x.c.vphase,
+                    x.lit_pool + x.lf->str_off, sel, row0);
+}
+
 // the comparison for ONE non-NULL row; x.mode is warp uniform, so the switch costs one predictable branch.
-// REGEX = false: no DFA walk here (k_flat_agg answers LK_REGEX leaves on LM_BYTES pages with regex_rows, in its RX
-// instantiations only)
+// REGEX = false: no DFA walk and no set probe here (k_flat_agg answers LK_REGEX leaves on LM_BYTES pages with regex_rows,
+// and LM_INSET leaves with inset_rows, in its RX instantiations only)
 template <bool REGEX = true>
 __device__ __forceinline__ bool leaf_row(const LeafCtx& x, uint32_t row) {
   switch (x.mode) {
@@ -407,6 +452,7 @@ __device__ __forceinline__ bool leaf_row(const LeafCtx& x, uint32_t row) {
       return (x.lf->flags & 1u) ? !t : t;
     }
     default: {
+      if (REGEX && x.mode == LM_INSET) return inset_row(x, row);
       const uint32_t pb = x.c.phase + row;
       return cmp_i64(int64_t((x.c.colw[pb >> 5] >> (pb & 31)) & 1u), x.lit, x.cmp);
     }
@@ -516,6 +562,7 @@ __device__ __forceinline__ uint32_t leaf_dense(const LeafCtx& x, uint32_t tc, ui
   switch (x.mode) {
     case LM_FALSE: return 0u;
     case LM_TRUE: return 0xffffffffu;
+    case LM_INSET:
     case LM_BYTES: {   // only the rows in `need` (in range, not NULL: a NULL row owns no bytes)
       uint32_t m = 0, mm = need;
       while (mm) {
@@ -889,8 +936,8 @@ __device__ __forceinline__ void pct_emit(const DevPairSet& ps, uint32_t vsel, co
 }
 
 // DIST: the instantiation with the COUNT(DISTINCT) pass, PCT: the one with the MEDIAN / PERCENTILE_CONT pair emission,
-// RX: the one with the DFA walk of a regular expression over pages without a dictionary (queries without them run code
-// that does not contain them)
+// RX: the one with the out-of-line leaves over pages without a dictionary, a regular expression's DFA walk and an IN
+// list's set probe (queries without them run code that does not contain them)
 template <int KR, bool HASHED, bool DIST = false, bool PCT = false, bool RX = false>
 __global__ void __launch_bounds__(kAggThreads, 1)
 k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLayout L, const __grid_constant__ DevScanArgs a) {
@@ -939,10 +986,12 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
         if (plan.conj) {
           for (uint32_t l = 0; l < plan.nleaves; l++) {
             LeafCtx x;
-            leaf_ctx<true>(x, plan, a, st, base, L, l);
+            leaf_ctx<true, RX>(x, plan, a, st, base, L, l);
             uint32_t m = 0;
             if (RX && x.mode == LM_BYTES && x.lkind == LK_REGEX) {
               m = uint32_t(regex_rows(x, sel, tc));
+            } else if (RX && x.mode == LM_INSET) {
+              m = uint32_t(inset_rows(x, sel, tc));
             } else if (!x.c.absent && !x.c.vw && x.lkind != LK_IS_NULL && x.lkind != LK_IS_NOT_NULL) {   // no NULLs in this slab: plain comparison
 #pragma unroll
               for (int i = 0; i < KR; i++)
@@ -962,10 +1011,10 @@ k_flat_agg(const __grid_constant__ DevPlan plan, const __grid_constant__ FlatLay
             const DevPredOp op = plan.pred[i];
             if (op.kind == PK_LEAF) {
               LeafCtx x;
-              leaf_ctx<true>(x, plan, a, st, base, L, op.arg);
+              leaf_ctx<true, RX>(x, plan, a, st, base, L, op.arg);
               Tri32 v{0u, 0u};
-              if (RX && x.mode == LM_BYTES && x.lkind == LK_REGEX) {
-                const uint64_t r = regex_rows(x, sel, tc);
+              if (RX && (x.mode == LM_INSET || (x.mode == LM_BYTES && x.lkind == LK_REGEX))) {
+                const uint64_t r = x.mode == LM_INSET ? inset_rows(x, sel, tc) : regex_rows(x, sel, tc);
                 v = {uint32_t(r), uint32_t(r >> 32)};
               } else
 #pragma unroll

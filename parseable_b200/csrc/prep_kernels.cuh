@@ -11,6 +11,7 @@
 
 #include "decode_core.cuh"
 #include "device_structs.hpp"
+#include "in_set.cuh"
 #include "regex_match.cuh"
 
 namespace pqb {
@@ -113,10 +114,13 @@ __global__ void k_leaf_luts(DevPrepArgs a, const __grid_constant__ DevPlan plan)
         const uint8_t* lit = a.lit_pool + lf.str_off;
         if (lf.kind == LK_CMP) t = cmp_result(cmp_bytes(s, len, lit, lf.str_len), lf.cmp);
         else if (lf.kind == LK_REGEX) t = regex_match(s, len, lit) != ((lf.flags & 1u) != 0);   // once per dictionary entry
+        else if (lf.kind == LK_IN) t = in_set_has_bytes(lit, s, len);
         else {
           t = like_match(s, len, lit, lf.str_len, lf.cmp, (lf.flags & 2u) != 0);
           if (lf.flags & 1u) t = !t;
         }
+      } else if (lf.kind == LK_IN) {   // Int64 / Float64: the entry's 8 bytes (Float64: its bits) in the set
+        t = in_set_has_u64(a.lit_pool + lf.str_off, load_u64_unaligned(a.arena + ch.dict_off + uint64_t(e) * 8));
       } else if (kind == DK_I64) {
         t = cmp_i64((int64_t)load_u64_unaligned(a.arena + ch.dict_off + uint64_t(e) * 8), lf.lit_i64, lf.cmp);
       } else if (kind == DK_F64) {

@@ -33,6 +33,7 @@
 #include "order_kernels.cuh"
 #include "percentile_kernels.cuh"
 #include "hash_merge.cuh"
+#include "in_set.cuh"
 #include "regex_compile.hpp"
 
 namespace pqb {
@@ -138,7 +139,62 @@ struct HostLeaf {
   DevLeaf d{};
   int qcol = -1;
   std::string str;
+  // LK_IN: the distinct members, sorted in the column's order, for pruning (Int64 / Timestamp / Date32 signed, Float64 as
+  // doubles, Utf8 bytewise); in_nan: some Float64 member is a NaN
+  std::vector<int64_t> in_i64;
+  std::vector<double> in_f64;
+  std::vector<std::string> in_str;
+  bool in_nan = false;
 };
+
+// min / max statistics of an Int64 / Timestamp / Date32 chunk (an INT32 (Date32) leaf's sign-extended like its values)
+bool stats_i64(const ColumnStats& st, int64_t& mn, int64_t& mx) {
+  if (st.min.size() == 8 && st.max.size() == 8) {
+    std::memcpy(&mn, st.min.data(), 8);
+    std::memcpy(&mx, st.max.data(), 8);
+    return true;
+  }
+  if (st.min.size() == 4 && st.max.size() == 4) {
+    int32_t a, b;
+    std::memcpy(&a, st.min.data(), 4);
+    std::memcpy(&b, st.max.data(), 4);
+    mn = a;
+    mx = b;
+    return true;
+  }
+  return false;
+}
+
+// An IN leaf is FALSE on a chunk none of whose members lies in the chunk's [min, max]
+Tri in_from_stats(const HostLeaf& lf, uint8_t kind, const ColumnStats& st) {
+  bool hit;
+  if (kind == DK_I64) {
+    int64_t mn, mx;
+    if (!stats_i64(st, mn, mx)) return TRI_MAYBE;
+    const auto it = std::lower_bound(lf.in_i64.begin(), lf.in_i64.end(), mn);
+    hit = it != lf.in_i64.end() && *it <= mx;
+  } else if (kind == DK_F64) {
+    if (st.min.size() != 8 || st.max.size() != 8) return TRI_MAYBE;
+    double mn, mx;
+    std::memcpy(&mn, st.min.data(), 8);
+    std::memcpy(&mx, st.max.data(), 8);
+    // as for `=`: NaN rows may lie outside [min, max], and the bounds may fold -0.0 / 0.0
+    if (lf.in_nan || std::isnan(mn) || std::isnan(mx) || mn == 0.0 || mx == 0.0) return TRI_MAYBE;
+    const auto it = std::lower_bound(lf.in_f64.begin(), lf.in_f64.end(), mn);
+    hit = it != lf.in_f64.end() && *it <= mx;
+  } else if (kind == DK_STR) {
+    // (a truncated max is still an upper bound)
+    auto cmps = [](const std::string& a, const std::string& b) {
+      return cmp_bytes((const uint8_t*)a.data(), uint32_t(a.size()), (const uint8_t*)b.data(), uint32_t(b.size()));
+    };
+    const auto it = std::lower_bound(lf.in_str.begin(), lf.in_str.end(), st.min,
+                                     [&](const std::string& a, const std::string& b) { return cmps(a, b) < 0; });
+    hit = it != lf.in_str.end() && cmps(*it, st.max) <= 0;
+  } else {
+    return TRI_MAYBE;
+  }
+  return hit ? TRI_MAYBE : TRI_FALSE;
+}
 
 // Can `col <cmp> lit` be decided for a whole chunk from its min/max statistics?
 Tri leaf_from_stats(const HostLeaf& lf, uint8_t kind, const TableChunk& ch, uint32_t rg_rows) {
@@ -153,22 +209,12 @@ Tri leaf_from_stats(const HostLeaf& lf, uint8_t kind, const TableChunk& ch, uint
   if (lf.d.kind == LK_IS_NULL) return no_nulls ? TRI_FALSE : (all_nulls ? TRI_TRUE : TRI_MAYBE);
   if (lf.d.kind == LK_IS_NOT_NULL) return no_nulls ? TRI_TRUE : (all_nulls ? TRI_FALSE : TRI_MAYBE);
   if (all_nulls) return TRI_FALSE;
+  if (lf.d.kind == LK_IN && st.has_min && st.has_max) return in_from_stats(lf, kind, st);
   if (lf.d.kind != LK_CMP || !st.has_min || !st.has_max) return TRI_MAYBE;
   int lo_c, hi_c;  // sign of compare(min, lit), compare(max, lit)
   if (kind == DK_I64) {
     int64_t mn, mx;
-    if (st.min.size() == 8 && st.max.size() == 8) {
-      std::memcpy(&mn, st.min.data(), 8);
-      std::memcpy(&mx, st.max.data(), 8);
-    } else if (st.min.size() == 4 && st.max.size() == 4) {   // an INT32 (Date32) leaf: sign-extended like its values
-      int32_t a, b;
-      std::memcpy(&a, st.min.data(), 4);
-      std::memcpy(&b, st.max.data(), 4);
-      mn = a;
-      mx = b;
-    } else {
-      return TRI_MAYBE;
-    }
+    if (!stats_i64(st, mn, mx)) return TRI_MAYBE;
     lo_c = mn < lf.d.lit_i64 ? -1 : (mn > lf.d.lit_i64 ? 1 : 0);
     hi_c = mx < lf.d.lit_i64 ? -1 : (mx > lf.d.lit_i64 ? 1 : 0);
   } else if (kind == DK_F64) {
@@ -1732,10 +1778,215 @@ void Query::run(const PqQueryDesc& d) {
   auto is_date = [&](uint32_t c) { return out_type_of(c) == PQ_T_DATE32; };
 
   // ---- predicate compile ----
+  // `col <cmp> lit` with the literal coerced into lf.d.cmp / lit_i64 / str, as PQ_OP_CMP coerces it; PQ_OP_IN coerces
+  // each of its elements as the PQ_EQ case
+  auto coerce_cmp = [&](HostLeaf& lf, uint32_t qc, int cmp, const PqLiteral& lit) {
+    const uint8_t kind = plan.cols[qc].kind;
+    lf.d.cmp = uint8_t(cmp);
+    // Date32 compares with Date32 only (DataFusion rejects the other pairs or casts both sides to Timestamp)
+    if (is_date(qc) != (lit.type == PQ_T_DATE32))
+      throw Error(PQ_ERR_UNSUPPORTED, std::string("comparison of the ") + type_name(out_type_of(qc)) + " column '" +
+                                          d.columns[qc].name + "' with a " + type_name(lit.type) + " literal is not on the GPU path");
+    if (lit.type == PQ_T_DATE32 && (lit.i64 < INT32_MIN || lit.i64 > INT32_MAX))
+      throw Error(PQ_ERR_INVALID_ARG, "Date32 literal outside int32 days");
+    // literal coercion as DataFusion's type coercion does for column-vs-literal (SURVEY §8 a11)
+    switch (kind) {
+      case DK_I64:
+        if (lit.type == PQ_T_I64 || lit.type == PQ_T_TS_MS || lit.type == PQ_T_DATE32) lf.d.lit_i64 = lit.i64;
+        else if (lit.type == PQ_T_F64 && std::nearbyint(lit.f64) == lit.f64 && lit.f64 >= -9223372036854775808.0 && lit.f64 < 9223372036854775808.0)
+          lf.d.lit_i64 = int64_t(lit.f64);
+        else if (lit.type == PQ_T_F64) {
+          // DataFusion coerces the COLUMN to Float64 and compares there.  Against a literal that is no int64 this
+          // has an exact integer restatement (a non-integer double is < 2^52 in magnitude, where the cast of
+          // any int64 at or beyond it cannot cross it):  v > 100.5  <=>  v > 100,  v < 100.5  <=>  v < 101,
+          // v = 100.5 never, v != 100.5 always (for non-NULL v).  A NaN sits by its sign bit (totalOrder): above
+          // every value without it, below every value (-inf included) with it.
+          const double L = lit.f64;
+          const int64_t kMin = std::numeric_limits<int64_t>::min();
+          auto never = [&] { lf.d.cmp = PQ_LT; lf.d.lit_i64 = kMin; };    // v < INT64_MIN
+          auto always = [&] { lf.d.cmp = PQ_GE; lf.d.lit_i64 = kMin; };   // v >= INT64_MIN
+          const bool nan = std::isnan(L);
+          const bool above = (nan && !std::signbit(L)) || L >= 9223372036854775808.0;   // greater than every int64
+          const bool below = (nan && std::signbit(L)) || L < -9223372036854775808.0;     // less than every int64
+          if (L == 9223372036854775808.0) {
+            // 2^63: the int64 values from 2^63 - 512 up round to it when cast (to nearest, ties to even), the
+            // others cast below it
+            const int64_t kTop = std::numeric_limits<int64_t>::max() - 511;
+            switch (cmp) {
+              case PQ_EQ: case PQ_GE: lf.d.cmp = PQ_GE; lf.d.lit_i64 = kTop; break;
+              case PQ_NE: case PQ_LT: lf.d.cmp = PQ_LT; lf.d.lit_i64 = kTop; break;
+              case PQ_LE: always(); break;
+              default: never(); break;   // PQ_GT
+            }
+          } else if (above || below) {
+            const bool lt = cmp == PQ_LT || cmp == PQ_LE, gt = cmp == PQ_GT || cmp == PQ_GE;
+            if (cmp == PQ_EQ) never();
+            else if (cmp == PQ_NE) always();
+            else if ((above && lt) || (below && gt)) always();
+            else never();
+          } else {
+            const int64_t fl = int64_t(std::floor(L)), ce = fl + 1;   // |L| < 2^52
+            switch (cmp) {
+              case PQ_EQ: never(); break;
+              case PQ_NE: always(); break;
+              case PQ_GT: case PQ_GE: lf.d.cmp = PQ_GT; lf.d.lit_i64 = fl; break;
+              default: lf.d.cmp = PQ_LT; lf.d.lit_i64 = ce; break;   // PQ_LT, PQ_LE
+            }
+          }
+        } else throw Error(PQ_ERR_INVALID_ARG, "Int64 column compared with a non-numeric literal");
+        break;
+      case DK_F64:
+        if (lit.type == PQ_T_F64) lf.d.lit_i64 = int64_t(f64_bits(lit.f64));
+        else if (lit.type == PQ_T_I64) lf.d.lit_i64 = int64_t(f64_bits(double(lit.i64)));  // `status = 200` on a Float64 column
+        else throw Error(PQ_ERR_INVALID_ARG, "Float64 column compared with a non-numeric literal");
+        break;
+      case DK_BOOL:
+        if (lit.type != PQ_T_BOOL) throw Error(PQ_ERR_INVALID_ARG, "Boolean column compared with a non-boolean literal");
+        lf.d.lit_i64 = lit.i64 ? 1 : 0;
+        break;
+      case DK_STR:
+        if (lit.type != PQ_T_UTF8) throw Error(PQ_ERR_INVALID_ARG, "Utf8 column compared with a non-string literal");
+        lf.str.assign(lit.str ? lit.str : "", lit.str_len);
+        break;
+      default: throw Error(PQ_ERR_UNSUPPORTED, "comparison on this column type");
+    }
+  };
   std::vector<HostLeaf> leaves;
   std::vector<DevPredOp> prog;
   std::vector<uint8_t> lit_pool(16, 0);
   bool has_null_const = false;
+  auto push_leaf = [&](HostLeaf& lf) {
+    if (leaves.size() >= (size_t)kMaxLeaves) throw Error(PQ_ERR_UNSUPPORTED, "too many leaf predicates");
+    if ((plan.cols[lf.qcol].kind == DK_STR && value_leaf(lf.d.kind)) || lf.d.kind == LK_IN) {
+      if (lit_pool.size() + lf.str.size() > 0xfffffff0ull) throw Error(PQ_ERR_UNSUPPORTED, "predicate literals too large");
+      lf.d.str_off = uint32_t(lit_pool.size());   // a multiple of 8: the pool starts at 16 and every entry is padded to 8
+      lf.d.str_len = uint32_t(lf.str.size());
+      lit_pool.insert(lit_pool.end(), lf.str.begin(), lf.str.end());
+      lit_pool.resize(align_up(uint32_t(lit_pool.size()) + 8, 8), 0);
+    }
+    prog.push_back({PK_LEAF, uint8_t(leaves.size())});
+    leaves.push_back(std::move(lf));
+  };
+  // PQ_OP_IN: the Kleene OR of `col = e` over the elements.  Its distinct matching values become one LK_IN leaf (one value:
+  // the LK_CMP / PQ_EQ leaf it equals; a Boolean column: a CMP leaf), the one element whose EQ restatement is a range
+  // (2^63 against Int64) its CMP leaf OR'd to it, a NULL element `OR NULL`, and NOT IN a NOT.  Pushes one value.
+  auto compile_in = [&](const PqPredOp& op, uint32_t qc, int depth) {
+    const std::string where = std::string("IN list on '") + d.columns[qc].name + "': ";
+    if (op.flags & ~(PQ_IN_NEGATED | PQ_IN_HAS_NULL)) throw Error(PQ_ERR_INVALID_ARG, where + "unknown flags");
+    const bool has_null = (op.flags & PQ_IN_HAS_NULL) != 0, negated = (op.flags & PQ_IN_NEGATED) != 0;
+    const PqLiteral& lit = op.lit;
+    if (lit.i64 < 0) throw Error(PQ_ERR_INVALID_ARG, where + "negative element count");
+    if (lit.i64 == 0 && !has_null) throw Error(PQ_ERR_INVALID_ARG, where + "no elements and no NULL");
+    if (lit.i64 > int64_t(kInSetMaxElems) || lit.str_len > kInSetMaxBytes)
+      throw Error(PQ_ERR_UNSUPPORTED, where + "more than 2^20 elements or 64 MiB of elements");
+    const uint32_t n = uint32_t(lit.i64);
+    if (n && !lit.str) throw Error(PQ_ERR_INVALID_ARG, where + "str == NULL with elements");
+    const uint8_t* p = reinterpret_cast<const uint8_t*>(lit.str);
+    const uint8_t kind = plan.cols[qc].kind;
+    // the elements: (offset, length) in str for Utf8, else 8 bytes each
+    std::vector<const uint8_t*> sp;
+    std::vector<uint32_t> sl;
+    if (lit.type == PQ_T_UTF8) {
+      uint64_t pos = 0;
+      for (uint32_t k = 0; k < n; k++) {
+        if (pos + 4 > lit.str_len) throw Error(PQ_ERR_INVALID_ARG, where + "element " + std::to_string(k) + " runs past str_len");
+        const uint32_t len = load_u32_unaligned(p + pos);
+        if (pos + 4 + len > lit.str_len) throw Error(PQ_ERR_INVALID_ARG, where + "element " + std::to_string(k) + " runs past str_len");
+        sp.push_back(p + pos + 4);
+        sl.push_back(len);
+        pos += 4 + uint64_t(len);
+      }
+      if (pos != lit.str_len) throw Error(PQ_ERR_INVALID_ARG, where + "str_len does not match the elements");
+    } else if (lit.str_len != uint64_t(n) * 8) {
+      throw Error(PQ_ERR_INVALID_ARG, where + "str_len is not 8 bytes per element");
+    }
+    // each element coerced as PQ_OP_CMP / PQ_EQ coerces its literal: a value, never equal (Int64 against a non-integral
+    // Float64), or, for 2^63 against Int64, the range v >= 2^63 - 511
+    std::vector<int64_t> vals;
+    bool top = false;
+    for (uint32_t k = 0; k < n; k++) {
+      PqLiteral el{};
+      el.type = lit.type;
+      if (lit.type == PQ_T_UTF8) { el.str = reinterpret_cast<const char*>(sp[k]); el.str_len = sl[k]; }
+      else std::memcpy(lit.type == PQ_T_F64 ? static_cast<void*>(&el.f64) : static_cast<void*>(&el.i64), p + uint64_t(k) * 8, 8);
+      if (lit.type == PQ_T_NULL) throw Error(PQ_ERR_INVALID_ARG, where + "element " + std::to_string(k) + " has no type");
+      HostLeaf e;
+      try {
+        coerce_cmp(e, qc, PQ_EQ, el);
+      } catch (const Error& x) {
+        throw Error(x.code, where + "element " + std::to_string(k) + ": " + x.what());
+      }
+      if (kind == DK_STR) break;   // every element is a Utf8 literal: their bytes are the values
+      if (e.d.cmp == PQ_EQ) vals.push_back(e.d.lit_i64);
+      else if (e.d.cmp == PQ_GE) top = true;
+    }
+    std::sort(vals.begin(), vals.end());
+    vals.erase(std::unique(vals.begin(), vals.end()), vals.end());
+    HostLeaf lf;
+    lf.qcol = int(qc);
+    lf.d.col = uint8_t(qc);
+    lf.d.kind = LK_CMP;
+    lf.d.cmp = PQ_EQ;
+    bool has_leaf = true;
+    if (n == 0) {
+      has_leaf = false;
+    } else if (kind == DK_BOOL) {
+      if (vals.size() == 2) { lf.d.cmp = PQ_GE; lf.d.lit_i64 = 0; }   // both: every non-NULL row
+      else lf.d.lit_i64 = vals[0];
+    } else if (kind == DK_STR) {
+      std::vector<uint32_t> ord(n);
+      for (uint32_t k = 0; k < n; k++) ord[k] = k;
+      auto less = [&](uint32_t a, uint32_t b) { return cmp_bytes(sp[a], sl[a], sp[b], sl[b]) < 0; };
+      std::sort(ord.begin(), ord.end(), less);
+      ord.erase(std::unique(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return !less(a, b) && !less(b, a); }), ord.end());
+      if (ord.size() == 1) {
+        lf.str.assign(reinterpret_cast<const char*>(sp[ord[0]]), sl[ord[0]]);
+      } else {
+        lf.d.kind = LK_IN;
+        for (uint32_t k : ord) lf.in_str.emplace_back(reinterpret_cast<const char*>(sp[k]), sl[k]);
+        const std::vector<uint8_t> blob = in_set_build_bytes(sp.data(), sl.data(), n);
+        lf.str.assign(blob.begin(), blob.end());
+      }
+    } else if (vals.empty()) {
+      if (top) has_leaf = false;
+      else { lf.d.cmp = PQ_LT; lf.d.lit_i64 = std::numeric_limits<int64_t>::min(); }   // no element matches a value
+    } else if (vals.size() == 1) {
+      lf.d.lit_i64 = vals[0];
+    } else {
+      lf.d.kind = LK_IN;
+      if (kind == DK_F64) {
+        for (int64_t v : vals) {
+          const double x = bits_f64(uint64_t(v));
+          if (std::isnan(x)) lf.in_nan = true;
+          else lf.in_f64.push_back(x);
+        }
+        std::sort(lf.in_f64.begin(), lf.in_f64.end());
+      } else {
+        lf.in_i64 = vals;
+      }
+      const std::vector<uint8_t> blob = in_set_build_u64(reinterpret_cast<const uint64_t*>(vals.data()), vals.size());
+      lf.str.assign(blob.begin(), blob.end());
+    }
+    if (leaves.size() + (has_leaf ? 1 : 0) + (top ? 1 : 0) > (size_t)kMaxLeaves) throw Error(PQ_ERR_UNSUPPORTED, "too many leaf predicates");
+    if (depth + ((has_leaf && top) || has_null ? 2 : 1) > kPredStack) throw Error(PQ_ERR_UNSUPPORTED, "predicate nesting too deep");
+    if (has_leaf) push_leaf(lf);
+    if (top) {
+      HostLeaf t;
+      t.qcol = int(qc);
+      t.d.col = uint8_t(qc);
+      t.d.kind = LK_CMP;
+      t.d.cmp = PQ_GE;
+      t.d.lit_i64 = std::numeric_limits<int64_t>::max() - 511;
+      push_leaf(t);
+      if (has_leaf) prog.push_back({PK_OR, 0});
+    }
+    if (has_null) {
+      prog.push_back({PK_CONST, 2});
+      has_null_const = true;
+      if (has_leaf || top) prog.push_back({PK_OR, 0});
+    }
+    if (negated && (has_leaf || top)) prog.push_back({PK_NOT, 0});
+  };
   {
     int depth = 0;
     for (uint32_t i = 0; i < d.n_pred; i++) {
@@ -1778,83 +2029,15 @@ void Query::run(const PqQueryDesc& d) {
           } else {
             lf.d.kind = LK_CMP;
             if (op.cmp < PQ_EQ || op.cmp > PQ_GE) throw Error(PQ_ERR_INVALID_ARG, "bad comparison operator");
-            lf.d.cmp = uint8_t(op.cmp);
-            // Date32 compares with Date32 only (DataFusion rejects the other pairs or casts both sides to Timestamp)
-            if (is_date(uint32_t(op.col)) != (op.lit.type == PQ_T_DATE32))
-              throw Error(PQ_ERR_UNSUPPORTED, std::string("comparison of the ") + type_name(out_type_of(uint32_t(op.col))) + " column '" +
-                                                  d.columns[op.col].name + "' with a " + type_name(op.lit.type) + " literal is not on the GPU path");
-            if (op.lit.type == PQ_T_DATE32 && (op.lit.i64 < INT32_MIN || op.lit.i64 > INT32_MAX))
-              throw Error(PQ_ERR_INVALID_ARG, "Date32 literal outside int32 days");
-            // literal coercion as DataFusion's type coercion does for column-vs-literal (SURVEY §8 a11)
-            switch (kind) {
-              case DK_I64:
-                if (op.lit.type == PQ_T_I64 || op.lit.type == PQ_T_TS_MS || op.lit.type == PQ_T_DATE32) lf.d.lit_i64 = op.lit.i64;
-                else if (op.lit.type == PQ_T_F64 && std::nearbyint(op.lit.f64) == op.lit.f64 && op.lit.f64 >= -9223372036854775808.0 && op.lit.f64 < 9223372036854775808.0)
-                  lf.d.lit_i64 = int64_t(op.lit.f64);
-                else if (op.lit.type == PQ_T_F64) {
-                  // DataFusion coerces the COLUMN to Float64 and compares there.  Against a literal that is no int64 this
-                  // has an exact integer restatement (a non-integer double is < 2^52 in magnitude, where the cast of
-                  // any int64 at or beyond it cannot cross it):  v > 100.5  <=>  v > 100,  v < 100.5  <=>  v < 101,
-                  // v = 100.5 never, v != 100.5 always (for non-NULL v).  A NaN sits by its sign bit (totalOrder): above
-                  // every value without it, below every value (-inf included) with it.
-                  const double L = op.lit.f64;
-                  const int64_t kMin = std::numeric_limits<int64_t>::min();
-                  auto never = [&] { lf.d.cmp = PQ_LT; lf.d.lit_i64 = kMin; };    // v < INT64_MIN
-                  auto always = [&] { lf.d.cmp = PQ_GE; lf.d.lit_i64 = kMin; };   // v >= INT64_MIN
-                  const bool nan = std::isnan(L);
-                  const bool above = (nan && !std::signbit(L)) || L >= 9223372036854775808.0;   // greater than every int64
-                  const bool below = (nan && std::signbit(L)) || L < -9223372036854775808.0;     // less than every int64
-                  if (L == 9223372036854775808.0) {
-                    // 2^63: the int64 values from 2^63 - 512 up round to it when cast (to nearest, ties to even), the
-                    // others cast below it
-                    const int64_t kTop = std::numeric_limits<int64_t>::max() - 511;
-                    switch (op.cmp) {
-                      case PQ_EQ: case PQ_GE: lf.d.cmp = PQ_GE; lf.d.lit_i64 = kTop; break;
-                      case PQ_NE: case PQ_LT: lf.d.cmp = PQ_LT; lf.d.lit_i64 = kTop; break;
-                      case PQ_LE: always(); break;
-                      default: never(); break;   // PQ_GT
-                    }
-                  } else if (above || below) {
-                    const bool lt = op.cmp == PQ_LT || op.cmp == PQ_LE, gt = op.cmp == PQ_GT || op.cmp == PQ_GE;
-                    if (op.cmp == PQ_EQ) never();
-                    else if (op.cmp == PQ_NE) always();
-                    else if ((above && lt) || (below && gt)) always();
-                    else never();
-                  } else {
-                    const int64_t fl = int64_t(std::floor(L)), ce = fl + 1;   // |L| < 2^52
-                    switch (op.cmp) {
-                      case PQ_EQ: never(); break;
-                      case PQ_NE: always(); break;
-                      case PQ_GT: case PQ_GE: lf.d.cmp = PQ_GT; lf.d.lit_i64 = fl; break;
-                      default: lf.d.cmp = PQ_LT; lf.d.lit_i64 = ce; break;   // PQ_LT, PQ_LE
-                    }
-                  }
-                } else throw Error(PQ_ERR_INVALID_ARG, "Int64 column compared with a non-numeric literal");
-                break;
-              case DK_F64:
-                if (op.lit.type == PQ_T_F64) lf.d.lit_i64 = int64_t(f64_bits(op.lit.f64));
-                else if (op.lit.type == PQ_T_I64) lf.d.lit_i64 = int64_t(f64_bits(double(op.lit.i64)));  // `status = 200` on a Float64 column
-                else throw Error(PQ_ERR_INVALID_ARG, "Float64 column compared with a non-numeric literal");
-                break;
-              case DK_BOOL:
-                if (op.lit.type != PQ_T_BOOL) throw Error(PQ_ERR_INVALID_ARG, "Boolean column compared with a non-boolean literal");
-                lf.d.lit_i64 = op.lit.i64 ? 1 : 0;
-                break;
-              case DK_STR:
-                if (op.lit.type != PQ_T_UTF8) throw Error(PQ_ERR_INVALID_ARG, "Utf8 column compared with a non-string literal");
-                lf.str.assign(op.lit.str ? op.lit.str : "", op.lit.str_len);
-                break;
-              default: throw Error(PQ_ERR_UNSUPPORTED, "comparison on this column type");
-            }
+            coerce_cmp(lf, uint32_t(op.col), op.cmp, op.lit);
           }
-          if (kind == DK_STR && value_leaf(lf.d.kind)) {
-            lf.d.str_off = uint32_t(lit_pool.size());   // a multiple of 8: the pool starts at 16 and every entry is padded to 8
-            lf.d.str_len = uint32_t(lf.str.size());
-            lit_pool.insert(lit_pool.end(), lf.str.begin(), lf.str.end());
-            lit_pool.resize(align_up(uint32_t(lit_pool.size()) + 8, 8), 0);
-          }
-          prog.push_back({PK_LEAF, uint8_t(leaves.size())});
-          leaves.push_back(lf);
+          push_leaf(lf);
+          depth++;
+          break;
+        }
+        case PQ_OP_IN: {
+          if (op.col < 0 || uint32_t(op.col) >= d.n_columns) throw Error(PQ_ERR_INVALID_ARG, "predicate column out of range");
+          compile_in(op, uint32_t(op.col), depth);
           depth++;
           break;
         }
@@ -1877,6 +2060,7 @@ void Query::run(const PqQueryDesc& d) {
       if (depth > kPredStack) throw Error(PQ_ERR_UNSUPPORTED, "predicate nesting too deep");
     }
     if (d.n_pred && depth != 1) throw Error(PQ_ERR_INVALID_ARG, "predicate program does not reduce to one value");
+    if (prog.size() > (size_t)kMaxPredOps) throw Error(PQ_ERR_UNSUPPORTED, "predicate program too long");
   }
 
   // ---- row-group pruning + constant folding of leaves that statistics decide everywhere ----
@@ -1999,7 +2183,7 @@ void Query::run(const PqQueryDesc& d) {
     // PQB_VERBOSE: per live leaf, the flat page kinds under it and the leaf mode each flat piece selects (leaf_ctx in
     // flat_scan.cuh: a register LUT for a dictionary of <= 32 entries at an index width <= 5), with the index widths
     // seen per mode; "off-grid" counts the index pieces whose first bit is off the 128-bit grid of the staged copy
-    static const char* const kLeafKind[] = {"?", "CMP", "IS_NULL", "IS_NOT_NULL", "LIKE", "REGEX"};
+    static const char* const kLeafKind[] = {"?", "CMP", "IS_NULL", "IS_NOT_NULL", "LIKE", "REGEX", "IN"};
     for (size_t l = 0; l < leaves.size(); l++) {
       if (leaf_slot[l] < 0) continue;
       const uint32_t s = uint32_t(slot_of[leaves[l].qcol]);
@@ -2028,7 +2212,7 @@ void Query::run(const PqQueryDesc& d) {
         modes += "}";
       }
       fprintf(stderr, "[pqb] leaf %d: column '%s', %s, flat pages %s, widest index %u, register LUT %s, off-grid %u, absent %u,%s\n",
-              leaf_slot[l], table->columns[shape_cols[s]].name.c_str(), kLeafKind[leaves[l].d.kind < 6 ? leaves[l].d.kind : 0],
+              leaf_slot[l], table->columns[shape_cols[s]].name.c_str(), kLeafKind[leaves[l].d.kind < 7 ? leaves[l].d.kind : 0],
               pk.empty() ? "-" : pk.c_str(), widest, bws[0] ? (bws[1] || bws[2] ? "some" : "all") : "none", offgrid, absent,
               modes.empty() ? " -" : modes.c_str());
     }
@@ -2049,7 +2233,7 @@ void Query::run(const PqQueryDesc& d) {
   {
     // k_scan: conjunction of 1-4 CMP/LIKE leaves: specialised octet pass over no-NULL dictionary slabs
     bool c4 = conj && nleaves >= 1 && nleaves <= 4;
-    for (uint32_t l = 0; l < nleaves; l++) c4 &= value_leaf(plan.leaves[l].kind);
+    for (uint32_t l = 0; l < nleaves; l++) c4 &= value_leaf(plan.leaves[l].kind) && plan.leaves[l].kind != LK_IN;
     const char* fa = getenv("PQB_FAST_AND");
     plan.fast_and = c4 && !(fa && fa[0] == '0');
   }
@@ -2286,6 +2470,14 @@ void Query::run(const PqQueryDesc& d) {
       refuse(std::string(ag.fn == AG_MIN ? "MIN(" : "MAX(") + d.columns[d.aggs[a].col].name +
              ") over Utf8 / Boolean needs a flat-store copy of every page the query reads: " + shape->why_general);
   }
+  // k_scan has no IN path: its pages are read through the flat store only
+  for (uint32_t l = 0; l < nleaves; l++)
+    if (plan.leaves[l].kind == LK_IN && n_general) {
+      refuse("IN list on '" + table->columns[shape_cols[plan.leaves[l].col]].name +
+             "' needs a flat-store copy of every page the query reads" +
+             (shape->why_general.empty() ? std::string(" (the flat kernels are switched off)") : ": " + shape->why_general));
+      break;
+    }
   if (merge_rows && n_general)   // (without other ranks: thrown with the other scan refusals below)
     refuse("ORDER BY on a scan needs a flat-store copy of every page the query reads: " + shape->why_general);
   // the merge breaks ties by __row_id, which is global only when every rank opened the same file list and scans its row
@@ -2295,9 +2487,13 @@ void Query::run(const PqQueryDesc& d) {
            std::to_string(table->shard_count) + ", shard_index " + std::to_string(table->shard_index) + " on rank " +
            std::to_string(comm_rank()) + " of " + std::to_string(comm_nranks()) + "): only then is __row_id global");
   if (!refusal.empty() && !agree) throw Error(PQ_ERR_UNSUPPORTED, refusal);
-  // k_flat_agg walks a regular expression's DFA per row only in its RX instantiations
+  // k_flat_agg answers an out-of-line leaf over pages without a dictionary (a regular expression's DFA walk, an IN list's
+  // set probe) only in its RX instantiations
   bool rx_bytes = false;
-  for (uint32_t l = 0; l < nleaves; l++) rx_bytes |= plan.leaves[l].kind == LK_REGEX && plan.cols[plan.leaves[l].col].has_plain;
+  for (uint32_t l = 0; l < nleaves; l++) {
+    const DevLeaf& lf = plan.leaves[l];
+    rx_bytes |= (lf.kind == LK_REGEX || lf.kind == LK_IN) && (plan.cols[lf.col].has_plain || plan.cols[lf.col].has_delta);
+  }
   plan.n_items = uint32_t(items.size());
   metrics.bytes_scanned = scanned_bytes;
   // an aggregated column whose footers promise null_count == 0 in every row group read: its non-null
@@ -3091,7 +3287,7 @@ void Query::run(const PqQueryDesc& d) {
         PQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(ctx.smem_optin())));
         kern<<<grid, kAggThreads, FL.total, stream>>>(kplan, FL, sa);
       };
-      if (rx_bytes) {   // a regular expression over pages without a dictionary: the instantiations with the DFA walk
+      if (rx_bytes) {   // a regular expression or an IN list over pages without a dictionary: the out-of-line leaves
         if (plan.npct) {
           if (plan.hashed) go(k_flat_agg<4, true, false, true, true>);
           else go(k_flat_agg<2, false, false, true, true>);

@@ -17,6 +17,7 @@ from __future__ import annotations
 import ctypes as C
 import datetime as _dt
 import re
+import struct
 from dataclasses import dataclass, field
 from typing import Any, Iterable, Sequence
 
@@ -41,7 +42,7 @@ class QueryError(RuntimeError):
 # ----------------------------------------------------------------------------- expressions
 @dataclass
 class Expr:
-    kind: str                      # 'col' 'lit' 'cmp' 'and' 'or' 'not' 'is_null' 'is_not_null' 'like' 'regex'
+    kind: str                      # 'col' 'lit' 'cmp' 'and' 'or' 'not' 'is_null' 'is_not_null' 'like' 'regex' 'in'
     args: tuple = ()
     op: int = 0
     flags: int = 0
@@ -73,6 +74,10 @@ class Expr:
         """``col ~ pattern`` (``~*``, ``!~``, ``!~*``): an unanchored regular-expression search (PQ_OP_REGEX)."""
         f = (L.PQ_REGEX_NEGATED if negated else 0) | (L.PQ_REGEX_CASE_INSENSITIVE if case_insensitive else 0)
         return Expr("regex", (self, Expr("lit", (pattern,))), flags=f)
+
+    def isin(self, values: Iterable, negated=False):
+        """``col [NOT] IN (values)`` (PQ_OP_IN): the Kleene OR of ``col = v``; ``None`` among the values is a NULL element."""
+        return Expr("in", (self, tuple(values)), flags=L.PQ_IN_NEGATED if negated else 0)
 
 
 def col(name: str) -> Expr:
@@ -216,6 +221,29 @@ class _Desc:
             raise TypeError(f"unsupported literal {v!r}")
         return out
 
+    def in_list(self, col: int, values: list, flags: int) -> L.PqPredOp:
+        """One PQ_OP_IN over elements of one literal type, packed as the header lays them out."""
+        t = self.literal(values[0]).type if values else L.PQ_T_NULL
+        if t == L.PQ_T_UTF8:
+            bs = [v.encode() if isinstance(v, str) else v for v in values]
+            data = b"".join(struct.pack("<I", len(b)) + b for b in bs)
+            return self._in_op(col, flags, t, len(bs), data)
+        if any(isinstance(v, int) and not -(1 << 63) <= v < (1 << 63) for v in values):
+            raise QueryError(L.PQ_ERR_INVALID_ARG, "IN list element outside int64")
+        lits = [self.literal(v) for v in values]
+        if t == L.PQ_T_F64:
+            data = struct.pack(f"<{len(lits)}d", *(x.f64 for x in lits))
+        else:
+            data = struct.pack(f"<{len(lits)}q", *(x.i64 for x in lits))
+        return self._in_op(col, flags, t, len(lits), data)
+
+    def _in_op(self, col: int, flags: int, t: int, n: int, data: bytes) -> L.PqPredOp:
+        buf = C.create_string_buffer(data, len(data) + 1)
+        self.keep.append(buf)
+        lit = L.PqLiteral()
+        lit.type, lit.i64, lit.str, lit.str_len = t, n, C.cast(buf, C.c_char_p), len(data)
+        return L.PqPredOp(kind=L.PQ_OP_IN, col=col, flags=flags, lit=lit)
+
     def compile_pred(self, e: Expr, ops: list):
         if e.kind in ("and", "or"):
             self.compile_pred(e.args[0], ops)
@@ -246,6 +274,31 @@ class _Desc:
             if a.kind != "col" or b.kind != "lit":
                 raise QueryError(L.PQ_ERR_UNSUPPORTED, "only column <op> literal comparisons are pushed to the GPU")
             ops.append(L.PqPredOp(kind=L.PQ_OP_CMP, col=self.col_index(a.args[0]), cmp=op, lit=self.literal(b.args[0])))
+        elif e.kind == "in":
+            c, values = e.args
+            if c.kind != "col":
+                raise QueryError(L.PQ_ERR_UNSUPPORTED, "IN on a non-column expression")
+            ci = self.col_index(c.args[0])
+            # one PQ_OP_IN per literal type, OR'd together; the NULL element and NOT go with the whole list
+            groups: dict = {}
+            for v in values:
+                if v is not None:
+                    t = L.PQ_T_UTF8 if isinstance(v, (str, bytes)) else self.literal(v).type
+                    groups.setdefault(t, []).append(v)
+            has_null = L.PQ_IN_HAS_NULL if any(v is None for v in values) else 0
+            if not groups:
+                if not has_null:
+                    raise QueryError(L.PQ_ERR_INVALID_ARG, "IN with an empty list")
+                groups[L.PQ_T_NULL] = []
+            for i, vs in enumerate(groups.values()):
+                ops.append(self.in_list(ci, vs, has_null if i == 0 else 0))
+                if i:
+                    ops.append(L.PqPredOp(kind=L.PQ_OP_OR))
+            if e.flags & L.PQ_IN_NEGATED:
+                if len(groups) == 1:
+                    ops[-1].flags |= L.PQ_IN_NEGATED
+                else:
+                    ops.append(L.PqPredOp(kind=L.PQ_OP_NOT))
         elif e.kind == "lit":
             ops.append(L.PqPredOp(kind=L.PQ_OP_CONST, lit=self.literal(e.args[0])))
         else:

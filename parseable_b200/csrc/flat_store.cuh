@@ -628,7 +628,7 @@ __device__ __forceinline__ bool dbp_decode_warp(const uint8_t* __restrict__ p, u
   uint32_t bad = 0;
   if (lane == 0) {
     if (!rd_varint(p, pos, end, bs) || !rd_varint(p, pos, end, nm) || !rd_varint(p, pos, end, total) || !rd_varint(p, pos, end, fz)) bad = 1;
-    if (!bad && (nm == 0 || nm > 32 || bs == 0 || bs % nm != 0 || (bs / nm) % 32 != 0 || bs > (1u << 20))) bad = 1;
+    if (!bad && (nm == 0 || bs == 0 || bs % nm != 0 || (bs / nm) % 32 != 0 || bs > (1u << 20))) bad = 1;
     if (!bad && (want != ~0u ? total != want : total > cap)) bad = 1;
   }
   bad = __shfl_sync(0xffffffffu, bad, 0);
@@ -644,7 +644,8 @@ __device__ __forceinline__ bool dbp_decode_warp(const uint8_t* __restrict__ p, u
   if (lane == 0 && nvals) put(0u, last);
   uint32_t done = 1;                        // values written
   while (done < nvals && !bad) {
-    // block header: min delta + one bit width per miniblock (lane m keeps width m)
+    // block header: min delta + one bit width per miniblock (any number of miniblocks: the format only asks that a
+    // miniblock hold a multiple of 32 values, and the Rust `parquet` crate or parquet-mr may write more than 32 of them)
     uint64_t mz = 0;
     if (lane == 0) { if (!rd_varint(p, pos, end, mz) || pos + nm > end) bad = 1; }
     bad = __shfl_sync(0xffffffffu, bad, 0);
@@ -652,10 +653,10 @@ __device__ __forceinline__ bool dbp_decode_warp(const uint8_t* __restrict__ p, u
     mz = __shfl_sync(0xffffffffu, mz, 0);
     pos = __shfl_sync(0xffffffffu, pos, 0);
     const int64_t min_delta = int64_t(mz >> 1) ^ -int64_t(mz & 1);
-    const uint32_t mybw = lane < nm ? p[pos + lane] : 0u;
+    const uint64_t wpos = pos;
     pos += nm;
     for (uint32_t m = 0; m < nm && done < nvals; m++) {
-      const uint32_t bw = __shfl_sync(0xffffffffu, mybw, m);
+      const uint32_t bw = p[wpos + m];   // the same byte for every lane: one broadcast load
       if (bw > 64 || pos + (uint64_t(vpm) * bw) / 8 > end + 8) { bad = 1; break; }
       const uint32_t take = nvals - done < vpm ? nvals - done : vpm;
       for (uint32_t v0 = 0; v0 < take; v0 += 32) {

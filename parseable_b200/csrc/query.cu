@@ -2394,8 +2394,12 @@ void Query::run(const PqQueryDesc& d) {
     plan.cols[s].max_bw = shape->max_bw[s];
     if (shape->has_delta[s] && plan.cols[s].kind != DK_I64)
       refuse("column '" + cname + "': DELTA_BINARY_PACKED is decoded for INT64 columns only");
-    if (shape->has_plain[s] && plan.cols[s].kind == DK_STR && shape->n_uncopied)
-      refuse("column '" + cname + "': PLAIN (dictionary-fallback) string pages without a flat-store copy are not decoded on the GPU");
+    // k_scan reads no string values out of pages without a dictionary (PLAIN, and DELTA_(LENGTH_)BYTE_ARRAY rewritten
+    // as PLAIN): a leaf over them would count no row.  So they are refused whenever k_scan takes items: pages without
+    // a flat-store copy, or the flat kernels switched off (then every page has a copy that no kernel reads)
+    if (shape->has_plain[s] && plan.cols[s].kind == DK_STR && n_general)
+      refuse("column '" + cname + "': PLAIN (dictionary-fallback) string pages without a flat-store copy are not decoded on the GPU" +
+             (flat_ok ? std::string() : std::string(" (the flat kernels are switched off)")));
     // k_scan reads a page's raw values at 8 bytes: a Date32 column the query reads (slot s) is read from its widened
     // flat-store copy only.  An item without a flat-store copy of any of its columns goes to k_scan whole, so one such
     // item among the query's columns refuses a query that reads a Date32 column
